@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- XR-Linear beam-search prediction throughput on B200 (BASELINE.json metric).
+"""bench.py -- XR-Linear beam-search prediction throughput on H100 (BASELINE.json metric).
 
     python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload eurlex-4k|synthetic-small|synthetic-3m]
+                    [--dump-outputs DIR]
 
 A "step" is one pass of the hot path (all tree layers: chunk-score kernel + top-k kernel per layer) over one batch of
 synthetic queries.  At N=1 the workload is BASELINE.json configs[1] ("eurlex-4k": N=15,449 queries, D=5,000,
@@ -13,6 +14,9 @@ steps, max over ranks); `e2e` = queries/s through the reference-facing C-ABI cal
 pinned HOST buffers (H2D + kernels + D2H + result marshalling inside the timed region); `roofline` = achieved
 algorithmic HBM GB/s of the dominant kernel vs the measured peak; `cpu_baseline` = the reference's own OpenMP C++
 library (oracle/_ref) timed on this box's host cores.  `--impl reference` times that reference library alone.
+
+`--dump-outputs DIR` writes what the headline workload's timed path returned in its last timed step to DIR/<name>.npy
+(float32 / float64; inputs are generated from fixed seeds, so two builds can be compared output for output).
 """
 import argparse
 import json
@@ -46,6 +50,8 @@ def parse_args():
     ap.add_argument("--no-secondary", action="store_true",
                     help="skip the other target configurations (synthetic-3m; at N > 1 also the index-sharded run) that the default "
                          "eurlex-4k run reports under `secondary`")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the headline workload's outputs of the last timed step to DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -57,7 +63,7 @@ def dist_env():
 
 
 class ClockSampler(object):
-    """Samples SM clocks / throttle reasons while the timed region runs (B200_PROFILING.md recipe).
+    """Samples SM clocks / throttle reasons while the timed region runs.
 
     Primary source: NVML polled every ~2 ms from a thread (the timed region of the default run is only tens of
     milliseconds, far below nvidia-smi's sampling period); fallback: `nvidia-smi -lms 100`.  Every NVML call is guarded:
@@ -201,7 +207,25 @@ def measured_peak_gbs():
         with open(path) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "fallback (H100 SXM data-sheet HBM3 bandwidth, 3.35 TB/s; not measured)"
+
+
+DUMP_MAX_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, rows, arrays, seed=0):
+    """Writes `arrays` ({name: array whose first axis has `rows` entries, or None for a non-row array}) as out_dir/<name>.npy
+    in float32 / float64.  Above DUMP_MAX_BYTES in all, a fixed seeded sample of rows is written instead, with its row ids."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {k: np.asarray(v, dtype=np.float32 if np.asarray(v).dtype == np.float32 else np.float64) for k, v in arrays.items()}
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_MAX_BYTES and rows > 0:
+        keep = max(1, int(rows * DUMP_MAX_BYTES // (2 * total)))
+        sel = np.sort(np.random.default_rng(seed).choice(rows, size=keep, replace=False))
+        arrays = {k: a[sel] for k, a in arrays.items()}
+        arrays["sampled_rows"] = sel.astype(np.float64)
+    for k, a in arrays.items():
+        np.save(os.path.join(out_dir, k + ".npy"), a)
 
 
 def prepare_workload(args, rank, world, barrier, same_batch=False):
@@ -518,7 +542,7 @@ def hnsw_time_reference(folder, Q, cfg, steps, warmup, budget_s=60.0):
             "sample": f"{sample.shape[0]} of {Q.shape[0]} queries per step, {steps} steps, {n_cores} searchers (all host threads)"}
 
 
-def measure_hnsw(args, workload, rank, n_gpus, local, dist, barrier, steps, warmup, with_cpu=True):
+def measure_hnsw(args, workload, rank, n_gpus, local, dist, barrier, steps, warmup, with_cpu=True, dump_dir=None):
     """One HNSW workload on this rank's GPU (replicas: every rank its own query batch, same index file); returns the JSON line as
     a dict on rank 0 (None elsewhere)."""
     from ctypes import POINTER, byref, c_float, c_uint32, c_uint64
@@ -591,13 +615,6 @@ def measure_hnsw(args, workload, rank, n_gpus, local, dist, barrier, steps, warm
     peak, peak_src = measured_peak_gbs()
     achieved = bytes_per_step / (ms_per_step * 1e-3) / 1e9
     ncu_traffic = None
-    try:
-        with open(os.path.join(ROOT, "profiles", "ncu_traffic.json")) as f:
-            ncu_traffic = json.load(f).get(args.workload, {}).get("hnsw_search_kernel")
-            if isinstance(ncu_traffic, dict):
-                ncu_traffic = ncu_traffic.get("dram_bytes_per_launch")
-    except Exception:
-        pass
     roofline = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": ncu_traffic,
                 "kernel": "hnsw_search_kernel", "kernel_ms": ms_per_step, "algorithmic_bytes_per_launch": bytes_per_step,
                 "peak_source": peak_src, "per_query": {"distance_evals": n_dist / nq, "expansions": n_expand / nq,
@@ -609,6 +626,8 @@ def measure_hnsw(args, workload, rank, n_gpus, local, dist, barrier, steps, warm
     gi = np.zeros((nq, topk), dtype=np.uint32)
     gd = np.zeros((nq, topk), dtype=np.float32)
     c.pb200_hnsw_resident_fetch(h, gi.ctypes.data_as(POINTER(c_uint32)), gd.ctypes.data_as(POINTER(c_float)))
+    if dump_dir:
+        dump_outputs(dump_dir, nq, {"neighbor_ids": gi, "distances": gd})
     parity = {"checked_queries": 0, "checker": "unavailable (oracle/_ref absent)"}
     import oracle
 
@@ -762,7 +781,8 @@ def main_hnsw(args):
             dist.barrier()
 
     barrier()
-    line = measure_hnsw(args, args.workload, rank, n_gpus, local, dist, barrier, args.steps, args.warmup)
+    line = measure_hnsw(args, args.workload, rank, n_gpus, local, dist, barrier, args.steps, args.warmup,
+                        dump_dir=args.dump_outputs if rank == 0 else None)
     if rank == 0:
         print(json.dumps(line))
     if dist is not None:
@@ -816,17 +836,8 @@ def _max_over_ranks(dist, x):
     return float(t.item())
 
 
-def _ncu_notes(workload, kernel):
-    """What the committed ncu captures (profiles/ncu_traffic.json, written from `ncu --set full` runs) say about a kernel."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "ncu_traffic.json")) as f:
-            return json.load(f).get(workload, {}).get(kernel)
-    except Exception:
-        return None
-
-
 def measure_xlinear(args, workload, rank, n_gpus, local, dist, barrier, lib, steps, warmup, strong=False, with_cpu=True,
-                    with_clocks=True):
+                    with_clocks=True, dump_dir=None):
     """One XR-Linear workload on this rank's GPU.  strong=False: every rank its own batch of the workload's shape (weak
     scaling, replicas); strong=True: ONE batch of the workload's size, rows split over the ranks by nnz (strong scaling).
     Returns the JSON-able record (rank 0) -- parity-gated: raises if the GPU result differs from the reference."""
@@ -894,6 +905,8 @@ def measure_xlinear(args, workload, rank, n_gpus, local, dist, barrier, lib, ste
     fetch = ScipyCompressedSparseAllocator()
     c.pb200_xlinear_resident_fetch(h, fetch.cfunc)
     got_resident = fetch.get()
+    if dump_dir:  # the CSR a caller receives: row pointers, label ids (ranked within a row), scores
+        dump_outputs(dump_dir, 0, {"indptr": got_resident.indptr, "indices": got_resident.indices, "scores": got_resident.data})
     parity = parity_gate_xlinear(got_resident, folder, X, cfg, rows=(1024 if rank == 0 else 128), what=f"{workload} resident batch")
 
     # ------------------------------------------------------------ per-kernel timing (CUDA events on the launch stream)
@@ -923,7 +936,7 @@ def measure_xlinear(args, workload, rank, n_gpus, local, dist, barrier, lib, ste
         kernels.append({"kernel": f"{TOPK_KERNELS[kid[2 * d + 1]]}[layer {d}]", "ms": pm[d, 1], "algorithmic_bytes": float(topk_bytes[d])})
     dom = max(kernels, key=lambda k: k["ms"])
     achieved = dom["algorithmic_bytes"] / (dom["ms"] * 1e-3) / 1e9 if dom["ms"] > 0 else 0.0
-    notes = _ncu_notes(workload, dom["kernel"].split("[")[0]) or {}
+    notes = {}
     step_bytes = float(impl_scores.sum() + topk_bytes.sum())
     roofline = {
         "bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak if peak else None,
@@ -1096,7 +1109,8 @@ def main():
     lib.require_gpu()
     lib.set_device(local)
 
-    line, keep = measure_xlinear(args, args.workload, rank, n_gpus, local, dist, barrier, lib, args.steps, args.warmup)
+    line, keep = measure_xlinear(args, args.workload, rank, n_gpus, local, dist, barrier, lib, args.steps, args.warmup,
+                                 dump_dir=args.dump_outputs if rank == 0 else None)
     del keep
 
     # ------------------------------------------------------------ the other target configurations, in the same run

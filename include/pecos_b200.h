@@ -1,7 +1,7 @@
 /*
  * pecos_b200 C ABI  --  libpecos_b200_float32.so
  *
- * Drop-in replacement, on one NVIDIA B200 (sm_100a), for the two inference hot paths that the reference exports
+ * Drop-in replacement, on one NVIDIA H100 (sm_90a), for the two inference hot paths that the reference exports
  * from pecos/core/libpecos.cpp and binds through ctypes in pecos/core/base.py:
  *
  *   XR-Linear beam-search prediction   (libpecos.cpp:116-176,  base.py:799-976, :990-1095)
@@ -128,7 +128,7 @@ void c_mlmodel_predict_on_selected_outputs_drm_f32(void* ptr, const ScipyDrmF32*
  * reference).  The chunked HBM layout of (W, C, bias) is built on first use and kept in a small LRU cache keyed by the
  * matrices' shapes, value pointer and a sampled content fingerprint (PB200_LAYER_CACHE entries, default 8): the
  * matrices are assumed immutable while cached (pb200_layer_cache_clear() drops them).
- * Validated on a B200 (tests/test_single_layer_gpu.py); oracle pinned against the reference in tests/test_oracle_cpu.py. */
+ * Tested in tests/test_single_layer_gpu.py; oracle pinned against the reference in tests/test_oracle_cpu.py. */
 void c_xlinear_single_layer_predict_csr_f32(const ScipyCsrF32* input_x, const ScipyCsrF32* csr_codes, ScipyCscF32* W,
                                             ScipyCscF32* C, const char* post_processor_str, const uint32_t only_topk,
                                             const int num_threads, const float bias, py_sparse_allocator_t pred_alloc);
@@ -198,7 +198,7 @@ int pb200_get_device(void);
 /* Pinned host memory for end-to-end runs (cudaMallocHost / cudaFreeHost). */
 void* pb200_host_alloc(size_t bytes);
 void pb200_host_free(void* ptr);
-/* Overwrite a scratch buffer larger than L2 (126 MB) so the next timed iteration starts cold. */
+/* Overwrite a scratch buffer larger than L2 (50 MB on an H100) so the next timed iteration starts cold. */
 void pb200_l2_flush(void);
 
 /* Device-resident query batch: upload once, run the layers with inputs already in HBM, fetch when wanted. */

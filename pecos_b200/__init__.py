@@ -1,4 +1,4 @@
-"""pecos_b200 -- B200-native (sm_100a) inference engine for PECOS's two retrieval hot paths.
+"""pecos_b200 -- H100-native (sm_90a) inference engine for PECOS's two retrieval hot paths.
 
 * :class:`pecos_b200.xlinear.XLinearModel` -- XR-Linear beam-search prediction (``pecos.xmc.xlinear.XLinearModel`` API)
 * :class:`pecos_b200.hnsw.HNSW` -- HNSW dense search (``pecos.ann.hnsw.HNSW`` API)

@@ -1,4 +1,4 @@
-"""Builds ``pecos_b200/lib/libpecos_b200_float32.so`` in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Builds ``pecos_b200/lib/libpecos_b200_float32.so`` in-tree with nvcc for sm_90a (H100) (cross-compiles without a GPU)."""
 import glob
 import os
 import subprocess
@@ -10,7 +10,7 @@ LIB_DIR = os.path.join(HERE, "lib")
 LIB_PATH = os.path.join(LIB_DIR, "libpecos_b200_float32.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-lineinfo",
     "-O3",
     "-std=c++17",

@@ -1,4 +1,4 @@
-"""ctypes shim over ``libpecos_b200_float32.so`` -- the B200 counterpart of ``pecos.core.base.corelib``.
+"""ctypes shim over ``libpecos_b200_float32.so`` -- the GPU counterpart of ``pecos.core.base.corelib``.
 
 Mirrors, for the two hot paths only, the reference's Python-side FFI layer:
 

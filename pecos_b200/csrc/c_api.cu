@@ -636,7 +636,7 @@ void c_mlmodel_predict_on_selected_outputs_drm_f32(void* ptr, const ScipyDrmF32*
 }
 
 // ------------------------------------------------ additions ------------------------------------------------------
-const char* pb200_version(void) { return "pecos_b200 0.1 (sm_100a)"; }
+const char* pb200_version(void) { return "pecos_b200 0.1 (sm_90a)"; }
 
 int pb200_device_count(void) {
     int n = 0;
@@ -671,7 +671,7 @@ void pb200_l2_flush(void) {
     std::lock_guard<std::mutex> lock(g_flush_mutex);
     PB200_CUDA(cudaSetDevice(g_device.load()));
     if (!g_flush_buf) g_flush_buf = new pb200::DeviceBuffer<unsigned char>();
-    const uint64_t bytes = 512ull << 20;  // 4x the 126 MB L2
+    const uint64_t bytes = 512ull << 20;  // 10x the 50 MB L2 of an H100
     g_flush_buf->reserve(bytes);
     static int tick = 0;
     PB200_CUDA(cudaMemset(g_flush_buf->get(), (++tick) & 0xFF, bytes));

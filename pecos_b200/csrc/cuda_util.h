@@ -15,7 +15,7 @@ inline void cuda_check(cudaError_t err, const char* what, const char* file, int 
     if (err != cudaSuccess) {
         throw std::runtime_error(std::string("pecos_b200: CUDA error '") + cudaGetErrorString(err) + "' in " + what +
                                  " (" + file + ":" + std::to_string(line) +
-                                 "). This library has no CPU fallback: a working sm_100a GPU is required.");
+                                 "). This library has no CPU fallback: a working sm_90a (H100) GPU is required.");
     }
 }
 #define PB200_CUDA(call) ::pb200::cuda_check((call), #call, __FILE__, __LINE__)

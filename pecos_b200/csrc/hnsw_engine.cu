@@ -1,4 +1,4 @@
-// HNSW dense search on B200 (sm_100a): one warp walks one query (see hnsw_engine.h for the reference map).
+// HNSW dense search on H100 (sm_90a): one warp walks one query (see hnsw_engine.h for the reference map).
 //
 // Per expansion of the best-first search the warp
 //   A. reads the node's neighbour list, test-and-sets the per-warp visited bitmap, compacts the not-yet-visited ids in
@@ -699,7 +699,7 @@ void HnswEngine::ensure_scratch_(uint32_t ef) {
     while (warps > 1 && static_cast<uint64_t>(warps) * per_warp > 96u * 1024u) warps >>= 1;
     if (static_cast<uint64_t>(warps) * per_warp > 200u * 1024u)
         throw std::runtime_error("pecos_b200: HNSW query dimension too large for the shared-memory staging area");
-    int sms = 148;
+    int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device_);
     const uint32_t ctas_per_sm = std::max<uint32_t>(1, std::min<uint32_t>((H.sparse ? 32u : 16u) / warps, static_cast<uint32_t>((220u * 1024u) / (static_cast<uint64_t>(warps) * per_warp))));
     uint32_t n_ctas = static_cast<uint32_t>(sms) * ctas_per_sm;

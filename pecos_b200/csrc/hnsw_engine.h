@@ -1,4 +1,4 @@
-// HNSW dense search engine on one B200.
+// HNSW dense search engine on one H100.
 //
 // Replaces (reference, CPU/OpenMP, one Searcher per thread):
 //   c_ann_hnsw_predict_* ............. pecos/core/libpecos.cpp:527-564

@@ -3,7 +3,7 @@
 //
 // Included by xlinear_engine.cu (inside its anonymous namespace, after the small device helpers).
 //
-// Why (profiles/r02_*): the query-major kernels spend 600 - 3,900 warp-instructions per pair on match compaction, prefix
+// Why: the query-major kernels spend 600 - 3,900 warp-instructions per pair on match compaction, prefix
 // sums and on putting colliding entries of a 32-entry group back into feature order, and every probe / extent / entry
 // access is a scattered global load (one L1 line each).  Here
 //   * at LOAD time every chunk of an eligible layer is packed into a self-contained IMAGE in HBM (xl_cm_build_images_kernel):
@@ -32,9 +32,9 @@ constexpr int kCmFeat = 8;                  // query features staged per pair an
 constexpr int kCmMaxWarps = 16;
 constexpr int kCmMinWarps = 4;
 constexpr uint32_t kCmMaxDup = 400;         // a column cap may at most quadruple the (virtual) chunks of a layer
-constexpr uint32_t kCmSmemBudget = 224u << 10;  // dynamic shared memory a CTA may take (227 KB is the sm_100a maximum)
+constexpr uint32_t kCmSmemBudget = 224u << 10;  // dynamic shared memory a CTA may take (227 KB is the sm_90a maximum)
 constexpr uint32_t kCmMinReuse = 24;        // average pairs per chunk below which the per-chunk staging does not pay
-constexpr uint32_t kCmMinPairs = 148u * 48u; // fewer pairs than this: the query-major kernels fill the GPU better
+constexpr uint32_t kCmMinPairsPerSm = 48u;  // fewer pairs than this per SM: the query-major kernels fill the GPU better
 constexpr uint32_t kCmDirectRows = 16384;   // feature spaces up to this size get a direct feature -> entry-range table
 constexpr uint32_t kCmEmpty = 0xFFFFFFFFu;
 
@@ -64,7 +64,7 @@ __host__ __device__ inline size_t cm_warp_bytes(uint32_t acc_cols, uint32_t stag
 // col_cap: a chunk wider than col_cap columns is cut into ceil(n_cols / col_cap) column ranges of (nearly) equal width, each
 // with its OWN image (only its entries) -- a "virtual chunk"; a (query, chunk) pair is then scored once per range.  The lookups
 // are repeated for the cut chunks, the accumulate work is not, and both the image and the per-warp accumulators shrink to the
-// cap, so more warps fit (occupancy is what the kernel is short of on wide chunks: profiles/r02_e, r02_i).  The cap is chosen
+// cap, so more warps fit (occupancy is what the kernel is short of on wide chunks).  The cap is chosen
 // at load so that only the few widest chunks of a layer are cut (cm_choose_cap).  e_max = most entries of one virtual chunk,
 // n_vc = number of virtual chunks.
 inline CmShape cm_shape(uint32_t fm_words, uint32_t w_rows, uint32_t r_max, uint32_t e_max, uint32_t col_cap, uint32_t n_chunks,
@@ -98,12 +98,12 @@ inline CmShape cm_shape(uint32_t fm_words, uint32_t w_rows, uint32_t r_max, uint
 inline CmPlan cm_plan(const CmShape& s, uint32_t n_chunks, uint64_t pairs, uint32_t n_sm, bool force) {
     CmPlan p;
     if (!s.ok || pairs == 0) return p;
-    // measured (profiles/r02_d, r02_e): with the 94 KB feature-map image of a large feature space the kernel does not beat the
-    // query-major kernels (S layers 1-4: 2.0 / 2.4 / 6.3 ms vs 1.9 / 1.9 / 2.0 ms) -- only direct-table layers take it by default
+    // with the 94 KB feature-map image of a large feature space the kernel does not beat the query-major kernels (S layers
+    // 1-4) -- only direct-table layers take it by default
     if (!force && !s.direct) return p;
     pairs = pairs * s.n_vc / std::max<uint32_t>(n_chunks, 1u);  // cut chunks are visited once per column range
     n_chunks = s.n_vc;
-    if (!force && (pairs < static_cast<uint64_t>(kCmMinReuse) * n_chunks || pairs < kCmMinPairs)) return p;
+    if (!force && (pairs < static_cast<uint64_t>(kCmMinReuse) * n_chunks || pairs < static_cast<uint64_t>(kCmMinPairsPerSm) * n_sm)) return p;
     const size_t per_warp = cm_warp_bytes(s.acc_cols, s.stages);
     uint32_t warps = static_cast<uint32_t>(std::min<size_t>(kCmMaxWarps, (kCmSmemBudget - s.img_bytes - 64) / per_warp));
     // no point in more lanes than a CTA's share of the pair list holds
@@ -573,7 +573,7 @@ constexpr int kCmgStages = 3;
 inline CmgPlan cmg_plan(uint32_t c_max, uint32_t e_max, uint32_t n_chunks, uint64_t pairs, uint32_t n_sm, bool force) {
     CmgPlan p;
     if (c_max == 0 || c_max > 256u || e_max >= 65535u || pairs == 0 || n_chunks == 0) return p;
-    if (!force && pairs < kCmMinPairs) return p;
+    if (!force && pairs < static_cast<uint64_t>(kCmMinPairsPerSm) * n_sm) return p;
     const size_t per_warp = cm_warp_bytes(c_max, kCmgStages);
     uint32_t warps = static_cast<uint32_t>(std::min<size_t>(kCmMaxWarps, (kCmSmemBudget - 64) / per_warp));
     if (warps < 2) return p;

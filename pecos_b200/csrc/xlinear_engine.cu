@@ -1,4 +1,4 @@
-// XR-Linear beam search on B200 (sm_100a): kernels + engine.  See xlinear_engine.h for the reference map.
+// XR-Linear beam search on H100 (sm_90a): kernels + engine.  See xlinear_engine.h for the reference map.
 //
 // Per tree layer two kernels run over a tile of queries:
 //
@@ -1007,7 +1007,7 @@ XLinearEngine::XLinearEngine(std::unique_ptr<XLinearHostModel> host, int device)
             dst.e_max = std::max(dst.e_max, rp[ch.nnz_rows]);
         }
         dst.rowext.reserve(std::max<uint64_t>(src.meta.size(), 4));
-        xl_build_rowext_kernel<<<148 * 8, 256, 0, stream_>>>(dst.chunks.get(), dst.meta.get(), dst.rowext.get(), src.n_chunks);
+        xl_build_rowext_kernel<<<n_sm_ * 8, 256, 0, stream_>>>(dst.chunks.get(), dst.meta.get(), dst.rowext.get(), src.n_chunks);
         PB200_CUDA(cudaGetLastError());
         model_bytes_ += src.meta.size() * 4;
         dst.view.chunks = dst.chunks.get();
@@ -1047,10 +1047,9 @@ XLinearEngine::XLinearEngine(std::unique_ptr<XLinearHostModel> host, int device)
                 if (e_max_out) *e_max_out = best;
                 return n_vc;
             };
-            // Policy (measured, eurlex-4k leaf: chunks of 62 +- 8 columns, widest 85): uncut 6 warps 0.78 ms; cap 64 (a third of
-            // the chunks cut) 10 warps 0.94 ms; every chunk in two ranges 14 warps 1.04 ms -- more warps raise the issue rate
-            // (32 -> 43 %) but the repeated lookups (+21 % instructions) and the uneven cost of cut / uncut pairs inside the
-            // equal-count CTA shares cost more.  So: the LARGEST cap that fits at all (no cut whenever the layer fits uncut).
+            // Policy: cutting more chunks gives more warps per CTA (a higher issue rate), but the repeated lookups and the
+            // uneven cost of cut / uncut pairs inside the equal-count CTA shares cost more on the eurlex-4k leaf (chunks of
+            // 62 +- 8 columns).  So: the LARGEST cap that fits at all (no cut whenever the layer fits uncut).
             CmShape shape;
             const uint32_t n_real = layout_for_cap(std::max<uint32_t>(src.c_max, 1u), nullptr, nullptr);
             for (uint32_t cap = std::max<uint32_t>(src.c_max, 1u); n_real > 0; cap = cap * 7 / 8) {
@@ -1242,10 +1241,9 @@ int XLinearEngine::score_layer_(size_t d, const QueryDev& q, uint32_t b_prev, in
         kernel<<<grid, block, smem1, stream_>>>(L, q, bid_(cur), bcnt_(cur), beam_stride_, cand_at_(cand_stride_q),
                                                cand_stride_q, c_stride, stats, q_cap, sb_cap, hdr_cap);
     };
-    // One warp per query over the whole beam (feature-major).  Measured on B200: it wins when the beam consists of
-    // MANY NARROW chunks (per-chunk bookkeeping dominates: S layers 1-4, 20 x 8 columns: 2.1-2.9 ms vs 3.1 ms), and
-    // loses on wide chunks where one warp per chunk keeps more loads in flight (E leaf 2.2 vs 1.45 ms, S leaf 12.7 vs
-    // 8.4 ms).  force_query_warp_ (kernel mode 3) selects it whenever it is eligible, for tests.
+    // One warp per query over the whole beam (feature-major).  It wins when the beam consists of MANY NARROW chunks
+    // (per-chunk bookkeeping dominates: S layers 1-4, 20 x 8 columns), and loses on wide chunks where one warp per chunk
+    // keeps more loads in flight (E and S leaves).  force_query_warp_ (kernel mode 3) selects it whenever it is eligible, for tests.
     const bool qw_eligible = lookup && b_prev <= static_cast<uint32_t>(kQwSlots) &&
                              cand_stride_q <= static_cast<uint64_t>(kQwNCap) && q.max_row_nnz <= kQwQCap;
     const bool query_warp = qw_eligible && !no_query_warp_ &&
@@ -1259,9 +1257,9 @@ int XLinearEngine::score_layer_(size_t d, const QueryDev& q, uint32_t b_prev, in
                           : CmPlan{};
     const bool chunk_major = cm.eligible;
     // the same lane-per-pair walk without a staged image (xl_cmg_scores_kernel) where the image variant does not apply: layers
-    // of large feature spaces / chunks visited by few pairs.  OPT-IN (kernel modes 8-10): bit-exact but measured slower than the
-    // query-major kernels on the 3M-label model (leaf 16.4 vs 5.4 ms: 92 registers + 224 KB keep 12 warps per SM, every lookup a
-    // dependent global load; profiles/r02_l_ncu_cmg.txt).  Mode 9: in place of the feature-map chunk kernel; 8: also of the
+    // of large feature spaces / chunks visited by few pairs.  OPT-IN (kernel modes 8-10): bit-exact but slower than the
+    // query-major kernels on the 3M-label leaf (92 registers + 224 KB keep 12 warps per SM, every lookup a dependent global
+    // load).  Mode 9: in place of the feature-map chunk kernel; 8: also of the
     // query-warp kernel.
     const CmgPlan cmg = (chunk_major_ && cmg_ && lookup && !collect_stats && !chunk_major && cm_offsets_fit && cm_slot_pos_.capacity() &&
                          (cmg_all_ || !query_warp))

@@ -1,4 +1,4 @@
-// XR-Linear beam-search engine on one B200: device-resident model + the two kernels per tree layer.
+// XR-Linear beam-search engine on one H100: device-resident model + the two kernels per tree layer.
 //
 // Replaces (reference, CPU/OpenMP):
 //   HierarchicalMLModel::predict ........ pecos/core/xmc/inference.hpp:2446-2488
@@ -253,10 +253,10 @@ private:
     bool no_topk_filter_ = false;
     bool chunk_major_ = true;   // chunk-major scoring wherever cm_plan() finds it eligible (kernel mode 6 switches it off)
     bool cm_force_ = false;     // kernel mode 5
-    bool cmg_ = false;          // image-less lane-per-pair kernel: opt-in (kernel modes 8, 9, 10); measured slower, DESIGN.md 3.3
+    bool cmg_ = false;          // image-less lane-per-pair kernel: opt-in (kernel modes 8, 9, 10); slower on the 3M-label model, DESIGN.md 3.3
     bool cmg_all_ = false;      // kernel modes 8, 10
     bool cm_image_ = true;      // staged-image chunk-major kernel (kernel mode 10 switches it off)
-    uint32_t n_sm_ = 148;
+    uint32_t n_sm_ = 132;
     DeviceBuffer<uint32_t> cm_slot_pos_, cm_count_, cm_bucket_ptr_, cm_item_ptr_, cm_pair_q_, cm_pair_pos_;
     bool force_block_topk_ = false;  // A/B switch: first-generation kernels (row-list streaming + block-wide sort)
     std::vector<XLinearLayerProfile> layer_profile_;

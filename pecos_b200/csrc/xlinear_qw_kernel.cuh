@@ -147,7 +147,7 @@ xl_query_warp_scores_kernel(const LayerDev L, const QueryDev X, const uint32_t* 
                 x[u] = 0.0f;
                 if (g < total) {
                     // independent binary searches: this kernel is latency-bound (32 warps/SM), and the serial row-start
-                    // mask chain of xl_rows_of_group measured slower here (S layers 2-4: 2.2 vs 1.9 ms)
+                    // mask chain of xl_rows_of_group slower here (S layers 2-4)
                     const int i = last_le_u32(off, m, g);  // off[i] <= g < off[i + 1]
                     e[u] = __ldg(ment[i] + (g - off[i]));
                     e[u].x += mb[i];

@@ -1,4 +1,4 @@
-"""``HNSW`` -- search-only B200 counterpart of ``pecos.ann.hnsw.HNSW``.
+"""``HNSW`` -- search-only GPU counterpart of ``pecos.ann.hnsw.HNSW``.
 
 The class keeps the reference's public surface for the load / search path, so code written against
 ``pecos.ann.hnsw.HNSW`` (pecos/ann/hnsw/model.py) runs unchanged:

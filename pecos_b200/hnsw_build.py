@@ -11,7 +11,7 @@ dependent graph of the incremental algorithm (the reference itself is nondetermi
 SEARCH on the saved file is bit-level: the reference and the CUDA engine return identical ids / distance bits on it
 (tests/test_hnsw_build_gpu.py).
 
-Algorithm (B200-first: the distance work is dense GEMMs on the tensor cores, cuBLAS through torch -- a plain library GEMM --
+Algorithm (GPU-first: the distance work is dense GEMMs on the tensor cores, cuBLAS through torch -- a plain library GEMM --
 instead of 10^9 dependent single-vector distance calls):
 
 1. node levels as the reference draws them: ``floor(-ln(U) / ln(M))`` (hnsw.hpp:785-793), entry point = first node of the top level;

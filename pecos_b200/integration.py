@@ -1,4 +1,4 @@
-"""Overlay the B200 hot-path symbols onto a live ``pecos.core.clib`` (see INTEGRATION.md section 2).
+"""Overlay the GPU hot-path symbols onto a live ``pecos.core.clib`` (see INTEGRATION.md section 2).
 
 ``overlay(clib)`` re-points the XR-Linear predict-only and HNSW (dense and sparse) search function pointers of the reference's
 ``corelib`` instance (pecos/core/base.py:481-539, :1951-1964) at ``libpecos_b200_float32.so``; every other symbol keeps

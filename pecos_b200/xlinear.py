@@ -1,4 +1,4 @@
-"""``XLinearModel`` -- predict-only mirror of ``pecos.xmc.xlinear.XLinearModel`` running on a B200.
+"""``XLinearModel`` -- predict-only mirror of ``pecos.xmc.xlinear.XLinearModel`` running on an H100.
 
 Same names, argument meaning and error behaviour as the reference for the prediction path:
 

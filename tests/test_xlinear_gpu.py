@@ -176,14 +176,17 @@ def test_two_layer_wide_beam_streaming_topk(tmp_path, gpu_clib, have_ref):
 
 
 def test_mmap_model_equals_npz_model(tmp_path, gpu_clib, have_ref, small_model):
-    if not have_ref:
-        pytest.fail("oracle/_ref did not travel to this box; compiling an mmap model needs the reference's c_xlinear_compile_mmap_model")
+    """The mmap folder is written by the reference's c_xlinear_compile_mmap_model where oracle/_ref is built, else by this
+    library's own (interchangeable with the reference's: tests/test_host_cpu.py, tests/golden/xlinear_toy/model_mmap)."""
     from oracle import ref
 
     folder, X, m, oracles = small_model
     mm_dir = str(tmp_path / "mmap_model")
     os.makedirs(mm_dir)
-    ref.compile_mmap_model(os.path.join(folder, "ranker"), os.path.join(mm_dir, "ranker"))
+    if have_ref:
+        ref.compile_mmap_model(os.path.join(folder, "ranker"), os.path.join(mm_dir, "ranker"))
+    else:
+        gpu_clib.clib_float32.c_xlinear_compile_mmap_model(os.path.join(folder, "ranker").encode(), os.path.join(mm_dir, "ranker").encode())
     mm = _load(mm_dir)
     a = m.predict(X, beam_size=5, only_topk=5)
     b = mm.predict(X, beam_size=5, only_topk=5)

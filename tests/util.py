@@ -91,3 +91,63 @@ def reachable_labels(layers):
         C = smat.csr_matrix(C)
         reach = np.asarray((C.astype(np.float32) @ reach.astype(np.float32)) > 0).ravel()
     return np.nonzero(reach)[0]
+
+
+class RecordedReference(object):
+    """Reference-library results that a test compares against, kept under tests/golden/ref_outputs/<name>.npz so that the
+    comparison also runs where the reference library (oracle/_ref) is not built.
+
+    With oracle/_ref present, `check` computes the reference result and compares in full (assert_csr_parity); with
+    PB200_RECORD_REF_OUTPUTS=1 it also records it.  Without oracle/_ref it compares with the record: row sizes and label ids
+    through a SHA-256 of the reference's (indptr, indices), scores at a fixed seeded sample of entries (`sample` per result)
+    within the same relative tolerance.  The inputs of every recorded call are generated from fixed seeds by the test."""
+
+    DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "ref_outputs")
+
+    def __init__(self, name, have_ref, sample=32):
+        self.path = os.path.join(self.DIR, name + ".npz")
+        self.live = bool(have_ref)
+        self.record = self.live and os.environ.get("PB200_RECORD_REF_OUTPUTS") == "1"
+        self.sample = sample
+        self.store = {} if self.live else dict(np.load(self.path))
+        self.used = set()
+
+    @staticmethod
+    def _pattern_digest(M):
+        import hashlib
+
+        h = hashlib.sha256()
+        h.update(np.asarray(M.shape, dtype=np.int64).tobytes())
+        h.update(np.asarray(M.indptr, dtype=np.int64).tobytes())
+        h.update(np.asarray(M.indices, dtype=np.int64).tobytes())
+        return np.frombuffer(h.digest(), dtype=np.uint8)
+
+    def _positions(self, key, nnz):
+        import zlib
+
+        rng = np.random.default_rng(zlib.crc32(key.encode()))
+        return np.sort(rng.choice(nnz, size=min(nnz, self.sample), replace=False)) if nnz else np.zeros(0, dtype=np.int64)
+
+    def check(self, key, got, compute, rtol=1e-5, what=""):
+        assert key not in self.used, f"duplicate key {key}"
+        self.used.add(key)
+        if self.live:
+            want = compute()
+            assert_csr_parity(got, want, rtol=rtol, what=what)
+            if self.record:
+                self.store[key + "|pattern"] = self._pattern_digest(want)
+                self.store[key + "|values"] = np.asarray(want.data, dtype=np.float32)[self._positions(key, want.nnz)]
+            return
+        assert np.array_equal(self._pattern_digest(got), self.store[key + "|pattern"]), f"{what}: row sizes / label ids differ from the recorded reference"
+        wd = self.store[key + "|values"]
+        gd = np.asarray(got.data, dtype=np.float32)[self._positions(key, got.nnz)]
+        rel = np.abs(gd.astype(np.float64) - wd.astype(np.float64)) / np.maximum(np.abs(wd), np.finfo(np.float32).tiny)
+        assert rel.size == 0 or rel.max() <= rtol, f"{what}: max relative score error {rel.max():.3e} > {rtol} vs the recorded reference"
+
+    def close(self):
+        """Writes the record (recording runs only); a test must check every recorded result."""
+        if self.record:
+            os.makedirs(self.DIR, exist_ok=True)
+            np.savez_compressed(self.path, **self.store)
+        elif not self.live:
+            assert {k.rsplit("|", 1)[0] for k in self.store} == self.used, "recorded reference results left unchecked"
