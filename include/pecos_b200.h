@@ -297,6 +297,27 @@ int pb200_hnsw_host_info(const char* model_dir, int metric, int sparse, uint64_t
  * the batch with twice the capacity (up to num_node + 1, which cannot overflow) -- this counts those re-runs. */
 uint32_t pb200_hnsw_vcap_retries(void* model_ptr);
 
+/* ============================================= index construction =============================================== */
+
+/* Distance kernels of the sparse (csr) HNSW builder (pecos_b200/hnsw_build.py).  Every argument is a DEVICE pointer on
+ * `device` (torch tensors' data_ptr()), work is enqueued on `stream` (a cudaStream_t, NULL = the legacy default stream) and
+ * the call returns without synchronising; the caller's current device is left as it was.  metric 0 = ip, 1 = l2.
+ * Base rows: row r = entries [row_ptr[r], row_ptr[r+1]) (u64) of ent, 8 bytes each {u32 index, f32 value}, indices strictly
+ * ascending.  Each returned distance is bit-identical to the reference's FeatVecSparse{IP,L2}Simd::distance of the two rows
+ * (ip: 1 - <x,y>; l2: -2<x,y>, see above).  work (may be NULL): a device u64 that is increased by the postings walked
+ * (block) or the row entries walked by the intersections (candidate sets). */
+
+/* Prefix-kNN blocks.  The candidate set is given by its inverted index: column f = postings [col_ptr[f], col_ptr[f+1]) (u64)
+ * of post, 8 bytes each {u32 position in the candidate set, f32 value}, positions ascending within a column.
+ * out (f32 [nq, nc]): out[q * nc + (p - c0)] = distance(row q_ids[q] (i64), candidate at position p), p in [c0, c0 + nc). */
+void pb200_sparse_block_distances(int device, int metric, const void* row_ptr, const void* ent, const void* q_ids, uint32_t nq,
+                                  const void* col_ptr, const void* post, uint32_t c0, uint32_t nc, void* out, void* work,
+                                  void* stream);
+/* Selection-heuristic candidate sets.  cand (i64 [n, C], C <= 512): row ids, -1 = empty slot.
+ * out (f32 [n, C, C]): out[t, i, j] = distance(cand[t, i], cand[t, j]); +inf where either slot is empty. */
+void pb200_sparse_candidate_distances(int device, int metric, const void* row_ptr, const void* ent, const void* cand, uint32_t n,
+                                      uint32_t C, void* out, void* work, void* stream);
+
 /* Host-only model ingest (no GPU needed): loads + builds the chunk layout, for layout tests.
  *   kind: 0 = npz folder, 1 = mmap folder.  dims out[8] = {w_rows, n_cols, out_cols, n_chunks, c_max, meta_len,
  *   n_entries, label_of_col_len}.  export copies the arrays into caller buffers (any may be NULL). */

@@ -15,6 +15,7 @@
 #include <unordered_set>
 #include <vector>
 
+#include "hnsw_build_sparse.h"
 #include "hnsw_engine.h"
 #include "xlinear_engine.h"
 
@@ -677,6 +678,27 @@ void pb200_l2_flush(void) {
     PB200_CUDA(cudaMemset(g_flush_buf->get(), (++tick) & 0xFF, bytes));
     PB200_CUDA(cudaDeviceSynchronize());
     PB200_API_END("pb200_l2_flush")
+}
+
+// ------------------------------------------------ index construction (sparse HNSW builder) ----------------------------
+void pb200_sparse_block_distances(int device, int metric, const void* row_ptr, const void* ent, const void* q_ids, uint32_t nq,
+                                  const void* col_ptr, const void* post, uint32_t c0, uint32_t nc, void* out, void* work,
+                                  void* stream) {
+    PB200_API_BEGIN
+    pb200::sparse_block_distances(device, metric, static_cast<const uint64_t*>(row_ptr), static_cast<const uint2*>(ent),
+                                  static_cast<const int64_t*>(q_ids), nq, static_cast<const uint64_t*>(col_ptr),
+                                  static_cast<const uint2*>(post), c0, nc, static_cast<float*>(out),
+                                  static_cast<unsigned long long*>(work), static_cast<cudaStream_t>(stream));
+    PB200_API_END("pb200_sparse_block_distances")
+}
+
+void pb200_sparse_candidate_distances(int device, int metric, const void* row_ptr, const void* ent, const void* cand, uint32_t n,
+                                      uint32_t C, void* out, void* work, void* stream) {
+    PB200_API_BEGIN
+    pb200::sparse_candidate_distances(device, metric, static_cast<const uint64_t*>(row_ptr), static_cast<const uint2*>(ent),
+                                      static_cast<const int64_t*>(cand), n, C, static_cast<float*>(out),
+                                      static_cast<unsigned long long*>(work), static_cast<cudaStream_t>(stream));
+    PB200_API_END("pb200_sparse_candidate_distances")
 }
 
 void pb200_xlinear_resident_upload_csr(void* ptr, const ScipyCsrF32* X) {

@@ -20,6 +20,7 @@
 //
 // HBM traffic per query (SURVEY 8d): n_dist * 4d + n_expand * 4(1+maxM0) + hops * 4(1+maxM) + 4d + 8k.
 #include "hnsw_engine.h"
+#include "sparse_distance.cuh"
 
 #include <algorithm>
 #include <atomic>
@@ -244,11 +245,7 @@ __device__ __forceinline__ void batch_distances_sparse(const HnswDev& ix, const 
                 if (j0 + 16u * u < len_max) ret = sparse_step(q, has[u], e[u], ret, lane);
             }
         }
-        if (hl == 0 && valid) {
-            // FeatVecSparseIPSimd: 1.0 - dot ; FeatVecSparseL2Simd: x_sq + y_sq - 2.0 * dot with x_sq = y_sq = 0 (see the header)
-            dist[slot] = (METRIC == HNSW_IP) ? static_cast<float>(1.0 - static_cast<double>(ret))
-                                             : static_cast<float>(static_cast<double>(0.0f) - 2.0 * static_cast<double>(ret));
-        }
+        if (hl == 0 && valid) dist[slot] = sparse_finalize<METRIC>(ret);
     }
     __syncwarp();
 }

@@ -12,8 +12,8 @@ ret_csr=True)``                                ``(indices, distances)`` arrays
 ``HNSW.searchers_create(n)`` / ``Searchers``   opaque scratch token (the per-warp scratch lives with the engine)
 =============================================  =======================================================
 
-Index construction stays on the reference CPU library (dense indices can also be built on the GPU:
-``pecos_b200.hnsw_build``).  Served index kinds: dense ``drm`` and sparse ``csr`` float32 with the ``ip`` or ``l2`` metric
+Index construction: ``pecos_b200.hnsw_build.build_hnsw_index`` builds dense and sparse indices on the GPU in the reference's
+format; the reference CPU library's ``HNSW.train`` remains usable, its indices load here unchanged.  Served index kinds: dense ``drm`` and sparse ``csr`` float32 with the ``ip`` or ``l2`` metric
 (csr rows: column indices strictly ascending -- queries are canonicalised with ``sum_duplicates()`` / ``sort_indices()``
 when needed).  There is no CPU fallback: loading without a visible CUDA device raises ``RuntimeError``.
 """
