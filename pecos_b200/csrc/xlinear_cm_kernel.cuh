@@ -13,14 +13,16 @@
 //     and 16-bit row pointers;
 //   * per call the pairs are bucketed by chunk on the device (count -> scan -> scatter; the reference's b_sort_by_chunk,
 //     pecos/core/xmc/inference.hpp:985-993);
-//   * the score kernel is PERSISTENT: one CTA per SM takes a contiguous 1/grid share of the chunk-sorted pair list, so it
-//     meets only a few chunks; a chunk's image arrives by ONE bulk asynchronous copy (cp.async.bulk + mbarrier, the TMA
-//     engine's non-tensor form) and serves every pair of the run; warps take 32-pair slices of the run;
+//   * the score kernel is PERSISTENT: one CTA per SM takes a contiguous share of the chunk-sorted pair list holding 1/grid
+//     of the estimated work (a pair's cost grows with its chunk's entry count: cm_pair_cost), so it meets only a few chunks
+//     and no CTA is left with the widest chunks' pairs; a chunk's image arrives by ONE bulk asynchronous copy
+//     (cp.async.bulk + mbarrier, the TMA engine's non-tensor form) and serves every pair of the run; warps take 32-pair
+//     slices of the run;
 //   * a lane walks its pair's query features in ascending order (staged global -> shared by cp.async, two rounds of 8 in
-//     flight), compacts the hits of a round in place as {entry range, x}, then streams the hit rows' entries -- ONE entry
-//     per iteration, warp-uniform trip count, so rows of different lengths do not serialise -- into the lane's PRIVATE
-//     accumulators acc[column][lane].  That is the reference's marching loop (inference.hpp:788-811): ascending feature
-//     order, separate multiply and add, bias row last; the order is right by construction and a column is only ever
+//     flight), compacts the hits of a round in place as {entry range, x}, then streams the hit rows' entries as one flat
+//     stream, kCmSlots entries per iteration across row boundaries (the warp's trip count follows the lane with the most
+//     entries), into the lane's PRIVATE accumulators acc[column][lane].  That is the reference's marching loop
+//     (inference.hpp:788-811): ascending feature order, separate multiply and add, bias row last; a column is only ever
 //     touched by the lane that owns the pair: no compaction across lanes, no conflict resolution.
 //
 // Bit-identical to the query-major kernels (tests/test_chunk_major_gpu.py).  Eligibility: shape (cm_shape, at load: width
@@ -29,6 +31,7 @@
 #pragma once
 
 constexpr int kCmFeat = 8;                  // query features staged per pair and round (two rounds in flight per warp)
+constexpr int kCmSlots = 4;                 // entries a lane adds per iteration of the accumulate phase
 constexpr int kCmMaxWarps = 16;
 constexpr int kCmMinWarps = 4;
 constexpr uint32_t kCmMaxDup = 400;         // a column cap may at most quadruple the (virtual) chunks of a layer
@@ -42,10 +45,9 @@ struct CmWork {
     uint32_t* slot_pos;     // [rows x beam_stride] first candidate position of every beam slot
     uint32_t* count;        // [n_chunks] pairs per chunk, reused as the scatter cursor
     uint32_t* bucket_ptr;   // [n_chunks + 1]
-    uint32_t* item_ptr;     // [n_chunks + 1] (unused by the persistent score kernel; kept by the scan)
+    uint64_t* cost_ptr;     // [n_chunks + 1] exclusive prefix of the chunks' estimated work (cm_pair_cost x pairs)
     uint32_t* pair_q;       // [pairs] query of a pair, grouped by chunk
     uint32_t* pair_pos;     // [pairs] candidate position of the pair's first column inside the query's row
-    uint32_t item_pairs;
 };
 
 struct CmPlan {  // per call
@@ -64,8 +66,8 @@ __host__ __device__ inline size_t cm_warp_bytes(uint32_t acc_cols, uint32_t stag
 // col_cap: a chunk wider than col_cap columns is cut into ceil(n_cols / col_cap) column ranges of (nearly) equal width, each
 // with its OWN image (only its entries) -- a "virtual chunk"; a (query, chunk) pair is then scored once per range.  The lookups
 // are repeated for the cut chunks, the accumulate work is not, and both the image and the per-warp accumulators shrink to the
-// cap, so more warps fit (occupancy is what the kernel is short of on wide chunks).  The cap is chosen
-// at load so that only the few widest chunks of a layer are cut (cm_choose_cap).  e_max = most entries of one virtual chunk,
+// cap, so more warps fit.  The load path takes the largest cap that fits (see the policy note in xlinear_engine.cu): a layer
+// is only cut when its widest chunk does not fit next to kCmMinWarps warps.  e_max = most entries of one virtual chunk,
 // n_vc = number of virtual chunks.
 inline CmShape cm_shape(uint32_t fm_words, uint32_t w_rows, uint32_t r_max, uint32_t e_max, uint32_t col_cap, uint32_t n_chunks,
                         uint32_t n_vc) {
@@ -274,41 +276,63 @@ xl_cm_count_kernel(const LayerDev L, const QueryDev X, const uint32_t* __restric
     }
 }
 
-// single CTA: exclusive scans of the pair counts (bucket offsets) and of the work items per chunk; count[] becomes the
-// scatter cursor
+// Estimated work of one pair of a (virtual) chunk with E entries in a feature space of D rows: a pair looks up each of its
+// query's features (about nnz shared-memory lookups) and adds the entries of the rows it hits (about nnz x E / D), so its
+// cost is proportional to D + E -- one lookup weighs about as much as one entry (both are a few scattered shared-memory
+// accesses).  The accumulate phase dominates on wide chunks, so pairs of an 84-column chunk cost ~1.3x those of a 62-column one.
+__device__ __forceinline__ uint32_t cm_pair_cost(uint32_t w_rows, uint32_t entries) { return w_rows + entries; }
+
+__device__ __forceinline__ uint64_t warp_incl_scan64(uint64_t v, int lane) {
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+        const uint64_t t = __shfl_up_sync(kFull, v, d);
+        if (lane >= d) v += t;
+    }
+    return v;
+}
+
+// single CTA: exclusive scans of the pair counts (bucket offsets) and of the chunks' estimated work (cost_ptr; images ==
+// nullptr: one unit per pair); count[] becomes the scatter cursor.  A chunk's entry count is read from its image header.
 __global__ void __launch_bounds__(1024)
-xl_cm_scan_kernel(const uint32_t n_chunks, CmWork w) {
-    __shared__ uint32_t s_pairs[32], s_items[32];
-    __shared__ uint32_t carry_pairs, carry_items;
+xl_cm_scan_kernel(const uint32_t n_chunks, CmWork w, const unsigned char* __restrict__ images, const uint32_t img_bytes,
+                  const uint32_t w_rows) {
+    __shared__ uint32_t s_pairs[32];
+    __shared__ uint64_t s_cost[32];
+    __shared__ uint32_t carry_pairs;
+    __shared__ uint64_t carry_cost;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (threadIdx.x == 0) { carry_pairs = 0; carry_items = 0; }
+    if (threadIdx.x == 0) { carry_pairs = 0; carry_cost = 0; }
     __syncthreads();
     for (uint32_t c0 = 0; c0 < n_chunks; c0 += 1024) {
         const uint32_t c = c0 + threadIdx.x;
         const uint32_t n = (c < n_chunks) ? w.count[c] : 0u;
-        const uint32_t it = (n + w.item_pairs - 1) / w.item_pairs;
-        const uint32_t in_p = warp_incl_scan(n, lane), in_i = warp_incl_scan(it, lane);
-        if (lane == 31) { s_pairs[warp] = in_p; s_items[warp] = in_i; }
+        const uint32_t unit = (images && n) ? cm_pair_cost(w_rows, reinterpret_cast<const uint32_t*>(images + static_cast<uint64_t>(c) * img_bytes)[3]) : 1u;
+        const uint64_t cost = static_cast<uint64_t>(n) * unit;
+        const uint32_t in_p = warp_incl_scan(n, lane);
+        const uint64_t in_c = warp_incl_scan64(cost, lane);
+        if (lane == 31) { s_pairs[warp] = in_p; s_cost[warp] = in_c; }
         __syncthreads();
         if (warp == 0) {
-            const uint32_t a = s_pairs[lane], b = s_items[lane];
-            const uint32_t ia = warp_incl_scan(a, lane), ib = warp_incl_scan(b, lane);
+            const uint32_t a = s_pairs[lane];
+            const uint64_t b = s_cost[lane];
+            const uint32_t ia = warp_incl_scan(a, lane);
+            const uint64_t ib = warp_incl_scan64(b, lane);
             s_pairs[lane] = ia - a;
-            s_items[lane] = ib - b;
+            s_cost[lane] = ib - b;
         }
         __syncthreads();
         const uint32_t ex_p = carry_pairs + s_pairs[warp] + in_p - n;
-        const uint32_t ex_i = carry_items + s_items[warp] + in_i - it;
+        const uint64_t ex_c = carry_cost + s_cost[warp] + in_c - cost;
         if (c < n_chunks) {
             w.bucket_ptr[c] = ex_p;
-            w.item_ptr[c] = ex_i;
+            w.cost_ptr[c] = ex_c;
             w.count[c] = ex_p;  // cursor
         }
         __syncthreads();
-        if (threadIdx.x == 1023) { carry_pairs = ex_p + n; carry_items = ex_i + it; }
+        if (threadIdx.x == 1023) { carry_pairs = ex_p + n; carry_cost = ex_c + cost; }
         __syncthreads();
     }
-    if (threadIdx.x == 0) { w.bucket_ptr[n_chunks] = carry_pairs; w.item_ptr[n_chunks] = carry_items; }
+    if (threadIdx.x == 0) { w.bucket_ptr[n_chunks] = carry_pairs; w.cost_ptr[n_chunks] = carry_cost; }
 }
 
 // one warp per query: append (query, position) to the pair list of every scored slot's chunk (order inside a bucket is
@@ -335,8 +359,75 @@ xl_cm_scatter_kernel(const LayerDev L, const uint32_t* __restrict__ beam_id, con
     }
 }
 
+// First pair of share b of the chunk-sorted pair list when it is cut into `shares` contiguous shares of (nearly) equal
+// estimated work (cost_ptr).  A cut inside a chunk falls on the nearest pair, rounded to a whole 32-pair slice of the chunk.
+// Monotone in b, so the shares tile the list.
+__device__ inline uint32_t cm_share_begin(const CmWork& w, uint32_t n_vc, uint32_t b, uint32_t shares) {
+    if (b >= shares) return w.bucket_ptr[n_vc];
+    const uint64_t T = w.cost_ptr[n_vc];
+    const uint64_t t = static_cast<uint64_t>(T / shares) * b + (T % shares) * b / shares;  // floor(T * b / shares) without overflow
+    if (t >= T) return w.bucket_ptr[n_vc];
+    uint32_t lo = 0, hi = n_vc;  // largest c with cost_ptr[c] <= t: a non-empty chunk, as cost_ptr[c + 1] > t
+    while (hi - lo > 1) {
+        const uint32_t mid = (lo + hi) >> 1;
+        if (w.cost_ptr[mid] <= t) lo = mid; else hi = mid;
+    }
+    const uint32_t n = w.bucket_ptr[lo + 1] - w.bucket_ptr[lo];
+    const uint64_t unit = (w.cost_ptr[lo + 1] - w.cost_ptr[lo]) / n;  // every pair of a chunk costs the same
+    const uint64_t k = ((t - w.cost_ptr[lo] + unit / 2) / unit + 16u) & ~static_cast<uint64_t>(31);
+    return w.bucket_ptr[lo] + (k < n ? static_cast<uint32_t>(k) : n);
+}
+
+// Diagnostics: built with -DPB200_CM_TRACE (tools/profile_cm_kernel.py) the score kernel records, for its last launch, every
+// CTA's %globaltimer start / end and every warp's clock64 cycles by phase in g_cm_trace:
+//   [0] grid, [1] warps per CTA, then per CTA: start ns, end ns, kCmMaxWarps x kCmPhases cycles.
+// Without the define CmTrace is empty and the kernel is unchanged.
+enum { kCmPhImage, kCmPhStaging, kCmPhLookup, kCmPhAccumulate, kCmPhSlice, kCmPhases };
+#ifdef PB200_CM_TRACE
+constexpr uint32_t kCmTraceCtas = 1024;
+constexpr uint32_t kCmTraceCta = 2 + kCmMaxWarps * kCmPhases;
+__device__ unsigned long long g_cm_trace[2 + kCmTraceCtas * kCmTraceCta];
+__device__ __forceinline__ unsigned long long cm_globaltimer() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+struct CmTrace {
+    unsigned long long start;
+    long long t, ph[kCmPhases];
+    __device__ void begin() {
+        start = cm_globaltimer();
+        t = clock64();
+        for (int p = 0; p < kCmPhases; ++p) ph[p] = 0;
+    }
+    __device__ void mark(int p) {
+        const long long n = clock64();
+        ph[p] += n - t;
+        t = n;
+    }
+    __device__ void flush(int warp, int lane) {  // every thread of the CTA calls it once, last
+        __syncthreads();
+        if (blockIdx.x >= kCmTraceCtas) return;
+        unsigned long long* rec = g_cm_trace + 2 + blockIdx.x * kCmTraceCta;
+        if (threadIdx.x == 0) {
+            if (blockIdx.x == 0) { g_cm_trace[0] = gridDim.x; g_cm_trace[1] = blockDim.x >> 5; }
+            rec[0] = start;
+            rec[1] = cm_globaltimer();
+        }
+        if (lane == 0)
+            for (int p = 0; p < kCmPhases; ++p) rec[2 + warp * kCmPhases + p] = static_cast<unsigned long long>(ph[p]);
+    }
+};
+#else
+struct CmTrace {
+    __device__ void begin() {}
+    __device__ void mark(int) {}
+    __device__ void flush(int, int) {}
+};
+#endif
+
 template <bool DIRECT, int STAGES>
-__global__ void __launch_bounds__(kCmMaxWarps * 32)
+__global__ void __launch_bounds__(kCmMaxWarps * 32, 1)
 xl_cm_scores_kernel(const LayerDev L, const QueryDev X, const CmWork w, const CmShape S, const unsigned char* __restrict__ images,
                     float* __restrict__ cand, const uint64_t cand_stride_q) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -366,13 +457,17 @@ xl_cm_scores_kernel(const LayerDev L, const QueryDev X, const CmWork w, const Cm
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     }
     __syncthreads();
+    CmTrace trace;
+    trace.begin();
 
-    // ---- this CTA's contiguous share of the (virtual-)chunk-sorted pair list
+    // ---- this CTA's contiguous share of the (virtual-)chunk-sorted pair list: an equal share of the estimated WORK
     const uint32_t n_vc = S.n_vc;
-    const uint64_t P = w.bucket_ptr[n_vc];
-    const uint32_t begin = static_cast<uint32_t>(P * blockIdx.x / gridDim.x);
-    const uint32_t end = static_cast<uint32_t>(P * (blockIdx.x + 1ull) / gridDim.x);
-    if (begin >= end) return;
+    const uint32_t begin = cm_share_begin(w, n_vc, blockIdx.x, gridDim.x);
+    const uint32_t end = cm_share_begin(w, n_vc, blockIdx.x + 1u, gridDim.x);
+    if (begin >= end) {
+        trace.flush(warp, lane);
+        return;
+    }
     uint32_t c;
     {
         uint32_t lo = 0, hi = n_vc;  // largest c with bucket_ptr[c] <= begin (then skip empty buckets forward)
@@ -389,6 +484,55 @@ xl_cm_scores_kernel(const LayerDev L, const QueryDev X, const CmWork w, const Cm
     const int sub = lane / kCmFeat, fl = lane % kCmFeat;
     uint32_t parity = 0;
 
+    // Adds the entries of this lane's hit rows (hit_r[0, cnt): entry ranges in feature order, hit_x: their x; n_ent entries
+    // in all) to its accumulators.  The rows are ONE stream of entries, kCmSlots per iteration whatever the rows' lengths, so
+    // the warp's trip count follows the lane with the most entries, not (most hits) x (longest row).  Slots of one iteration
+    // may hold entries of different rows, or a column a non-canonical row repeats: a slot whose column an earlier slot of the
+    // iteration also adds to starts from that slot's sum instead of the loaded accumulator, and the stores go out in slot
+    // order -- every column sees exactly the sequential additions, in feature order (inference.hpp:788-811).
+    // hit_r / hit_x are read one past the last hit (the stride-9 row's spare word).
+    auto add_rows = [&](uint32_t cnt, uint32_t n_ent, const uint32_t* hit_r, const float* hit_x) {
+        const uint32_t trips = __reduce_max_sync(kFull, (n_ent + kCmSlots - 1u) / kCmSlots);
+        uint32_t h = 0, e = 0, ee = 0;
+        float x = 0.0f;
+        uint32_t next_r = hit_r[0];  // the next row's range and x, loaded ahead of their use
+        float next_x = hit_x[0];
+        for (uint32_t t = 0; t < trips; ++t) {
+            uint32_t es[kCmSlots], cs[kCmSlots];
+            float xs[kCmSlots], v[kCmSlots];
+            bool on[kCmSlots];  // true for a prefix of the slots
+#pragma unroll
+            for (int u = 0; u < kCmSlots; ++u) {
+                if (e == ee && h < cnt) {
+                    e = next_r & 0xFFFFu;
+                    ee = next_r >> 16;
+                    x = next_x;
+                    ++h;
+                    next_r = hit_r[h];
+                    next_x = hit_x[h];
+                }
+                on[u] = e < ee;
+                es[u] = e;  // an idle slot reads a valid (unused) entry
+                xs[u] = x;
+                e += on[u] ? 1u : 0u;
+            }
+#pragma unroll
+            for (int u = 0; u < kCmSlots; ++u) cs[u] = ec_s[es[u]];
+#pragma unroll
+            for (int u = 0; u < kCmSlots; ++u) v[u] = my_acc[cs[u] * 32u];
+#pragma unroll
+            for (int u = 0; u < kCmSlots; ++u) {
+                float a = v[u];
+#pragma unroll
+                for (int p = 0; p < u; ++p) a = (cs[p] == cs[u]) ? v[p] : a;  // v[p] already holds slot p's sum
+                v[u] = __fadd_rn(a, __fmul_rn(xs[u], ew_s[es[u]]));
+            }
+#pragma unroll
+            for (int u = 0; u < kCmSlots; ++u)
+                if (on[u]) my_acc[cs[u] * 32u] = v[u];
+        }
+    };
+
     for (uint32_t i = begin; i < end;) {
         while (w.bucket_ptr[c + 1] <= i) ++c;                        // virtual chunk holding pair i
         const uint32_t run_end = min(end, w.bucket_ptr[c + 1]);
@@ -397,6 +541,7 @@ xl_cm_scores_kernel(const LayerDev L, const QueryDev X, const CmWork w, const Cm
         if (threadIdx.x == 0) cm_bulk_load(static_cast<uint32_t>(__cvta_generic_to_shared(img)), images + static_cast<uint64_t>(c) * S.img_bytes, S.img_bytes, mbar);
         cm_mbar_wait(mbar, parity);
         parity ^= 1u;
+        trace.mark(kCmPhImage);
         const uint32_t bias_range = hdr_s[0];
         const uint32_t n_cols = hdr_s[1];
 
@@ -443,12 +588,14 @@ xl_cm_scores_kernel(const LayerDev L, const QueryDev X, const CmWork w, const Cm
 #pragma unroll
             for (int st = 0; st < STAGES - 1; ++st) stage_round(static_cast<uint32_t>(st) * kCmFeat, st);
             for (uint32_t col = 0; col < n_cols; ++col) my_acc[col * 32] = 0.0f;
+            trace.mark(kCmPhSlice);
             uint32_t prev_f = kCmEmpty;
             int buf = 0;
             for (uint32_t t0 = 0; t0 < qn_max; t0 += kCmFeat, buf = (buf + 1 == STAGES) ? 0 : buf + 1) {
                 stage_round(t0 + (STAGES - 1) * kCmFeat, (buf + STAGES - 1) % STAGES);  // refills the buffer consumed last round
                 cm_cp_async_wait<STAGES - 1>();
                 __syncwarp();
+                trace.mark(kCmPhStaging);
                 uint32_t* my_idx = st_idx + buf * kBuf + lane * kStride;
                 float* my_val = st_val + buf * kBuf + lane * kStride;
                 const uint32_t n_here = (qn > t0) ? min(static_cast<uint32_t>(kCmFeat), qn - t0) : 0u;
@@ -481,74 +628,43 @@ xl_cm_scores_kernel(const LayerDev L, const QueryDev X, const CmWork w, const Cm
                     }
                     rq[k] = range;
                 }
-                uint32_t cnt = 0;
+                uint32_t cnt = 0, n_ent = 0;
 #pragma unroll
                 for (int k = 0; k < kCmFeat; ++k) {
-                    if (static_cast<int>(rq[k] >> 16) > static_cast<int>(rq[k] & 0xFFFFu)) {
+                    const uint32_t e0 = rq[k] & 0xFFFFu, e1 = rq[k] >> 16;
+                    if (e1 > e0) {
                         my_idx[cnt] = rq[k];
                         my_val[cnt] = xq[k];
                         ++cnt;
+                        n_ent += e1 - e0;
                     }
                 }
+                trace.mark(kCmPhLookup);
                 // phase 2: the hit rows' entries, in feature order, into this lane's accumulators
-                if (L.has_dup_cols) {
-                    // a row may repeat a column (non-canonical W): strictly one entry at a time
-                    for (uint32_t hi = 0; hi < cnt; ++hi) {
-                        const uint32_t range = my_idx[hi];
-                        const float x = my_val[hi];
-                        const uint32_t ee = range >> 16;
-                        for (uint32_t e = range & 0xFFFFu; e < ee; ++e) {
-                            float* a = my_acc + static_cast<uint32_t>(ec_s[e]) * 32u;
-                            *a = __fadd_rn(*a, __fmul_rn(x, ew_s[e]));
-                        }
-                    }
-                } else {
-                    // the columns of ONE row are distinct, so its entries are independent: four at a time -- their column /
-                    // weight loads, accumulator loads, multiply-adds and stores overlap instead of forming one dependent chain
-                    // per entry.  Rows stay in feature order (program order of the accumulator accesses).
-                    for (uint32_t hi = 0; hi < cnt; ++hi) {
-                        const uint32_t range = my_idx[hi];
-                        const float x = my_val[hi];
-                        const uint32_t ee = range >> 16;
-                        for (uint32_t e = range & 0xFFFFu; e < ee; e += 4u) {
-                            const uint32_t n = ee - e;  // >= 1
-                            const uint32_t c0 = ec_s[e];
-                            const uint32_t c1 = ec_s[e + (n > 1u ? 1u : 0u)];
-                            const uint32_t c2 = ec_s[e + (n > 2u ? 2u : 0u)];
-                            const uint32_t c3 = ec_s[e + (n > 3u ? 3u : 0u)];
-                            const float w0 = ew_s[e];
-                            const float w1 = ew_s[e + (n > 1u ? 1u : 0u)];
-                            const float w2 = ew_s[e + (n > 2u ? 2u : 0u)];
-                            const float w3 = ew_s[e + (n > 3u ? 3u : 0u)];
-                            float* a0 = my_acc + c0 * 32u;
-                            float* a1 = my_acc + c1 * 32u;
-                            float* a2 = my_acc + c2 * 32u;
-                            float* a3 = my_acc + c3 * 32u;
-                            const float v0 = *a0, v1 = *a1, v2 = *a2, v3 = *a3;
-                            *a0 = __fadd_rn(v0, __fmul_rn(x, w0));
-                            if (n > 1u) *a1 = __fadd_rn(v1, __fmul_rn(x, w1));
-                            if (n > 2u) *a2 = __fadd_rn(v2, __fmul_rn(x, w2));
-                            if (n > 3u) *a3 = __fadd_rn(v3, __fmul_rn(x, w3));
-                        }
-                    }
-                }
+                add_rows(cnt, n_ent, my_idx, my_val);
+                trace.mark(kCmPhAccumulate);
                 __syncwarp();
             }
             cm_cp_async_wait<0>();
-            if (have && bias_range) {  // bias row last (inference.hpp:806-811)
-                const uint32_t ee = bias_range >> 16;
-                for (uint32_t e = bias_range & 0xFFFFu; e < ee; ++e) {
-                    float* a = my_acc + static_cast<uint32_t>(ec_s[e]) * 32u;
-                    *a = __fadd_rn(*a, __fmul_rn(L.bias, ew_s[e]));
-                }
+            {  // bias row last (inference.hpp:806-811), through the staging buffer of round 0 (no copy is in flight any more)
+                uint32_t* b_idx = st_idx + lane * kStride;
+                float* b_val = st_val + lane * kStride;
+                const uint32_t b0 = bias_range & 0xFFFFu, b1 = bias_range >> 16;
+                const bool live = have && b1 > b0;
+                b_idx[0] = bias_range;
+                b_val[0] = L.bias;
+                add_rows(live ? 1u : 0u, live ? b1 - b0 : 0u, b_idx, b_val);
             }
+            trace.mark(kCmPhAccumulate);
             if (have) {
                 float* dst = cand + static_cast<uint64_t>(q) * cand_stride_q + pos;
                 for (uint32_t col = 0; col < n_cols; ++col) dst[col] = my_acc[col * 32];
             }
+            trace.mark(kCmPhSlice);
         }
         i = run_end;
     }
+    trace.flush(warp, lane);
 }
 
 

@@ -1047,9 +1047,10 @@ XLinearEngine::XLinearEngine(std::unique_ptr<XLinearHostModel> host, int device)
                 if (e_max_out) *e_max_out = best;
                 return n_vc;
             };
-            // Policy: cutting more chunks gives more warps per CTA (a higher issue rate), but the repeated lookups and the
-            // uneven cost of cut / uncut pairs inside the equal-count CTA shares cost more on the eurlex-4k leaf (chunks of
-            // 62 +- 8 columns).  So: the LARGEST cap that fits at all (no cut whenever the layer fits uncut).
+            // Policy: the LARGEST cap that fits at all (no cut whenever the layer fits uncut).  Cutting gives more warps per
+            // CTA, but every cut repeats the pair's lookups.  Measured on an H100 80GB HBM3 at 400 W (eurlex-4k leaf, chunks
+            // of 46 - 84 columns, work-weighted CTA shares): uncut, 6 warps, 0.82 ms; cap 42, 15 warps, 1.08 ms; cap 28,
+            // 16 warps, 1.07 ms -- the kernel is bound by the shared-memory accesses of lookups and entries, not by its warps.
             CmShape shape;
             const uint32_t n_real = layout_for_cap(std::max<uint32_t>(src.c_max, 1u), nullptr, nullptr);
             for (uint32_t cap = std::max<uint32_t>(src.c_max, 1u); n_real > 0; cap = cap * 7 / 8) {
@@ -1211,7 +1212,7 @@ void XLinearEngine::ensure_workspace_(const std::vector<LayerPlan>& plan, uint32
         cm_pair_pos_.reserve(static_cast<uint64_t>(tile_rows) * b_max * 4);
         cm_count_.reserve(chunks_max * 4 + 1);
         cm_bucket_ptr_.reserve(chunks_max * 4 + 1);
-        cm_item_ptr_.reserve(chunks_max * 4 + 1);
+        cm_cost_ptr_.reserve(chunks_max * 4 + 1);
     }
     cand_.reserve(static_cast<uint64_t>(tile_rows) * cand_max);
     if (sort_max) sortbuf_.reserve(static_cast<uint64_t>(tile_rows) * sort_max);
@@ -1267,24 +1268,22 @@ int XLinearEngine::score_layer_(size_t d, const QueryDev& q, uint32_t b_prev, in
                             : CmgPlan{};
     const bool chunk_major_global = cmg.eligible;
     if (chunk_major_global) {
-        CmWork w{cm_slot_pos_.get(), cm_count_.get(), cm_bucket_ptr_.get(), cm_item_ptr_.get(), cm_pair_q_.get(), cm_pair_pos_.get(),
-                 cmg.warps * 32u};
+        CmWork w{cm_slot_pos_.get(), cm_count_.get(), cm_bucket_ptr_.get(), cm_cost_ptr_.get(), cm_pair_q_.get(), cm_pair_pos_.get()};
         PB200_CUDA(cudaMemsetAsync(w.count, 0, (static_cast<uint64_t>(L.n_chunks) + 1) * 4, stream_));
         const uint32_t warp_grid = (rows * 32u + 127u) / 128u;
         xl_cm_count_kernel<<<warp_grid, 128, 0, stream_>>>(L, q, bid_(cur), bcnt_(cur), beam_stride_, rows, w, nullptr);
-        xl_cm_scan_kernel<<<1, 1024, 0, stream_>>>(L.n_chunks, w);
+        xl_cm_scan_kernel<<<1, 1024, 0, stream_>>>(L.n_chunks, w, nullptr, 0u, 0u);
         xl_cm_scatter_kernel<<<warp_grid, 128, 0, stream_>>>(L, bid_(cur), bcnt_(cur), beam_stride_, rows, w, nullptr);
         xl_cmg_scores_kernel<<<cmg.grid, cmg.warps * 32, cmg.smem, stream_>>>(L, q, w, cand_at_(cand_stride_q), cand_stride_q, L.c_max);
         launches_ += 3;
     } else if (chunk_major) {
         const CmShape& shape = layers_[d].cm_shape;
         const uint32_t n_vc = shape.n_vc;
-        CmWork w{cm_slot_pos_.get(), cm_count_.get(), cm_bucket_ptr_.get(), cm_item_ptr_.get(), cm_pair_q_.get(), cm_pair_pos_.get(),
-                 cm.warps * 32u};
+        CmWork w{cm_slot_pos_.get(), cm_count_.get(), cm_bucket_ptr_.get(), cm_cost_ptr_.get(), cm_pair_q_.get(), cm_pair_pos_.get()};
         PB200_CUDA(cudaMemsetAsync(w.count, 0, (static_cast<uint64_t>(n_vc) + 1) * 4, stream_));
         const uint32_t warp_grid = (rows * 32u + 127u) / 128u;
         xl_cm_count_kernel<<<warp_grid, 128, 0, stream_>>>(L, q, bid_(cur), bcnt_(cur), beam_stride_, rows, w, shape.vc_ptr);
-        xl_cm_scan_kernel<<<1, 1024, 0, stream_>>>(n_vc, w);
+        xl_cm_scan_kernel<<<1, 1024, 0, stream_>>>(n_vc, w, layers_[d].cm_images.get(), shape.img_bytes, L.w_rows);
         xl_cm_scatter_kernel<<<warp_grid, 128, 0, stream_>>>(L, bid_(cur), bcnt_(cur), beam_stride_, rows, w, shape.vc_ptr);
         auto launch_cm = [&](auto kernel) {
             kernel<<<cm.grid, cm.warps * 32, cm.smem, stream_>>>(L, q, w, shape, layers_[d].cm_images.get(), cand_at_(cand_stride_q), cand_stride_q);
@@ -1789,3 +1788,12 @@ XLinearEngine::Result XLinearEngine::resident_fetch() {
 #undef PB200_SELECTED_ENGINE
 
 }  // namespace pb200
+
+#ifdef PB200_CM_TRACE
+// diagnostics build only (tools/profile_cm_kernel.py): copies the chunk-major score kernel's trace (see CmTrace) to out
+extern "C" int pb200_cm_trace_fetch(unsigned long long* out, unsigned long long n) {
+    const unsigned long long cap = sizeof(pb200::g_cm_trace) / sizeof(unsigned long long);
+    if (cudaDeviceSynchronize() != cudaSuccess) return -1;
+    return cudaMemcpyFromSymbol(out, pb200::g_cm_trace, (n < cap ? n : cap) * sizeof(unsigned long long)) == cudaSuccess ? 0 : -1;
+}
+#endif

@@ -257,7 +257,8 @@ private:
     bool cmg_all_ = false;      // kernel modes 8, 10
     bool cm_image_ = true;      // staged-image chunk-major kernel (kernel mode 10 switches it off)
     uint32_t n_sm_ = 132;
-    DeviceBuffer<uint32_t> cm_slot_pos_, cm_count_, cm_bucket_ptr_, cm_item_ptr_, cm_pair_q_, cm_pair_pos_;
+    DeviceBuffer<uint32_t> cm_slot_pos_, cm_count_, cm_bucket_ptr_, cm_pair_q_, cm_pair_pos_;
+    DeviceBuffer<uint64_t> cm_cost_ptr_;
     bool force_block_topk_ = false;  // A/B switch: first-generation kernels (row-list streaming + block-wide sort)
     std::vector<XLinearLayerProfile> layer_profile_;
     std::vector<XLinearStats> layer_stats_;
