@@ -211,22 +211,14 @@ void pb200_xlinear_resident_fetch(void* ptr, py_sparse_allocator_t pred_alloc);
 /* Index sharding of the leaf layer over `shard_world` GPUs (one process per GPU; SURVEY.md 8e).  Upper layers are
  * replicated, so every rank walks the identical global beam; rank r keeps the weights of a contiguous range of leaf
  * chunks and scores only those.  weight_matrix_type < 0 loads an mmap folder.
- *   local:  runs all layers, writes this rank's top-k {u64 key, u32 id, f32 value}[rows][stride] and u32 count[rows]
- *           into CALLER-OWNED DEVICE buffers (the send buffers of ONE ncclAllGather); returns stride (<= capacity).
- *   merge:  gathered [world][rows][stride] lists -> global top-k, returned through pred_alloc like c_xlinear_predict_*.
+ *   local:  runs all layers, writes this rank's top-k as 16-byte records {u64 key, u32 id, f32 value}[rows][stride] into
+ *           the CALLER-OWNED DEVICE buffer rec_dev (the send buffer of ONE ncclAllGather, 16 B x rows x stride per rank);
+ *           key == 0 marks an empty slot, so no count array travels.  Returns stride (<= capacity).
+ *   merge:  gathered [world][rows][stride] records g_rec -> global top-k, returned through pred_alloc like
+ *           c_xlinear_predict_*.
  * The result is bit-identical to the unsharded prediction (keys carry the candidate's global position). */
 void* pb200_xlinear_load_sharded(const char* model_path, int weight_matrix_type, uint32_t shard_rank, uint32_t shard_world);
 void pb200_xlinear_get_shard(void* ptr, uint32_t* out /* rank, world, leaf_chunk_begin, leaf_chunk_end */);
-uint32_t pb200_xlinear_sharded_local_csr(void* ptr, const ScipyCsrF32* input_x, uint32_t overridden_beam_size,
-                                         const char* overridden_post_processor_str, uint32_t overridden_only_topk,
-                                         uint32_t stride_capacity, void* keys_dev, void* ids_dev, void* vals_dev, void* cnt_dev);
-void pb200_xlinear_sharded_merge(void* ptr, uint32_t world, uint32_t rows, uint32_t stride, uint32_t overridden_only_topk,
-                                 const void* g_keys, const void* g_ids, const void* g_vals, const void* g_cnt,
-                                 py_sparse_allocator_t pred_alloc);
-
-/* Packed form of the exchange: rec_dev / g_rec hold 16-byte records {u64 key, u32 id, f32 value} ([rows][stride] locally,
- * [world][rows][stride] gathered); key == 0 marks an empty slot, so no count array travels and the whole exchange is ONE
- * ncclAllGather of one buffer (16 B x rows x stride per rank). */
 uint32_t pb200_xlinear_sharded_local_csr_packed(void* ptr, const ScipyCsrF32* input_x, uint32_t overridden_beam_size,
                                                 const char* overridden_post_processor_str, uint32_t overridden_only_topk,
                                                 uint32_t stride_capacity, void* rec_dev);
@@ -238,17 +230,20 @@ void pb200_xlinear_sharded_merge_packed(void* ptr, uint32_t world, uint32_t rows
  *   stats:   out[7*d + {0..6}] = chunks, sum R, sum m, sum e, sum c, sum nnz(x), sum beam-out   (last stats pass) */
 void pb200_xlinear_set_profile(void* ptr, int on);
 /* Kernel generation selector for A/B tests (results are identical): 0 = row-list streaming + block-wide sort,
- * 1 = default (feature-map kernels + warp top-k; query-warp kernel for beams of many narrow chunks), 2 = feature-map
- * lookups with one warp per chunk only, 3 = query-warp kernel wherever it is eligible, 4 = as 1 but the warp top-k
- * evaluates the post-processor for every candidate (no single-precision estimate filter), 5 = as 1 plus the EXPERIMENTAL
- * chunk-major score kernel on eligible layers (written without GPU access at the end of round 1, not validated yet).
+ * 1 = default (feature-map kernels + warp top-k; query-warp kernel for beams of many narrow chunks; chunk-major kernel on
+ * layers whose chunk images fit and whose chunks are visited by enough pairs), 2 = as 1 but feature-map lookups with one
+ * warp per chunk in place of the query-warp kernel, 3 = as 1 but the query-warp kernel wherever it is eligible and the
+ * chunk-major kernel is not chosen, 4 = as 1 but the warp top-k evaluates the post-processor for every candidate (no
+ * single-precision estimate filter), 5 = as 1 plus the chunk-major kernel on every layer with chunk images (its reuse and
+ * occupancy heuristics ignored), 6 = as 1 without the chunk-major kernel (query-major kernels only).  Any other value
+ * behaves as 1.
  * Returns 1 when every layer has a feature map (PB200_FEATMAP_MB caps their total size at load time, default 32768). */
 int pb200_xlinear_set_lookup(void* ptr, int on);
 void pb200_xlinear_reset_profile(void* ptr);
 void pb200_xlinear_get_profile(void* ptr, double* out);
 /* out[2*depth]: per layer {score kernel, top-k kernel} of the last call.  Score: 0 row-list streaming, 1 feature-map
- * lookup (xl_chunk_scores_kernel), 2 dense, 3 xl_query_warp_scores_kernel, 4 xl_cm_scores_kernel (experimental).  Top-k: 0 xl_topk_kernel, 1 xl_topk_warp_kernel,
- * 2 xl_topk_filter_kernel. */
+ * lookup (xl_chunk_scores_kernel), 2 dense, 3 xl_query_warp_scores_kernel, 4 xl_cm_scores_kernel.  Top-k: 0 xl_topk_kernel,
+ * 1 xl_topk_warp_kernel, 2 xl_topk_filter_kernel. */
 void pb200_xlinear_get_kernel_ids(void* ptr, int* out);
 void pb200_xlinear_get_stats(void* ptr, uint64_t* out);
 uint64_t pb200_xlinear_launches(void* ptr);

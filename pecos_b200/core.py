@@ -446,10 +446,6 @@ class B200CoreLib(object):
         fp(c.pb200_xlinear_resident_fetch, None, [c_void_p, ScipyCompressedSparseAllocator.CFUNCTYPE])
         fp(c.pb200_xlinear_load_sharded, c_void_p, [c_char_p, c_int, c_uint32, c_uint32])
         fp(c.pb200_xlinear_get_shard, None, [c_void_p, POINTER(c_uint32)])
-        fp(c.pb200_xlinear_sharded_local_csr, c_uint32, [c_void_p, POINTER(ScipyCsrF32), c_uint32, c_char_p, c_uint32, c_uint32,
-                                                           c_void_p, c_void_p, c_void_p, c_void_p])
-        fp(c.pb200_xlinear_sharded_merge, None, [c_void_p, c_uint32, c_uint32, c_uint32, c_uint32, c_void_p, c_void_p, c_void_p,
-                                                 c_void_p, ScipyCompressedSparseAllocator.CFUNCTYPE])
         fp(c.pb200_xlinear_sharded_local_csr_packed, c_uint32, [c_void_p, POINTER(ScipyCsrF32), c_uint32, c_char_p, c_uint32, c_uint32,
                                                                   c_void_p])
         fp(c.pb200_xlinear_sharded_merge_packed, None, [c_void_p, c_uint32, c_uint32, c_uint32, c_uint32, c_void_p,

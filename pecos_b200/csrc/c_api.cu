@@ -736,27 +736,6 @@ void pb200_xlinear_get_shard(void* ptr, uint32_t* out) {
     PB200_API_END("pb200_xlinear_get_shard")
 }
 
-uint32_t pb200_xlinear_sharded_local_csr(void* ptr, const ScipyCsrF32* X, uint32_t beam, const char* pp, uint32_t topk,
-                                         uint32_t stride_capacity, void* keys_dev, void* ids_dev, void* vals_dev, void* cnt_dev) {
-    PB200_API_BEGIN
-    PB200_LOCK_XL(ptr)
-    return engine_of(ptr).sharded_local_csr(X->row_ptr, X->col_idx, X->val, X->rows, X->cols, beam, pp, topk, stride_capacity,
-                                            static_cast<unsigned long long*>(keys_dev), static_cast<uint32_t*>(ids_dev),
-                                            static_cast<float*>(vals_dev), static_cast<uint32_t*>(cnt_dev));
-    PB200_API_END("pb200_xlinear_sharded_local_csr")
-}
-
-void pb200_xlinear_sharded_merge(void* ptr, uint32_t world, uint32_t rows, uint32_t stride, uint32_t topk, const void* g_keys,
-                                 const void* g_ids, const void* g_vals, const void* g_cnt, py_sparse_allocator_t pred_alloc) {
-    PB200_API_BEGIN
-    PB200_LOCK_XL(ptr)
-    auto r = engine_of(ptr).sharded_merge(world, rows, stride, topk, static_cast<const unsigned long long*>(g_keys),
-                                          static_cast<const uint32_t*>(g_ids), static_cast<const float*>(g_vals),
-                                          static_cast<const uint32_t*>(g_cnt));
-    emit_result(r, pred_alloc);
-    PB200_API_END("pb200_xlinear_sharded_merge")
-}
-
 uint32_t pb200_xlinear_sharded_local_csr_packed(void* ptr, const ScipyCsrF32* X, uint32_t beam, const char* pp, uint32_t topk,
                                                 uint32_t stride_capacity, void* rec_dev) {
     PB200_API_BEGIN

@@ -267,7 +267,7 @@ xl_cm_count_kernel(const LayerDev L, const QueryDev X, const uint32_t* __restric
         if (j < cnt) {
             w.slot_pos[static_cast<uint64_t>(q) * beam_stride + j] = run + incl - width;
             if (scored) {  // one pair per non-empty column range of the chunk
-                const uint32_t v0 = vc_ptr ? vc_ptr[p] : p, nr = vc_ptr ? vc_ptr[p + 1] - v0 : 1u;  // nullptr: no column ranges
+                const uint32_t v0 = vc_ptr[p], nr = vc_ptr[p + 1] - v0;
                 const uint32_t cw = (width + nr - 1u) / max(nr, 1u);
                 for (uint32_t hh = 0; hh < nr && hh * cw < width; ++hh) atomicAdd(&w.count[v0 + hh], 1u);
             }
@@ -291,8 +291,8 @@ __device__ __forceinline__ uint64_t warp_incl_scan64(uint64_t v, int lane) {
     return v;
 }
 
-// single CTA: exclusive scans of the pair counts (bucket offsets) and of the chunks' estimated work (cost_ptr; images ==
-// nullptr: one unit per pair); count[] becomes the scatter cursor.  A chunk's entry count is read from its image header.
+// single CTA: exclusive scans of the pair counts (bucket offsets) and of the chunks' estimated work (cost_ptr); count[]
+// becomes the scatter cursor.  A chunk's entry count is read from its image header.
 __global__ void __launch_bounds__(1024)
 xl_cm_scan_kernel(const uint32_t n_chunks, CmWork w, const unsigned char* __restrict__ images, const uint32_t img_bytes,
                   const uint32_t w_rows) {
@@ -306,7 +306,7 @@ xl_cm_scan_kernel(const uint32_t n_chunks, CmWork w, const unsigned char* __rest
     for (uint32_t c0 = 0; c0 < n_chunks; c0 += 1024) {
         const uint32_t c = c0 + threadIdx.x;
         const uint32_t n = (c < n_chunks) ? w.count[c] : 0u;
-        const uint32_t unit = (images && n) ? cm_pair_cost(w_rows, reinterpret_cast<const uint32_t*>(images + static_cast<uint64_t>(c) * img_bytes)[3]) : 1u;
+        const uint32_t unit = n ? cm_pair_cost(w_rows, reinterpret_cast<const uint32_t*>(images + static_cast<uint64_t>(c) * img_bytes)[3]) : 1u;
         const uint64_t cost = static_cast<uint64_t>(n) * unit;
         const uint32_t in_p = warp_incl_scan(n, lane);
         const uint64_t in_c = warp_incl_scan64(cost, lane);
@@ -349,7 +349,7 @@ xl_cm_scatter_kernel(const LayerDev L, const uint32_t* __restrict__ beam_id, con
         const uint4 h = *reinterpret_cast<const uint4*>(&L.chunks[p]);
         if ((h.w & kChunkAbsent) || h.y == 0) continue;
         const uint32_t pos = w.slot_pos[static_cast<uint64_t>(q) * beam_stride + j];
-        const uint32_t v0 = vc_ptr ? vc_ptr[p] : p, nr = vc_ptr ? vc_ptr[p + 1] - v0 : 1u;
+        const uint32_t v0 = vc_ptr[p], nr = vc_ptr[p + 1] - v0;
         const uint32_t cw = (h.y + nr - 1u) / max(nr, 1u);
         for (uint32_t hh = 0; hh < nr && hh * cw < h.y; ++hh) {
             const uint32_t at = atomicAdd(&w.count[v0 + hh], 1u);
@@ -665,216 +665,4 @@ xl_cm_scores_kernel(const LayerDev L, const QueryDev X, const CmWork w, const Cm
         i = run_end;
     }
     trace.flush(warp, lane);
-}
-
-
-// ------------------------------------------------------------------------------------------------------------------
-// Lane-per-pair scoring WITHOUT a staged image, for layers whose chunks cannot be staged (large feature spaces: the feature map
-// alone is 62 KB of bits per chunk; chunks visited by few pairs: the 3M-label leaf has ~61 pairs per chunk).  Same walk as
-// xl_cm_scores_kernel -- pairs in chunk order, a lane marches through ITS OWN pair, private accumulators acc[col][lane], no
-// cross-lane compaction, no conflict rounds -- but the lookups (feature-map cell), the matched rows' extents and their entries
-// are read from global memory: because the pairs are chunk-sorted, the 32 lanes of a warp and the neighbouring warps work on
-// the same chunk, so those reads hit L1 / L2 (the query-major kernel sends every probe of such a layer to DRAM).  Every load
-// phase of a round is issued for all of the round's features / hits before the first use (8 independent loads in flight per
-// lane).  No CTA-wide state: warps are fully independent (no barrier, no staging of an image).
-// ------------------------------------------------------------------------------------------------------------------
-struct CmgPlan {
-    bool eligible = false;
-    uint32_t warps = 0, grid = 0;
-    size_t smem = 0;
-};
-
-constexpr int kCmgStages = 3;
-
-inline CmgPlan cmg_plan(uint32_t c_max, uint32_t e_max, uint32_t n_chunks, uint64_t pairs, uint32_t n_sm, bool force) {
-    CmgPlan p;
-    if (c_max == 0 || c_max > 256u || e_max >= 65535u || pairs == 0 || n_chunks == 0) return p;
-    if (!force && pairs < static_cast<uint64_t>(kCmMinPairsPerSm) * n_sm) return p;
-    const size_t per_warp = cm_warp_bytes(c_max, kCmgStages);
-    uint32_t warps = static_cast<uint32_t>(std::min<size_t>(kCmMaxWarps, (kCmSmemBudget - 64) / per_warp));
-    if (warps < 2) return p;
-    p.eligible = true;
-    p.warps = warps;
-    p.smem = warps * per_warp + 64;
-    p.grid = n_sm * (p.smem <= (110u << 10) ? 2u : 1u);  // warps are independent: two CTAs per SM when they fit
-    return p;
-}
-
-__global__ void __launch_bounds__(kCmMaxWarps * 32)
-xl_cmg_scores_kernel(const LayerDev L, const QueryDev X, const CmWork w, float* __restrict__ cand, const uint64_t cand_stride_q,
-                     const uint32_t acc_cols) {
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    constexpr int STAGES = kCmgStages;
-    const int lane = threadIdx.x & 31;
-    const int warp = threadIdx.x >> 5;
-    const int nwarps = blockDim.x >> 5;
-    constexpr int kStride = kCmFeat + 1;
-    constexpr int kBuf = 32 * kStride;
-    unsigned char* mine = smem_raw + static_cast<size_t>(warp) * cm_warp_bytes(acc_cols, STAGES);
-    uint32_t* st_idx = reinterpret_cast<uint32_t*>(mine);
-    float* st_val = reinterpret_cast<float*>(st_idx + STAGES * kBuf);
-    float* my_acc = st_val + STAGES * kBuf + lane;
-
-    // ---- this WARP's contiguous share of the chunk-sorted pair list (whole 32-pair slices, never across a chunk boundary)
-    const uint32_t n_chunks = L.n_chunks;
-    const uint64_t P = w.bucket_ptr[n_chunks];
-    const uint64_t gw = static_cast<uint64_t>(blockIdx.x) * nwarps + warp, tw = static_cast<uint64_t>(gridDim.x) * nwarps;
-    const uint32_t begin = static_cast<uint32_t>(P * gw / tw);
-    const uint32_t end = static_cast<uint32_t>(P * (gw + 1ull) / tw);
-    if (begin >= end) return;
-    uint32_t c;
-    {
-        uint32_t lo = 0, hi = n_chunks;
-        while (hi - lo > 1) {
-            const uint32_t mid = (lo + hi) >> 1;
-            if (w.bucket_ptr[mid] <= begin) lo = mid; else hi = mid;
-        }
-        c = lo;
-    }
-    constexpr int kPerIter = 32 / kCmFeat;
-    constexpr int kIters = 32 / kPerIter;
-    const int sub = lane / kCmFeat, fl = lane % kCmFeat;
-
-    for (uint32_t s0 = begin; s0 < end;) {
-        while (w.bucket_ptr[c + 1] <= s0) ++c;
-        const uint32_t run_end = min(end, w.bucket_ptr[c + 1]);
-        const uint32_t s1 = min(s0 + 32u, run_end);                  // this slice: pairs [s0, s1) of chunk c
-        const ChunkHeader h = L.chunks[c];
-        const uint2* __restrict__ fm_g = L.featmap + static_cast<uint64_t>(c) * L.fm_words;
-        const uint2* __restrict__ ext_g = reinterpret_cast<const uint2*>(L.rowext + h.meta_off);
-        const uint2* __restrict__ ent_g = L.entries + h.ent_off;
-        const uint32_t n_cols = h.n_cols;
-        const uint32_t R = h.nnz_rows;
-
-        const uint32_t pidx = s0 + lane;
-        const bool have = pidx < s1;
-        uint32_t q = 0, pos = 0, qn = 0;
-        uint64_t qb = 0;
-        if (have) {
-            q = w.pair_q[pidx];
-            pos = w.pair_pos[pidx];
-            qb = X.row_ptr[q] - X.nnz_base;
-            qn = static_cast<uint32_t>(X.row_ptr[q + 1] - X.nnz_base - qb);
-        }
-        const uint32_t qn_max = __reduce_max_sync(kFull, qn);
-        uint32_t src_o[kIters], src_n[kIters];
-#pragma unroll
-        for (int it = 0; it < kIters; ++it) {
-            const int pi = it * kPerIter + sub;
-            src_o[it] = static_cast<uint32_t>(__shfl_sync(kFull, qb, pi)) + fl;
-            src_n[it] = __shfl_sync(kFull, qn, pi);
-        }
-        auto stage_round = [&](uint32_t t0, int buf) {
-            if (t0 < qn_max) {
-                uint32_t* di = st_idx + buf * kBuf + sub * kStride + fl;
-                float* dv = st_val + buf * kBuf + sub * kStride + fl;
-#pragma unroll
-                for (int it = 0; it < kIters; ++it) {
-                    if (t0 + fl < src_n[it]) {
-                        cm_cp_async4(di + it * kPerIter * kStride, X.col_idx + src_o[it] + t0);
-                        cm_cp_async4(dv + it * kPerIter * kStride, X.val + src_o[it] + t0);
-                    }
-                }
-            }
-            cm_cp_async_commit();
-        };
-        __syncwarp();
-#pragma unroll
-        for (int st = 0; st < STAGES - 1; ++st) stage_round(static_cast<uint32_t>(st) * kCmFeat, st);
-        for (uint32_t col = 0; col < n_cols; ++col) my_acc[col * 32] = 0.0f;
-        uint32_t prev_f = kCmEmpty;
-        int buf = 0;
-        for (uint32_t t0 = 0; t0 < qn_max; t0 += kCmFeat, buf = (buf + 1 == STAGES) ? 0 : buf + 1) {
-            stage_round(t0 + (STAGES - 1) * kCmFeat, (buf + STAGES - 1) % STAGES);
-            cm_cp_async_wait<STAGES - 1>();
-            __syncwarp();
-            uint32_t* my_idx = st_idx + buf * kBuf + lane * kStride;
-            float* my_val = st_val + buf * kBuf + lane * kStride;
-            const uint32_t n_here = (qn > t0) ? min(static_cast<uint32_t>(kCmFeat), qn - t0) : 0u;
-            // phase 1a: the round's features and their feature-map cells (global, independent loads)
-            uint32_t fq[kCmFeat];
-            float xq[kCmFeat];
-            uint2 cell[kCmFeat];
-#pragma unroll
-            for (int k = 0; k < kCmFeat; ++k) {
-                fq[k] = (static_cast<uint32_t>(k) < n_here) ? my_idx[k] : kCmEmpty;
-                xq[k] = my_val[k];
-            }
-#pragma unroll
-            for (int k = 0; k < kCmFeat; ++k) {
-                const uint32_t f = fq[k];
-                const bool dup = (f == prev_f);  // a repeated column index only counts once (the first occurrence)
-                if (static_cast<uint32_t>(k) < n_here) prev_f = f;
-                const bool live = static_cast<uint32_t>(k) < n_here && !dup && f < L.w_rows && R > 0;
-                cell[k] = live ? __ldg(fm_g + (f >> 5)) : make_uint2(0u, 0u);
-                if (!live) fq[k] = 0u;  // bit 0 of an all-zero cell: no hit
-            }
-            // phase 1b: rows of the hits, compacted in place as {row, x}
-            uint32_t cnt = 0;
-#pragma unroll
-            for (int k = 0; k < kCmFeat; ++k) {
-                const uint32_t bit = fq[k] & 31u;
-                if ((cell[k].x >> bit) & 1u) {
-                    my_idx[cnt] = cell[k].y + __popc(cell[k].x & ((1u << bit) - 1u));
-                    my_val[cnt] = xq[k];
-                    ++cnt;
-                }
-            }
-            // phase 1c: the hit rows' extents (independent loads), stored back as packed ranges
-#pragma unroll
-            for (int k0 = 0; k0 < kCmFeat; k0 += 4) {
-                uint2 ex[4];
-#pragma unroll
-                for (int u = 0; u < 4; ++u) ex[u] = (static_cast<uint32_t>(k0 + u) < cnt) ? __ldg(ext_g + my_idx[k0 + u]) : make_uint2(0u, 0u);
-#pragma unroll
-                for (int u = 0; u < 4; ++u) if (static_cast<uint32_t>(k0 + u) < cnt) my_idx[k0 + u] = ex[u].x | (ex[u].y << 16);
-            }
-            // phase 2: entries of the hit rows, in feature order; four independent entries of a row at a time (a row's columns
-            // are distinct unless the model is non-canonical: then strictly one at a time)
-            for (uint32_t hi = 0; hi < cnt; ++hi) {
-                const uint32_t range = my_idx[hi];
-                const float x = my_val[hi];
-                const uint32_t ee = range >> 16;
-                if (L.has_dup_cols) {
-                    for (uint32_t e = range & 0xFFFFu; e < ee; ++e) {
-                        const uint2 en = __ldg(ent_g + e);
-                        float* a = my_acc + en.x * 32u;
-                        *a = __fadd_rn(*a, __fmul_rn(x, __uint_as_float(en.y)));
-                    }
-                    continue;
-                }
-                for (uint32_t e = range & 0xFFFFu; e < ee; e += 4u) {
-                    const uint32_t n = ee - e;
-                    const uint2 e0 = __ldg(ent_g + e);
-                    const uint2 e1 = __ldg(ent_g + e + (n > 1u ? 1u : 0u));
-                    const uint2 e2 = __ldg(ent_g + e + (n > 2u ? 2u : 0u));
-                    const uint2 e3 = __ldg(ent_g + e + (n > 3u ? 3u : 0u));
-                    float* a0 = my_acc + e0.x * 32u;
-                    float* a1 = my_acc + e1.x * 32u;
-                    float* a2 = my_acc + e2.x * 32u;
-                    float* a3 = my_acc + e3.x * 32u;
-                    const float v0 = *a0, v1 = *a1, v2 = *a2, v3 = *a3;
-                    *a0 = __fadd_rn(v0, __fmul_rn(x, __uint_as_float(e0.y)));
-                    if (n > 1u) *a1 = __fadd_rn(v1, __fmul_rn(x, __uint_as_float(e1.y)));
-                    if (n > 2u) *a2 = __fadd_rn(v2, __fmul_rn(x, __uint_as_float(e2.y)));
-                    if (n > 3u) *a3 = __fadd_rn(v3, __fmul_rn(x, __uint_as_float(e3.y)));
-                }
-            }
-            __syncwarp();
-        }
-        cm_cp_async_wait<0>();
-        if (have && (h.has_bias & 1u) && R > 0) {  // bias row last (inference.hpp:806-811)
-            const uint2 br = __ldg(ext_g + (R - 1u));
-            for (uint32_t e = br.x; e < br.y; ++e) {
-                const uint2 en = __ldg(ent_g + e);
-                float* a = my_acc + en.x * 32u;
-                *a = __fadd_rn(*a, __fmul_rn(L.bias, __uint_as_float(en.y)));
-            }
-        }
-        if (have) {
-            float* dst = cand + static_cast<uint64_t>(q) * cand_stride_q + pos;
-            for (uint32_t col = 0; col < n_cols; ++col) dst[col] = my_acc[col * 32];
-        }
-        s0 = s1;
-    }
 }

@@ -783,61 +783,6 @@ xl_topk_warp_kernel(const LayerDev L, const int pp_kind, const int pp_p, const i
 #include "xlinear_selected.cuh"
 #undef PB200_SELECTED_KERNELS
 
-// K3 (index sharding): merge the per-GPU top-k lists gathered by ONE all-gather into the global top-k.
-// gathered layout: [world][rows][stride] for keys / ids / vals and [world][rows] for counts.  Keys are globally unique
-// (they embed the candidate's position in the full prolongated row), so the merge is an exact arg-max selection.
-__global__ void __launch_bounds__(kSelWarps * 32)
-xl_merge_topk_kernel(const unsigned long long* __restrict__ g_keys, const uint32_t* __restrict__ g_ids,
-                     const float* __restrict__ g_vals, const uint32_t* __restrict__ g_cnt, const uint32_t world,
-                     const uint32_t rows, const uint32_t stride, const uint32_t k, uint32_t* __restrict__ out_id,
-                     float* __restrict__ out_val, uint32_t* __restrict__ out_cnt) {
-    __shared__ unsigned long long s_keys[kSelWarps][kSelKeys];
-    const int lane = threadIdx.x & 31;
-    const int warp = threadIdx.x >> 5;
-    const uint32_t q = blockIdx.x * kSelWarps + warp;
-    if (q >= rows) return;
-    unsigned long long* keys = s_keys[warp];
-    const uint32_t n = world * stride;
-    unsigned long long best = 0ull;
-    uint32_t total = 0;
-    for (uint32_t i = lane; i < n; i += 32) {
-        const uint32_t g = i / stride, r = i - g * stride;
-        const uint32_t c = g_cnt[static_cast<uint64_t>(g) * rows + q];
-        unsigned long long key = 0ull;
-        if (r < c) { key = g_keys[(static_cast<uint64_t>(g) * rows + q) * stride + r]; ++total; }
-        keys[i] = key;
-        best = key > best ? key : best;
-    }
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) total += __shfl_xor_sync(kFull, total, d);
-    __syncwarp();
-    const uint32_t kk = min(k, total);
-    if (lane == 0) out_cnt[q] = kk;
-    for (uint32_t rnk = 0; rnk < kk; ++rnk) {
-        unsigned long long top = best;
-#pragma unroll
-        for (int d = 16; d > 0; d >>= 1) {
-            const unsigned long long o = __shfl_xor_sync(kFull, top, d);
-            top = o > top ? o : top;
-        }
-        // the owner lane finds the slot of `top` among its stride-32 subset
-        uint32_t slot = 0xFFFFFFFFu;
-        if (best == top) {
-            for (uint32_t i = lane; i < n; i += 32) if (keys[i] == top) { slot = i; break; }
-        }
-        if (slot != 0xFFFFFFFFu) {
-            const uint32_t g = slot / stride, r = slot - g * stride;
-            const uint64_t src = (static_cast<uint64_t>(g) * rows + q) * stride + r;
-            out_id[static_cast<uint64_t>(q) * k + rnk] = g_ids[src];
-            out_val[static_cast<uint64_t>(q) * k + rnk] = g_vals[src];
-            keys[slot] = 0ull;
-            best = 0ull;
-            for (uint32_t i = lane; i < n; i += 32) { const unsigned long long key = keys[i]; best = key > best ? key : best; }
-        }
-        __syncwarp();
-    }
-}
-
 // Packed exchange records for index sharding: ONE 16-byte {key, id, value} record per (query, rank) slot, key == 0 marks an
 // empty slot (a valid key is never 0: its low word is ~position), so the per-query counts need not travel: the whole exchange
 // is a single all-gather of one buffer.
@@ -859,7 +804,9 @@ __global__ void xl_shard_pack_kernel(const unsigned long long* __restrict__ keys
     rec[i] = out;
 }
 
-// merge of the gathered packed records [world][rows][stride]: same selection as xl_merge_topk_kernel
+// Merge of the per-GPU top-k records gathered by ONE all-gather ([world][rows][stride]) into the global top-k.  Keys are
+// globally unique (they embed the candidate's position in the full prolongated row), so the merge is an exact arg-max
+// selection: for each output rank, the lane holding the warp's largest key finds its slot and emits that record.
 __global__ void __launch_bounds__(kSelWarps * 32)
 xl_merge_packed_kernel(const ShardRecord* __restrict__ g_rec, const uint32_t world, const uint32_t rows, const uint32_t stride,
                        const uint32_t k, uint32_t* __restrict__ out_id, float* __restrict__ out_val, uint32_t* __restrict__ out_cnt) {
@@ -1020,7 +967,6 @@ XLinearEngine::XLinearEngine(std::unique_ptr<XLinearHostModel> host, int device)
         dst.view.c_max = src.c_max;
         dst.view.w_rows = src.w_rows;
         dst.view.bias = src.bias;
-        dst.view.has_dup_cols = src.has_dup_cols ? 1 : 0;
         // chunk images for the chunk-major score kernel (xlinear_cm_kernel.cuh), where the layer's shape allows it.  A column
         // cap cuts the widest chunks of the layer into column ranges ("virtual chunks") when the layer does not fit uncut.
         dst.cm_shape = CmShape{};
@@ -1100,7 +1046,6 @@ XLinearEngine::XLinearEngine(std::unique_ptr<XLinearHostModel> host, int device)
     PB200_CUDA(cudaFuncSetAttribute(xl_cm_scores_kernel<true, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kCmSmemBudget)));
     PB200_CUDA(cudaFuncSetAttribute(xl_cm_scores_kernel<false, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kCmSmemBudget)));
     PB200_CUDA(cudaFuncSetAttribute(xl_cm_scores_kernel<false, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kCmSmemBudget)));
-    PB200_CUDA(cudaFuncSetAttribute(xl_cmg_scores_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kCmSmemBudget)));
     PB200_CUDA(cudaFuncSetAttribute(xl_query_warp_scores_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
     PB200_CUDA(cudaFuncSetAttribute(xl_query_warp_scores_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
     stats_dev_.reserve(8 * layers_.size());
@@ -1134,9 +1079,6 @@ void XLinearEngine::set_kernel_mode(int mode) {
     no_topk_filter_ = (mode == 4);
     chunk_major_ = on && (mode != 6);
     cm_force_ = (mode == 5);
-    cmg_ = (mode == 8 || mode == 9 || mode == 10);  // 9: as 1 plus the image-less lane-per-pair kernel on lookup layers without an image
-    cmg_all_ = (mode == 8 || mode == 10);  // 8: image-less lane-per-pair kernel also in place of the query-warp kernel
-    cm_image_ = (mode != 10);              // 10: as 8, and in place of the staged-image kernel too (tests: every layer on it)
 }
 
 bool XLinearEngine::has_feature_maps() const {
@@ -1253,30 +1195,11 @@ int XLinearEngine::score_layer_(size_t d, const QueryDev& q, uint32_t b_prev, in
     // and the chunks are visited by enough pairs to amortise the staging; otherwise the query-major kernels below.
     // (the statistics pass always runs the query-major kernels: their counters are the canonical ones)
     const bool cm_offsets_fit = static_cast<uint64_t>(rows) * std::max<uint32_t>(q.max_row_nnz, 1u) < (1ull << 32);  // 32-bit feature offsets
-    const CmPlan cm = (chunk_major_ && cm_image_ && lookup && !collect_stats && cm_offsets_fit && cm_slot_pos_.capacity() && layers_[d].cm_images.capacity())
+    const CmPlan cm = (chunk_major_ && lookup && !collect_stats && cm_offsets_fit && cm_slot_pos_.capacity() && layers_[d].cm_images.capacity())
                           ? cm_plan(layers_[d].cm_shape, L.n_chunks, static_cast<uint64_t>(rows) * b_prev, n_sm_, cm_force_)
                           : CmPlan{};
     const bool chunk_major = cm.eligible;
-    // the same lane-per-pair walk without a staged image (xl_cmg_scores_kernel) where the image variant does not apply: layers
-    // of large feature spaces / chunks visited by few pairs.  OPT-IN (kernel modes 8-10): bit-exact but slower than the
-    // query-major kernels on the 3M-label leaf (92 registers + 224 KB keep 12 warps per SM, every lookup a dependent global
-    // load).  Mode 9: in place of the feature-map chunk kernel; 8: also of the
-    // query-warp kernel.
-    const CmgPlan cmg = (chunk_major_ && cmg_ && lookup && !collect_stats && !chunk_major && cm_offsets_fit && cm_slot_pos_.capacity() &&
-                         (cmg_all_ || !query_warp))
-                            ? cmg_plan(L.c_max, layers_[d].e_max, L.n_chunks, static_cast<uint64_t>(rows) * b_prev, n_sm_, cm_force_ || cmg_all_)
-                            : CmgPlan{};
-    const bool chunk_major_global = cmg.eligible;
-    if (chunk_major_global) {
-        CmWork w{cm_slot_pos_.get(), cm_count_.get(), cm_bucket_ptr_.get(), cm_cost_ptr_.get(), cm_pair_q_.get(), cm_pair_pos_.get()};
-        PB200_CUDA(cudaMemsetAsync(w.count, 0, (static_cast<uint64_t>(L.n_chunks) + 1) * 4, stream_));
-        const uint32_t warp_grid = (rows * 32u + 127u) / 128u;
-        xl_cm_count_kernel<<<warp_grid, 128, 0, stream_>>>(L, q, bid_(cur), bcnt_(cur), beam_stride_, rows, w, nullptr);
-        xl_cm_scan_kernel<<<1, 1024, 0, stream_>>>(L.n_chunks, w, nullptr, 0u, 0u);
-        xl_cm_scatter_kernel<<<warp_grid, 128, 0, stream_>>>(L, bid_(cur), bcnt_(cur), beam_stride_, rows, w, nullptr);
-        xl_cmg_scores_kernel<<<cmg.grid, cmg.warps * 32, cmg.smem, stream_>>>(L, q, w, cand_at_(cand_stride_q), cand_stride_q, L.c_max);
-        launches_ += 3;
-    } else if (chunk_major) {
+    if (chunk_major) {
         const CmShape& shape = layers_[d].cm_shape;
         const uint32_t n_vc = shape.n_vc;
         CmWork w{cm_slot_pos_.get(), cm_count_.get(), cm_bucket_ptr_.get(), cm_cost_ptr_.get(), cm_pair_q_.get(), cm_pair_pos_.get()};
@@ -1314,11 +1237,12 @@ int XLinearEngine::score_layer_(size_t d, const QueryDev& q, uint32_t b_prev, in
     }
     PB200_CUDA(cudaGetLastError());
     ++launches_;
-    layer_profile_[d].scores_kernel = chunk_major_global ? 5 : chunk_major ? 4 : query_warp ? 3 : dense ? 2 : lookup ? 1 : 0;
+    layer_profile_[d].scores_kernel = chunk_major ? 4 : query_warp ? 3 : dense ? 2 : lookup ? 1 : 0;
     return layer_profile_[d].scores_kernel;
 }
 
-// Runs every layer over one tile of queries.  The last layer writes into res_*_dev_ at row offset res_row0_.
+// Runs every layer over one tile of queries.  The last layer writes into res_*_dev_ (shard_*_ in an index-sharded run) at
+// row offset res_rows_.
 // ext_beam: beam_*_[0] already hold the beam entering the first layer (single-layer entry point); combine_first: that
 // layer combines its scores with the beam values (a previous prediction was given).
 void XLinearEngine::run_tile_(const QueryDev& q, const std::vector<LayerPlan>& plan, bool collect_stats, bool ext_beam,
@@ -1350,11 +1274,11 @@ void XLinearEngine::run_tile_(const QueryDev& q, const std::vector<LayerPlan>& p
         const bool last = (d + 1 == depth);
         uint32_t* o_id; float* o_val; uint32_t* o_cnt; uint32_t o_stride;
         unsigned long long* o_key = nullptr;
-        if (last && ext_ids_) {  // index-sharded run: local top-k goes straight into the caller's (NCCL send) buffers
-            o_id = ext_ids_ + static_cast<uint64_t>(res_rows_) * res_stride_;
-            o_val = ext_vals_ + static_cast<uint64_t>(res_rows_) * res_stride_;
-            o_cnt = ext_cnt_ + res_rows_;
-            o_key = ext_keys_ + static_cast<uint64_t>(res_rows_) * res_stride_;
+        if (last && shard_run_) {  // index-sharded run: the local top-k, with keys, to be packed into exchange records
+            o_id = shard_ids_.get() + static_cast<uint64_t>(res_rows_) * res_stride_;
+            o_val = shard_vals_.get() + static_cast<uint64_t>(res_rows_) * res_stride_;
+            o_cnt = shard_cnt_.get() + res_rows_;
+            o_key = shard_keys_.get() + static_cast<uint64_t>(res_rows_) * res_stride_;
             o_stride = res_stride_;
         } else if (last) {
             o_id = res_ids_dev_.get() + static_cast<uint64_t>(res_rows_) * res_stride_;
@@ -1683,18 +1607,22 @@ double XLinearEngine::resident_predict(uint32_t beam_size, const char* post_proc
     return static_cast<double>(ms);
 }
 
-uint32_t XLinearEngine::sharded_local_csr(const uint64_t* row_ptr, const uint32_t* col_idx, const float* val, uint32_t rows,
-                                          uint32_t cols, uint32_t beam_size, const char* post_processor, uint32_t only_topk,
-                                          uint32_t stride_capacity, unsigned long long* keys_dev, uint32_t* ids_dev,
-                                          float* vals_dev, uint32_t* cnt_dev) {
+uint32_t XLinearEngine::sharded_local_csr_packed(const uint64_t* row_ptr, const uint32_t* col_idx, const float* val, uint32_t rows,
+                                                 uint32_t cols, uint32_t beam_size, const char* post_processor, uint32_t only_topk,
+                                                 uint32_t stride_capacity, void* rec_dev) {
     PB200_CUDA(cudaSetDevice(device_));
     const auto plan = make_plan_(beam_size, post_processor, only_topk);
     const uint32_t stride = plan.back().k_cap;
     if (stride > stride_capacity) throw std::runtime_error("pecos_b200: sharded output buffers are too narrow for this top-k");
     const uint32_t tile = pick_tile_rows_(plan, rows);
     ensure_workspace_(plan, tile);
+    const uint64_t n = static_cast<uint64_t>(rows) * stride;
+    shard_keys_.reserve(n + 1);
+    shard_ids_.reserve(n + 1);
+    shard_vals_.reserve(n + 1);
+    shard_cnt_.reserve(static_cast<uint64_t>(rows) + 1);
     res_stride_ = stride;
-    ext_keys_ = keys_dev; ext_ids_ = ids_dev; ext_vals_ = vals_dev; ext_cnt_ = cnt_dev;
+    shard_run_ = true;
     try {
         for (uint32_t r0 = 0; r0 < rows; r0 += tile) {
             const uint32_t tr = std::min(tile, rows - r0);
@@ -1708,48 +1636,12 @@ uint32_t XLinearEngine::sharded_local_csr(const uint64_t* row_ptr, const uint32_
             PB200_CUDA(cudaStreamSynchronize(stream_));
         }
     } catch (...) {
-        ext_keys_ = nullptr; ext_ids_ = nullptr; ext_vals_ = nullptr; ext_cnt_ = nullptr;
+        shard_run_ = false;
         throw;
     }
-    ext_keys_ = nullptr; ext_ids_ = nullptr; ext_vals_ = nullptr; ext_cnt_ = nullptr;
-    return stride;
-}
-
-XLinearEngine::Result XLinearEngine::sharded_merge(uint32_t world, uint32_t rows, uint32_t stride, uint32_t only_topk,
-                                                   const unsigned long long* g_keys, const uint32_t* g_ids,
-                                                   const float* g_vals, const uint32_t* g_cnt) {
-    PB200_CUDA(cudaSetDevice(device_));
-    if (static_cast<uint64_t>(world) * stride > static_cast<uint64_t>(kSelKeys))
-        throw std::runtime_error("pecos_b200: world * top-k exceeds the merge kernel's capacity");
-    const uint32_t k = only_topk ? only_topk : static_cast<uint32_t>(host_->layers.back().only_topk);
-    const uint32_t k_out = std::min<uint32_t>(k, world * stride);
-    res_stride_ = k_out;
-    res_ids_dev_.reserve(static_cast<uint64_t>(rows) * k_out + 1);
-    res_vals_dev_.reserve(static_cast<uint64_t>(rows) * k_out + 1);
-    res_cnt_dev_.reserve(static_cast<uint64_t>(rows) + 1);
-    if (rows) {
-        xl_merge_topk_kernel<<<(rows + kSelWarps - 1) / kSelWarps, kSelWarps * 32, 0, stream_>>>(
-            g_keys, g_ids, g_vals, g_cnt, world, rows, stride, k_out, res_ids_dev_.get(), res_vals_dev_.get(), res_cnt_dev_.get());
-        PB200_CUDA(cudaGetLastError());
-        ++launches_;
-    }
-    return finish_result_(rows, k_out);
-}
-
-uint32_t XLinearEngine::sharded_local_csr_packed(const uint64_t* row_ptr, const uint32_t* col_idx, const float* val, uint32_t rows,
-                                                 uint32_t cols, uint32_t beam_size, const char* post_processor, uint32_t only_topk,
-                                                 uint32_t stride_capacity, void* rec_dev) {
-    PB200_CUDA(cudaSetDevice(device_));
-    const uint64_t n = static_cast<uint64_t>(rows) * std::max<uint32_t>(stride_capacity, 1u);
-    shard_keys_.reserve(n + 1);
-    shard_ids_.reserve(n + 1);
-    shard_vals_.reserve(n + 1);
-    shard_cnt_.reserve(static_cast<uint64_t>(rows) + 1);
-    const uint32_t stride = sharded_local_csr(row_ptr, col_idx, val, rows, cols, beam_size, post_processor, only_topk, stride_capacity,
-                                              shard_keys_.get(), shard_ids_.get(), shard_vals_.get(), shard_cnt_.get());
-    const uint64_t total = static_cast<uint64_t>(rows) * stride;
-    if (total) {
-        xl_shard_pack_kernel<<<static_cast<uint32_t>((total + 255) / 256), 256, 0, stream_>>>(
+    shard_run_ = false;
+    if (n) {
+        xl_shard_pack_kernel<<<static_cast<uint32_t>((n + 255) / 256), 256, 0, stream_>>>(
             shard_keys_.get(), shard_ids_.get(), shard_vals_.get(), shard_cnt_.get(), rows, stride, static_cast<ShardRecord*>(rec_dev));
         PB200_CUDA(cudaGetLastError());
         ++launches_;

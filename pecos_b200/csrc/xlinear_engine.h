@@ -32,7 +32,6 @@ struct LayerDev {
     uint32_t c_max;
     uint32_t w_rows;
     float bias;
-    int has_dup_cols;
 };
 
 // Chunk-major score kernel (xlinear_cm_kernel.cuh)
@@ -75,7 +74,7 @@ struct XLinearLayerProfile {
     double scores_ms = 0.0;  // score kernel of the layer
     double topk_ms = 0.0;    // top-k kernel of the layer
     uint64_t launches = 0;
-    int scores_kernel = 0;   // last launch: 0 row-list streaming, 1 feature-map lookup, 2 dense, 3 query-warp, 4 chunk-major, 5 chunk-major without image
+    int scores_kernel = 0;   // last launch: 0 row-list streaming, 1 feature-map lookup, 2 dense, 3 query-warp, 4 chunk-major
     int topk_kernel = 0;     // last launch: 0 block-wide sort, 1 warp arg-max, 2 estimate filter
 };
 
@@ -129,25 +128,18 @@ public:
     double resident_predict(uint32_t beam_size, const char* post_processor, uint32_t only_topk, bool collect_stats);
     Result resident_fetch();
 
-    // Index sharding (leaf layer split over `world` GPUs, SURVEY 8e).  sharded_local_csr runs every layer on this GPU's
-    // shard and writes the LOCAL top-k {key, id, value}[rows][stride] + count[rows] into caller-owned device buffers
-    // (the NCCL all-gather send buffers); sharded_merge reduces the gathered [world][rows][stride] lists to the global
-    // top-k.  Returns the stride used.
-    uint32_t sharded_local_csr(const uint64_t* row_ptr, const uint32_t* col_idx, const float* val, uint32_t rows, uint32_t cols,
-                               uint32_t beam_size, const char* post_processor, uint32_t only_topk, uint32_t stride_capacity,
-                               unsigned long long* keys_dev, uint32_t* ids_dev, float* vals_dev, uint32_t* cnt_dev);
-    Result sharded_merge(uint32_t world, uint32_t rows, uint32_t stride, uint32_t only_topk, const unsigned long long* g_keys,
-                         const uint32_t* g_ids, const float* g_vals, const uint32_t* g_cnt);
-
-    // Packed form: ONE buffer of 16-byte {u64 key, u32 id, f32 value} records [rows][stride] (key == 0: empty slot), so the
-    // exchange is a single all-gather; sharded_merge_packed consumes the gathered [world][rows][stride] records.
+    // Index sharding (leaf layer split over `world` GPUs, SURVEY 8e).  sharded_local_csr_packed runs every layer on this
+    // GPU's shard and writes the LOCAL top-k into the caller-owned device buffer rec_dev (the NCCL all-gather send buffer)
+    // as 16-byte {u64 key, u32 id, f32 value} records [rows][stride] (key == 0: empty slot), so the exchange is a single
+    // all-gather; returns the stride used.  sharded_merge_packed reduces the gathered [world][rows][stride] records to the
+    // global top-k.
     uint32_t sharded_local_csr_packed(const uint64_t* row_ptr, const uint32_t* col_idx, const float* val, uint32_t rows, uint32_t cols,
                                       uint32_t beam_size, const char* post_processor, uint32_t only_topk, uint32_t stride_capacity,
                                       void* rec_dev);
     Result sharded_merge_packed(uint32_t world, uint32_t rows, uint32_t stride, uint32_t only_topk, const void* g_rec);
 
     void set_profile(bool on) { profile_ = on; }
-    // false = stream the chunk row lists (first-generation kernel) even when feature maps exist; for A/B tests
+    // kernel selection for A/B runs and cross-checks: modes 0 - 6, listed at the definition; any other value behaves as 1
     void set_kernel_mode(int mode);
     bool has_feature_maps() const;
     const std::vector<XLinearLayerProfile>& layer_profile() const { return layer_profile_; }
@@ -237,10 +229,7 @@ private:
     DeviceBuffer<unsigned long long> shard_keys_;  // local top-k of an index-sharded run before packing
     DeviceBuffer<uint32_t> shard_ids_, shard_cnt_;
     DeviceBuffer<float> shard_vals_;
-    unsigned long long* ext_keys_ = nullptr;  // caller-owned leaf outputs of an index-sharded run
-    uint32_t* ext_ids_ = nullptr;
-    float* ext_vals_ = nullptr;
-    uint32_t* ext_cnt_ = nullptr;
+    bool shard_run_ = false;  // the last layer writes into shard_*_ (inside sharded_local_csr_packed)
 
     // host result staging (pinned)
     PinnedBuffer<uint32_t> out_ids_;
@@ -253,9 +242,6 @@ private:
     bool no_topk_filter_ = false;
     bool chunk_major_ = true;   // chunk-major scoring wherever cm_plan() finds it eligible (kernel mode 6 switches it off)
     bool cm_force_ = false;     // kernel mode 5
-    bool cmg_ = false;          // image-less lane-per-pair kernel: opt-in (kernel modes 8, 9, 10); slower on the 3M-label model, DESIGN.md 3.3
-    bool cmg_all_ = false;      // kernel modes 8, 10
-    bool cm_image_ = true;      // staged-image chunk-major kernel (kernel mode 10 switches it off)
     uint32_t n_sm_ = 132;
     DeviceBuffer<uint32_t> cm_slot_pos_, cm_count_, cm_bucket_ptr_, cm_pair_q_, cm_pair_pos_;
     DeviceBuffer<uint64_t> cm_cost_ptr_;

@@ -18,7 +18,6 @@
 #pragma once
 
 #include <algorithm>
-#include <atomic>
 #include <cmath>
 #include <thread>
 
@@ -99,7 +98,6 @@ struct ChunkedLayerHost {
     std::string post_processor_name = "l3-hinge";
     PostProc post_processor;
     bool reordered = false;
-    bool has_dup_cols = false;  // some chunk row holds the same column twice (non-canonical W)
     std::vector<ChunkHeader> chunks;
     std::vector<uint32_t> meta;
     std::vector<ChunkEntry> entries;
@@ -232,7 +230,6 @@ inline void build_chunked_layer(const CscHost& W, const CscHost& C, float bias, 
 
     const bool use_bias = bias > 0.0f;
     std::vector<std::vector<uint32_t>> chunk_rows(L.n_chunks), chunk_rptr(L.n_chunks);
-    std::atomic<bool> dup{false};
 
     parallel_for_chunks(L.n_chunks, [&](uint64_t p) {
         struct Nz { uint64_t key; float val; };  // key = row << 32 | column offset; gather order is column-major so a
@@ -272,8 +269,6 @@ inline void build_chunked_layer(const CscHost& W, const CscHost& C, float bias, 
                 rptr.push_back(static_cast<uint32_t>(i));
                 last_row = r;
                 first = false;
-            } else if (out[i - 1].col_offset == co) {
-                dup.store(true);
             }
             out[i].col_offset = co;
             out[i].val = nz[i].val;
@@ -283,7 +278,6 @@ inline void build_chunked_layer(const CscHost& W, const CscHost& C, float bias, 
         // check_bias_explicit (inference.hpp:500-502) gated by bias > 0 (inference.hpp:679-690)
         h.has_bias = (use_bias && rows.back() == W.rows - 1) ? 1u : 0u;
     });
-    L.has_dup_cols = dup.load();
 
     uint64_t meta_total = 0;
     L.c_max = 0; L.r_max = 0;
@@ -566,16 +560,6 @@ inline void load_mmap_layer(const std::string& folder, bool lazy_load, ChunkedLa
                 out_rp[r] = static_cast<uint32_t>(rel);
             }
             ent_cursor = in_rp[h.nnz_rows];
-        }
-        // duplicate (row, col) detection for the serial-accumulate fallback
-        L.has_dup_cols = false;
-        for (uint32_t p = 0; p < chunk_count && !L.has_dup_cols; ++p) {
-            const ChunkHeader& h = L.chunks[p];
-            const uint32_t* m = L.meta.data() + h.meta_off;
-            const uint32_t* rpv = m + round_up4(h.nnz_rows);
-            for (uint32_t r = 0; r < h.nnz_rows && !L.has_dup_cols; ++r)
-                for (uint32_t i = rpv[r] + 1; i < rpv[r + 1]; ++i)
-                    if (L.entries[h.ent_off + i].col_offset == L.entries[h.ent_off + i - 1].col_offset) { L.has_dup_cols = true; break; }
         }
     }
     {

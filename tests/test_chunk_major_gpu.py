@@ -45,11 +45,12 @@ def test_chunk_major_kernel_equals_default_kernels_and_oracles(tmp_path, gpu_cli
             Xd.indices[s + 1] = Xd.indices[s]
             Xd.indices[s + 3] = Xd.indices[s + 2]
     Xd.has_sorted_indices = True
+    Xl = synth.make_queries(133, 200, 400, 300)  # long rows: many rounds of the staging ring
     m, oracles = XLinearModel.load(folder, is_predict_only=True), _oracles(folder, have_ref)
     c = gpu_clib.clib_float32
     h = m.model.model_chain
     for pp in ("l3-hinge", "noop", "log-sigmoid"):
-        for Xq in (X, Xd):
+        for Xq in (X, Xd, Xl):
             c.pb200_xlinear_set_lookup(h, 6)
             base = m.predict(Xq, beam_size=10, only_topk=8, post_processor=pp)
             kid = (c_int * 6)()
@@ -90,40 +91,3 @@ def test_chunk_major_tiles_and_small_batches(tmp_path, gpu_clib, have_ref):
     assert_csr_parity(small, base[:5], rtol=0.0, what="small batch")
     c.pb200_xlinear_set_lookup(h, 1)
 
-
-@pytest.mark.parametrize("permute,prune,sizes,bias", [(False, 0.0, [4, 24, 1500], 1.0), (True, 0.2, [8, 64, 512], 1.0), (True, 0.1, [6, 300], -1.0)])
-def test_imageless_lane_per_pair_kernel_equals_query_major_kernels_and_oracles(tmp_path, gpu_clib, have_ref, permute, prune, sizes, bias):
-    """xl_cmg_scores_kernel (lane per pair, lookups / extents / entries read from global memory in chunk order; opt-in:
-    measured slower than the query-major kernels on the 3M-label model, kept as a validated A/B arm): kernel mode 10 puts EVERY layer on it --
-    same bits as the query-major kernels (mode 6), ids bit-exact / scores 1e-5 vs both oracles."""
-    from pecos_b200.xlinear import XLinearModel
-
-    folder = str(tmp_path / "m")
-    layers = random_tree(631, sizes, 400, 24, bias=bias, permute=permute, prune=prune)
-    synth.save_xlinear_model(folder, layers, bias=bias, only_topk=8)
-    X = csr_with_empty_rows(synth.make_queries(632, 2000, 400, 48), [0, 9, 1999])
-    Xd = X.copy()
-    for r in (3, 11, 500):  # repeated column indices: only the first occurrence counts
-        s, e = Xd.indptr[r], Xd.indptr[r + 1]
-        if e - s >= 4:
-            Xd.indices[s + 1] = Xd.indices[s]
-            Xd.indices[s + 3] = Xd.indices[s + 2]
-    Xd.has_sorted_indices = True
-    Xl = synth.make_queries(633, 200, 400, 300)  # long rows: many rounds of the staging ring
-    m, oracles = XLinearModel.load(folder, is_predict_only=True), _oracles(folder, have_ref)
-    c = gpu_clib.clib_float32
-    h = m.model.model_chain
-    kid = (c_int * 6)()
-    for Xq in (X, Xd, Xl):
-        for pp in ("l3-hinge", "noop"):
-            c.pb200_xlinear_set_lookup(h, 6)
-            base = m.predict(Xq, beam_size=10, only_topk=8, post_processor=pp)
-            c.pb200_xlinear_set_lookup(h, 10)
-            got = m.predict(Xq, beam_size=10, only_topk=8, post_processor=pp)
-            c.pb200_xlinear_get_kernel_ids(h, kid)
-            assert all(kid[2 * d] == 5 for d in range(len(sizes))), "kernel mode 10 must put every layer on the image-less kernel"
-            assert_csr_parity(got, base, rtol=0.0, what=f"image-less lane-per-pair vs query-major {pp}")
-            if Xq is X:
-                for name, o in oracles.items():
-                    assert_csr_parity(got[:150], o.predict(Xq[:150], 10, pp, 8), what=f"image-less lane-per-pair vs {name} {pp}")
-    c.pb200_xlinear_set_lookup(h, 1)

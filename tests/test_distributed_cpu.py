@@ -9,7 +9,7 @@ import pytest
 from pecos_b200 import synth
 from pecos_b200.distributed import split_rows_by_nnz
 
-from .util import merge_topk_numpy, random_tree
+from .util import merge_shards_numpy, random_tree
 
 
 def test_split_rows_by_nnz_balances_and_covers():
@@ -68,7 +68,7 @@ def _worker(rank, world, port, folder, out_dir):
         g = [comm.all_gather(torch.from_numpy(a)).numpy() for a in (keys, ids, vals, cnt)]
         assert g[0].shape == (world, X.shape[0], k) and g[3].shape == (world, X.shape[0])
         assert np.array_equal(g[1][rank], ids)               # own slice sits at index `rank`
-        m_ids, m_vals, m_cnt = merge_topk_numpy(g[0].view(np.uint64), g[1], g[2], g[3], k)
+        m_ids, m_vals, m_cnt = merge_shards_numpy(g[0].view(np.uint64), g[1], g[2], g[3], k)
         for q in range(X.shape[0]):
             w_lab = want.indices[want.indptr[q]:want.indptr[q + 1]]
             assert m_cnt[q] == w_lab.size

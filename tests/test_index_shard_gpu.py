@@ -15,6 +15,9 @@ pytestmark = pytest.mark.gpu
 
 
 def _sharded_predict(clib, ranker, X, world, beam, topk, pp=None):
+    """The production exchange: every rank's local top-k as ONE buffer of 16-byte {key, id, value} records (key == 0: empty),
+    ONE all-gather (emulated by torch.stack), merge of the gathered records.  Also returns the shard ranges and the number of
+    local records (non-zero keys) over all ranks."""
     import torch
 
     from pecos_b200.core import ScipyCompressedSparseAllocator, ScipyCsrF32
@@ -31,32 +34,26 @@ def _sharded_predict(clib, ranker, X, world, beam, topk, pp=None):
         assert ranges[0][0] == 0 and all(ranges[i][1] == ranges[i + 1][0] for i in range(world - 1))
         rows = X.shape[0]
         cx = ScipyCsrF32.init_from(X)
-        bufs = []
-        stride = None
+        recs, stride = [], None
         for h in handles:
-            keys = torch.zeros((rows, topk), dtype=torch.int64, device=dev)
-            ids = torch.zeros((rows, topk), dtype=torch.int32, device=dev)
-            vals = torch.zeros((rows, topk), dtype=torch.float32, device=dev)
-            cnt = torch.zeros((rows,), dtype=torch.int32, device=dev)
+            rec = torch.zeros((rows, topk, 2), dtype=torch.int64, device=dev)
             torch.cuda.synchronize()
-            s = c.pb200_xlinear_sharded_local_csr(h, byref(cx), beam, pp.encode() if pp else None, topk, topk,
-                                                  keys.data_ptr(), ids.data_ptr(), vals.data_ptr(), cnt.data_ptr())
+            s = c.pb200_xlinear_sharded_local_csr_packed(h, byref(cx), beam, pp.encode() if pp else None, topk, topk, rec.data_ptr())
             assert stride in (None, s)
             stride = s
-            bufs.append(tuple(t.view(-1)[: rows * s].view(rows, s) for t in (keys, ids, vals)) + (cnt,))
-        g = [torch.stack([b[i] for b in bufs]).contiguous() for i in range(4)]
+            recs.append(rec.view(-1)[: rows * s * 2].view(rows, s, 2))
+        g = torch.stack(recs).contiguous()
         torch.cuda.synchronize()
         alloc = ScipyCompressedSparseAllocator()
-        c.pb200_xlinear_sharded_merge(handles[0], world, rows, stride, topk, g[0].data_ptr(), g[1].data_ptr(), g[2].data_ptr(),
-                                      g[3].data_ptr(), alloc.cfunc)
-        return alloc.get(), ranges, int(g[3].sum().item())
+        c.pb200_xlinear_sharded_merge_packed(handles[0], world, rows, stride, topk, g.data_ptr(), alloc.cfunc)
+        return alloc.get(), ranges, int((g[..., 0] != 0).sum().item())
     finally:
         for h in handles:
             c.c_xlinear_destruct_model(h)
 
 
 @pytest.mark.parametrize("world", [2, 3, 8])
-def test_index_sharded_prediction_is_bit_identical(tmp_path, gpu_clib, world):
+def test_packed_index_sharded_prediction_is_bit_identical(tmp_path, gpu_clib, world):
     from pecos_b200.xlinear import XLinearModel
 
     folder = str(tmp_path / "m")
@@ -71,7 +68,7 @@ def test_index_sharded_prediction_is_bit_identical(tmp_path, gpu_clib, world):
         assert n_local >= want.nnz  # the union of the local lists covers the global top-k
 
 
-def test_saturated_ties_across_shards(tmp_path, gpu_clib):
+def test_packed_exchange_saturated_ties_across_shards(tmp_path, gpu_clib):
     """All-tie scores: only the embedded global position can order candidates that live on different GPUs."""
     from pecos_b200.xlinear import XLinearModel
 
@@ -85,37 +82,6 @@ def test_saturated_ties_across_shards(tmp_path, gpu_clib):
     assert_csr_parity(got, want, rtol=0.0, what="saturated, world=4")
 
 
-def _sharded_predict_packed(clib, ranker, X, world, beam, topk):
-    """The production exchange: every rank's local top-k as ONE buffer of 16-byte {key, id, value} records (key == 0: empty),
-    ONE all-gather (emulated by torch.stack), merge of the gathered records."""
-    import torch
-
-    from pecos_b200.core import ScipyCompressedSparseAllocator, ScipyCsrF32
-
-    c = clib.clib_float32
-    dev = torch.device("cuda", 0)
-    handles = [c_void_p(c.pb200_xlinear_load_sharded(ranker.encode(), 2, r, world)) for r in range(world)]
-    try:
-        rows = X.shape[0]
-        cx = ScipyCsrF32.init_from(X)
-        recs, stride = [], None
-        for h in handles:
-            rec = torch.zeros((rows, topk, 2), dtype=torch.int64, device=dev)
-            torch.cuda.synchronize()
-            s = c.pb200_xlinear_sharded_local_csr_packed(h, byref(cx), beam, None, topk, topk, rec.data_ptr())
-            assert stride in (None, s)
-            stride = s
-            recs.append(rec.view(-1)[: rows * s * 2].view(rows, s, 2))
-        g = torch.stack(recs).contiguous()
-        torch.cuda.synchronize()
-        alloc = ScipyCompressedSparseAllocator()
-        c.pb200_xlinear_sharded_merge_packed(handles[0], world, rows, stride, topk, g.data_ptr(), alloc.cfunc)
-        return alloc.get()
-    finally:
-        for h in handles:
-            c.c_xlinear_destruct_model(h)
-
-
 @pytest.mark.parametrize("world", [2, 8])
 def test_packed_single_allgather_exchange_is_bit_identical(tmp_path, gpu_clib, world):
     from pecos_b200.xlinear import XLinearModel
@@ -125,5 +91,5 @@ def test_packed_single_allgather_exchange_is_bit_identical(tmp_path, gpu_clib, w
     synth.save_xlinear_model(folder, layers, bias=1.0, only_topk=12)
     X = synth.make_queries(322, 333, 400, 40)
     want = XLinearModel.load(folder, is_predict_only=True).predict(X, beam_size=9, only_topk=12)
-    got = _sharded_predict_packed(gpu_clib, os.path.join(folder, "ranker"), X, world, 9, 12)
+    got, _, _ = _sharded_predict(gpu_clib, os.path.join(folder, "ranker"), X, world, 9, 12)
     assert_csr_parity(got, want, rtol=0.0, what=f"packed exchange, world {world}")

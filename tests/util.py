@@ -64,8 +64,8 @@ def csr_with_empty_rows(X, rows):
     return X
 
 
-def merge_topk_numpy(g_keys, g_ids, g_vals, g_cnt, k):
-    """Reference semantics of the index-sharding merge kernel (test-only): per query keep the k largest 64-bit keys
+def merge_shards_numpy(g_keys, g_ids, g_vals, g_cnt, k):
+    """Reference semantics of the index-sharding merge (test-only): per query keep the k largest 64-bit keys
     among the valid entries of all ranks.  g_* have shape [world, rows, stride], g_cnt [world, rows]."""
     world, rows, stride = g_keys.shape
     out_ids = np.zeros((rows, k), dtype=np.uint32)
