@@ -174,6 +174,13 @@ std::vector<uint32_t> split_rows_by_nnz(const uint64_t* row_ptr, uint32_t rows, 
     return cut;
 }
 
+// the C-ABI matrix arguments as the engine sees them (an absent matrix: empty)
+pb200::HostMatrix host_matrix(const ScipyCsrF32* Xs, const ScipyDrmF32* Xd = nullptr) {
+    if (Xs) return pb200::HostMatrix{Xs->row_ptr, Xs->col_idx, Xs->val, nullptr, Xs->rows, Xs->cols};
+    if (Xd) return pb200::HostMatrix{nullptr, nullptr, nullptr, Xd->val, Xd->rows, Xd->cols};
+    return pb200::HostMatrix{};
+}
+
 constexpr uint32_t kFanOutMinRows = 256;  // below this many rows per device a single engine serves the call
 
 pb200::DeviceBuffer<unsigned char>* g_flush_buf = nullptr;
@@ -254,8 +261,8 @@ void c_xlinear_predict_csr_f32(void* ptr, const ScipyCsrF32* X, const uint32_t o
     const auto cut = split_rows_by_nnz(X->row_ptr, X->rows, n);
     std::vector<pb200::XLinearEngine::Result> parts(n);
     fan_out(n, [&](size_t i) {
-        parts[i] = H.engines[i]->predict_csr(X->row_ptr + cut[i], X->col_idx, X->val, cut[i + 1] - cut[i], X->cols,
-                                             overridden_beam_size, overridden_post_processor_str, overridden_only_topk);
+        const pb200::HostMatrix x{X->row_ptr + cut[i], X->col_idx, X->val, nullptr, cut[i + 1] - cut[i], X->cols};
+        parts[i] = H.engines[i]->predict(x, overridden_beam_size, overridden_post_processor_str, overridden_only_topk);
     });
     emit_results(parts, pred_alloc);
     PB200_API_END("c_xlinear_predict_csr_f32")
@@ -275,8 +282,8 @@ void c_xlinear_predict_drm_f32(void* ptr, const ScipyDrmF32* X, const uint32_t o
     fan_out(n, [&](size_t i) {
         const uint32_t r0 = static_cast<uint32_t>(static_cast<uint64_t>(X->rows) * i / n);
         const uint32_t r1 = static_cast<uint32_t>(static_cast<uint64_t>(X->rows) * (i + 1) / n);
-        parts[i] = H.engines[i]->predict_drm(X->val + static_cast<uint64_t>(r0) * X->cols, r1 - r0, X->cols, overridden_beam_size,
-                                             overridden_post_processor_str, overridden_only_topk);
+        const pb200::HostMatrix x{nullptr, nullptr, nullptr, X->val + static_cast<uint64_t>(r0) * X->cols, r1 - r0, X->cols};
+        parts[i] = H.engines[i]->predict(x, overridden_beam_size, overridden_post_processor_str, overridden_only_topk);
     });
     emit_results(parts, pred_alloc);
     PB200_API_END("c_xlinear_predict_drm_f32")
@@ -305,14 +312,11 @@ void predict_selected(void* ptr, const ScipyCsrF32* Xs, const ScipyDrmF32* Xd, c
                       py_sparse_allocator_t pred_alloc) {
     PB200_LOCK_XL(ptr)
     auto& eng = engine_of(ptr);
-    const uint32_t rows = Xs ? Xs->rows : Xd->rows;
-    const uint32_t cols = Xs ? Xs->cols : Xd->cols;
+    const pb200::HostMatrix x = host_matrix(Xs, Xd);
     if (!sel) throw std::runtime_error("selected_outputs_csr is required");
-    if (sel->rows != rows) throw std::runtime_error("Instance dimension of query and selected output matrix do not match");
-    if (Xd && cols != eng.host().nr_features()) throw std::runtime_error("dense query width != nr_features");
-    auto r = eng.predict_selected(Xs ? Xs->row_ptr : nullptr, Xs ? Xs->col_idx : nullptr, Xs ? Xs->val : nullptr,
-                                  Xd ? Xd->val : nullptr, rows, cols, sel->row_ptr, sel->col_idx, sel->cols, pp);
-    emit_selected(r, pred_alloc);
+    if (sel->rows != x.rows) throw std::runtime_error("Instance dimension of query and selected output matrix do not match");
+    if (Xd && x.cols != eng.host().nr_features()) throw std::runtime_error("dense query width != nr_features");
+    emit_selected(eng.predict_selected(x, host_matrix(sel), pp), pred_alloc);
 }
 
 }  // namespace
@@ -435,19 +439,15 @@ std::shared_ptr<XLinearHandle> layer_engine(const ScipyCscF32* W, const ScipyCsc
 void single_layer_predict(const ScipyCsrF32* Xs, const ScipyDrmF32* Xd, const ScipyCsrF32* codes, ScipyCscF32* W,
                           ScipyCscF32* C, const char* pp, uint32_t only_topk, float bias, py_sparse_allocator_t pred_alloc) {
     if (!pp) throw std::runtime_error("single layer: post_processor_str is required");
-    const uint32_t rows = Xs ? Xs->rows : Xd->rows;
-    const uint32_t cols = Xs ? Xs->cols : Xd->cols;
+    const pb200::HostMatrix x = host_matrix(Xs, Xd);
     auto h = layer_engine(W, C, bias);
     std::lock_guard<std::mutex> lock(h->mu);
     auto& eng = *h->engines[0];
     // MLModel::predict_internal checks (inference.hpp:2041-2051)
-    if (codes && codes->rows != rows) throw std::runtime_error("Instance dimension of query and prev_layer_pred matrix do not match");
+    if (codes && codes->rows != x.rows) throw std::runtime_error("Instance dimension of query and prev_layer_pred matrix do not match");
     if (codes && codes->cols != C->cols) throw std::runtime_error("Label dimension of prev_layer_pred and C matrix do not match");
-    if (Xd && cols != eng.host().nr_features()) throw std::runtime_error("dense query width != nr_features");
-    auto r = eng.predict_single_layer(Xs ? Xs->row_ptr : nullptr, Xs ? Xs->col_idx : nullptr, Xs ? Xs->val : nullptr,
-                                      Xd ? Xd->val : nullptr, rows, cols, codes ? codes->row_ptr : nullptr,
-                                      codes ? codes->col_idx : nullptr, codes ? codes->val : nullptr, pp, only_topk);
-    emit_result(r, pred_alloc);
+    if (Xd && x.cols != eng.host().nr_features()) throw std::runtime_error("dense query width != nr_features");
+    emit_result(eng.predict_single_layer(x, host_matrix(codes), pp, only_topk), pred_alloc);
 }
 
 // c_xlinear_single_layer_predict_on_selected_outputs_* (libpecos.cpp:238-273): one layer handed over by the caller, scores of
@@ -457,19 +457,15 @@ void single_layer_predict_selected(const ScipyCsrF32* Xs, const ScipyDrmF32* Xd,
                                    ScipyCscF32* W, ScipyCscF32* C, const char* pp, float bias, py_sparse_allocator_t pred_alloc) {
     if (!pp) throw std::runtime_error("single layer: post_processor_str is required");
     if (!sel) throw std::runtime_error("selected_outputs_csr is required");
-    const uint32_t rows = Xs ? Xs->rows : Xd->rows;
-    const uint32_t cols = Xs ? Xs->cols : Xd->cols;
+    const pb200::HostMatrix x = host_matrix(Xs, Xd);
     auto h = layer_engine(W, C, bias);
     std::lock_guard<std::mutex> lock(h->mu);
     auto& eng = *h->engines[0];
-    if (sel->rows != rows) throw std::runtime_error("Instance dimension of query and selected output matrix do not match");
-    if (codes && codes->rows != rows) throw std::runtime_error("Instance dimension of query and prev_layer_pred matrix do not match");
+    if (sel->rows != x.rows) throw std::runtime_error("Instance dimension of query and selected output matrix do not match");
+    if (codes && codes->rows != x.rows) throw std::runtime_error("Instance dimension of query and prev_layer_pred matrix do not match");
     if (codes && codes->cols != C->cols) throw std::runtime_error("Label dimension of prev_layer_pred and C matrix do not match");
-    if (Xd && cols != eng.host().nr_features()) throw std::runtime_error("dense query width != nr_features");
-    auto r = eng.predict_selected(Xs ? Xs->row_ptr : nullptr, Xs ? Xs->col_idx : nullptr, Xs ? Xs->val : nullptr,
-                                  Xd ? Xd->val : nullptr, rows, cols, sel->row_ptr, sel->col_idx, sel->cols, pp,
-                                  codes ? codes->row_ptr : nullptr, codes ? codes->col_idx : nullptr, codes ? codes->val : nullptr);
-    emit_selected(r, pred_alloc);
+    if (Xd && x.cols != eng.host().nr_features()) throw std::runtime_error("dense query width != nr_features");
+    emit_selected(eng.predict_selected(x, host_matrix(sel), pp, host_matrix(codes)), pred_alloc);
 }
 
 }  // namespace
@@ -565,17 +561,13 @@ void mlmodel_predict(void* ptr, const ScipyCsrF32* Xs, const ScipyDrmF32* Xd, co
     PB200_LOCK_XL(ptr)
     auto& eng = engine_of(ptr);
     const auto& L = eng.host().layers.at(0);
-    const uint32_t rows = Xs ? Xs->rows : Xd->rows;
-    const uint32_t cols = Xs ? Xs->cols : Xd->cols;
-    if (codes && codes->rows != rows) throw std::runtime_error("Instance dimension of query and prev_layer_pred matrix do not match");
+    const pb200::HostMatrix x = host_matrix(Xs, Xd);
+    if (codes && codes->rows != x.rows) throw std::runtime_error("Instance dimension of query and prev_layer_pred matrix do not match");
     if (codes && codes->cols != L.n_chunks) throw std::runtime_error("Label dimension of prev_layer_pred and C matrix do not match");
-    if (Xd && cols != eng.host().nr_features()) throw std::runtime_error("dense query width != nr_features");
+    if (Xd && x.cols != eng.host().nr_features()) throw std::runtime_error("dense query width != nr_features");
     // only_topk_to_use / post_processor_to_use (inference.hpp:2055-2058): the override if given, else the stored value
     const uint32_t k = only_topk > 0 ? only_topk : static_cast<uint32_t>(L.only_topk);
-    auto r = eng.predict_single_layer(Xs ? Xs->row_ptr : nullptr, Xs ? Xs->col_idx : nullptr, Xs ? Xs->val : nullptr,
-                                      Xd ? Xd->val : nullptr, rows, cols, codes ? codes->row_ptr : nullptr,
-                                      codes ? codes->col_idx : nullptr, codes ? codes->val : nullptr, pp, k);
-    emit_result(r, pred_alloc);
+    emit_result(eng.predict_single_layer(x, host_matrix(codes), pp, k), pred_alloc);
 }
 
 void mlmodel_predict_selected(void* ptr, const ScipyCsrF32* Xs, const ScipyDrmF32* Xd, const ScipyCsrF32* sel,
@@ -583,17 +575,13 @@ void mlmodel_predict_selected(void* ptr, const ScipyCsrF32* Xs, const ScipyDrmF3
     PB200_LOCK_XL(ptr)
     auto& eng = engine_of(ptr);
     const auto& L = eng.host().layers.at(0);
-    const uint32_t rows = Xs ? Xs->rows : Xd->rows;
-    const uint32_t cols = Xs ? Xs->cols : Xd->cols;
+    const pb200::HostMatrix x = host_matrix(Xs, Xd);
     if (!sel) throw std::runtime_error("selected_outputs_csr is required");
-    if (sel->rows != rows) throw std::runtime_error("Instance dimension of query and selected output matrix do not match");
-    if (codes && codes->rows != rows) throw std::runtime_error("Instance dimension of query and prev_layer_pred matrix do not match");
+    if (sel->rows != x.rows) throw std::runtime_error("Instance dimension of query and selected output matrix do not match");
+    if (codes && codes->rows != x.rows) throw std::runtime_error("Instance dimension of query and prev_layer_pred matrix do not match");
     if (codes && codes->cols != L.n_chunks) throw std::runtime_error("Label dimension of prev_layer_pred and C matrix do not match");
-    if (Xd && cols != eng.host().nr_features()) throw std::runtime_error("dense query width != nr_features");
-    auto r = eng.predict_selected(Xs ? Xs->row_ptr : nullptr, Xs ? Xs->col_idx : nullptr, Xs ? Xs->val : nullptr,
-                                  Xd ? Xd->val : nullptr, rows, cols, sel->row_ptr, sel->col_idx, sel->cols, pp,
-                                  codes ? codes->row_ptr : nullptr, codes ? codes->col_idx : nullptr, codes ? codes->val : nullptr);
-    emit_selected(r, pred_alloc);
+    if (Xd && x.cols != eng.host().nr_features()) throw std::runtime_error("dense query width != nr_features");
+    emit_selected(eng.predict_selected(x, host_matrix(sel), pp, host_matrix(codes)), pred_alloc);
 }
 
 }  // namespace
@@ -704,7 +692,7 @@ void pb200_sparse_candidate_distances(int device, int metric, const void* row_pt
 void pb200_xlinear_resident_upload_csr(void* ptr, const ScipyCsrF32* X) {
     PB200_API_BEGIN
     PB200_LOCK_XL(ptr)
-    engine_of(ptr).resident_upload_csr(X->row_ptr, X->col_idx, X->val, X->rows, X->cols);
+    engine_of(ptr).resident_upload_csr(host_matrix(X));
     PB200_API_END("pb200_xlinear_resident_upload_csr")
 }
 
@@ -740,7 +728,7 @@ uint32_t pb200_xlinear_sharded_local_csr_packed(void* ptr, const ScipyCsrF32* X,
                                                 uint32_t stride_capacity, void* rec_dev) {
     PB200_API_BEGIN
     PB200_LOCK_XL(ptr)
-    return engine_of(ptr).sharded_local_csr_packed(X->row_ptr, X->col_idx, X->val, X->rows, X->cols, beam, pp, topk, stride_capacity, rec_dev);
+    return engine_of(ptr).sharded_local_csr_packed(host_matrix(X), beam, pp, topk, stride_capacity, rec_dev);
     PB200_API_END("pb200_xlinear_sharded_local_csr_packed")
 }
 

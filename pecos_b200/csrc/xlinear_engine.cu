@@ -779,9 +779,23 @@ xl_topk_warp_kernel(const LayerDev L, const int pp_kind, const int pp_p, const i
 
 #include "xlinear_topk_filter.cuh"
 
-#define PB200_SELECTED_KERNELS
-#include "xlinear_selected.cuh"
-#undef PB200_SELECTED_KERNELS
+// predict_selected: one CTA per query; its entries [ent_ptr[q], ent_ptr[q + 1]) read candidate ent_pos[e] of the query's row
+// and, when `combine`, the value of entry prev_ptr[q] + ent_parent[e] of the previous layer
+__global__ void __launch_bounds__(128)
+xl_selected_gather_kernel(const float* __restrict__ cand, const uint64_t cand_stride_q, const uint64_t* __restrict__ ent_ptr,
+                          const uint32_t* __restrict__ ent_pos, const uint32_t* __restrict__ ent_parent,
+                          const uint64_t* __restrict__ prev_ptr, const float* __restrict__ prev_val, float* __restrict__ cur_val,
+                          const int pp_kind, const int pp_p, const int combine) {
+    const uint32_t q = blockIdx.x;
+    const uint64_t b = ent_ptr[q], e = ent_ptr[q + 1];
+    const float* cq = cand + static_cast<uint64_t>(q) * cand_stride_q;
+    const uint64_t pb = combine ? prev_ptr[q] : 0;
+    for (uint64_t i = b + threadIdx.x; i < e; i += blockDim.x) {
+        float v = xl_transform(cq[ent_pos[i]], pp_kind, pp_p);
+        if (combine) v = xl_combine(v, prev_val[pb + ent_parent[i]], pp_kind);
+        cur_val[i] = v;
+    }
+}
 
 // Packed exchange records for index sharding: ONE 16-byte {key, id, value} record per (query, rank) slot, key == 0 marks an
 // empty slot (a valid key is never 0: its low word is ~position), so the per-query counts need not travel: the whole exchange
@@ -912,11 +926,6 @@ XLinearEngine::XLinearEngine(std::unique_ptr<XLinearHostModel> host, int device)
     PB200_CUDA(cudaStreamCreateWithFlags(&copy_stream_, cudaStreamNonBlocking));
     for (auto& e : up_ev_) PB200_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     for (auto& e : use_ev_) PB200_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    if (const char* env = std::getenv("PB200_XL_PIPELINE")) {  // 0 = off, n >= 2 = number of sub-tiles (default 4)
-        const int v = std::atoi(env);
-        pipeline_uploads_ = v != 0;
-        if (v >= 2) pipeline_parts_ = static_cast<uint32_t>(std::min(v, 64));
-    }
     layers_.resize(host_->layers.size());
     uint64_t cmimg_budget = 8ull << 30;     // bytes of HBM the chunk images of the chunk-major kernel may take in total
     if (const char* env = std::getenv("PB200_CMIMG_MB")) cmimg_budget = std::strtoull(env, nullptr, 10) << 20;
@@ -1091,13 +1100,14 @@ void XLinearEngine::reset_profile() {
     launches_ = 0;
 }
 
-std::vector<XLinearEngine::LayerPlan> XLinearEngine::make_plan_(uint32_t beam_size, const char* post_processor,
-                                                                 uint32_t only_topk) const {
+std::vector<XLinearEngine::LayerPlan> XLinearEngine::make_plan_(uint32_t beam_size, const char* post_processor, uint32_t only_topk,
+                                                                 const std::vector<uint32_t>& b_in, bool topk) const {
     const size_t depth = layers_.size();
     std::vector<LayerPlan> plan(depth);
     uint32_t b_prev = 1;
     for (size_t d = 0; d < depth; ++d) {
         const auto& L = host_->layers[d];
+        if (d < b_in.size() && b_in[d] > 0) b_prev = b_in[d];
         // local_only_topk (inference.hpp:2471) then only_topk_to_use (inference.hpp:2055)
         const uint32_t local = (d + 1 == depth) ? only_topk : beam_size;
         const uint32_t k = local > 0 ? local : static_cast<uint32_t>(L.only_topk);
@@ -1106,69 +1116,64 @@ std::vector<XLinearEngine::LayerPlan> XLinearEngine::make_plan_(uint32_t beam_si
         plan[d].b_prev = b_prev;
         const uint64_t cand_max = static_cast<uint64_t>(b_prev) * std::max<uint32_t>(L.c_max, 1u);
         plan[d].k_cap = static_cast<uint32_t>(std::max<uint64_t>(1, std::min<uint64_t>(k, cand_max)));
-        if (topk_kernel_smem(b_prev) > 200u * 1024u)
+        if (b_prev > 32768u || (topk && topk_kernel_smem(b_prev) > 200u * 1024u))
             throw std::runtime_error("pecos_b200: beam of " + std::to_string(b_prev) + " nodes exceeds the supported maximum");
         b_prev = plan[d].k_cap;
     }
     return plan;
 }
 
-uint32_t XLinearEngine::pick_tile_rows_(const std::vector<LayerPlan>& plan, uint32_t rows) const {
-    uint64_t budget = 8ull << 30;
-    if (const char* env = std::getenv("PB200_WORKSPACE_MB")) budget = std::max<uint64_t>(64, std::strtoull(env, nullptr, 10)) << 20;
-    uint64_t per_query = 16;
-    uint64_t beam_stride = 1, cand_max = 1, sort_max = 0;
-    for (size_t d = 0; d < plan.size(); ++d) {
-        const uint64_t c = static_cast<uint64_t>(plan[d].b_prev) * std::max<uint32_t>(host_->layers[d].c_max, 1u);
-        cand_max = std::max(cand_max, c);
-        beam_stride = std::max<uint64_t>(beam_stride, plan[d].k_cap);
-        if (c > static_cast<uint64_t>(kSortCap) && plan[d].k > static_cast<uint32_t>(kSortCap / 2)) sort_max = std::max<uint64_t>(sort_max, next_pow2_host(c));
-    }
-    per_query += 2 * beam_stride * 8 + cand_max * 4 + sort_max * 8;
-    uint64_t tile = std::max<uint64_t>(1, budget / per_query);
-    return static_cast<uint32_t>(std::min<uint64_t>(tile, std::max<uint32_t>(rows, 1u)));
-}
-
-void XLinearEngine::ensure_workspace_(const std::vector<LayerPlan>& plan, uint32_t tile_rows) {
-    uint64_t beam_stride = 1, cand_max = 1, sort_max = 0;
+uint32_t XLinearEngine::ensure_workspace_(const std::vector<LayerPlan>& plan, uint32_t rows, uint32_t dense_cols) {
+    // per query: the two ping-pong beams (stride = the widest beam entering or leaving a layer), the candidate row, the sort
+    // scratch of the block top-k, and the chunk-major kernel's slot positions and pair lists
+    uint64_t beam_stride = 1, cand_max = 1, sort_max = 0, b_max = 1, chunks_max = 1;
     for (size_t d = 0; d < plan.size(); ++d) {
         const uint64_t c = static_cast<uint64_t>(plan[d].b_prev) * std::max<uint32_t>(host_->layers[d].c_max, 1u);
         cand_max = std::max(cand_max, c);
         beam_stride = std::max<uint64_t>(beam_stride, std::max<uint32_t>(plan[d].k_cap, plan[d].b_prev));
         if (c > static_cast<uint64_t>(kSortCap) && plan[d].k > static_cast<uint32_t>(kSortCap / 2)) sort_max = std::max<uint64_t>(sort_max, next_pow2_host(c));
+        b_max = std::max<uint64_t>(b_max, plan[d].b_prev);
+        chunks_max = std::max<uint64_t>(chunks_max, host_->layers[d].n_chunks);
     }
+    const bool cm = chunk_major_ && has_feature_maps();
+    const uint64_t pairs = b_max * 4;  // up to 4 column ranges per chunk
+    const uint64_t per_query = 16 + 2 * beam_stride * 8 + cand_max * 4 + sort_max * 8 + (cm ? beam_stride * 4 + pairs * 8 : 0);
+    uint64_t budget = 8ull << 30;
+    if (const char* env = std::getenv("PB200_WORKSPACE_MB")) budget = std::max<uint64_t>(64, std::strtoull(env, nullptr, 10)) << 20;
+    uint64_t tile = std::min<uint64_t>(std::max<uint64_t>(1, budget / per_query), std::max<uint32_t>(rows, 1u));
+    if (dense_cols) tile = std::min<uint64_t>(tile, std::max<uint64_t>(1, (4ull << 30) / (static_cast<uint64_t>(dense_cols) * 4)));
+
     beam_stride_ = static_cast<uint32_t>(beam_stride);
     for (int b = 0; b < 2; ++b) {
-        beam_id_[b].reserve(static_cast<uint64_t>(tile_rows) * beam_stride);
-        beam_val_[b].reserve(static_cast<uint64_t>(tile_rows) * beam_stride);
-        beam_cnt_[b].reserve(tile_rows);
+        beam_id_[b].reserve(tile * beam_stride);
+        beam_val_[b].reserve(tile * beam_stride);
+        beam_cnt_[b].reserve(tile);
     }
-    if (chunk_major_ && has_feature_maps()) {
-        uint64_t b_max = 1, chunks_max = 1;
-        for (size_t d = 0; d < plan.size(); ++d) {
-            b_max = std::max<uint64_t>(b_max, plan[d].b_prev);
-            chunks_max = std::max<uint64_t>(chunks_max, host_->layers[d].n_chunks);
-        }
-        cm_slot_pos_.reserve(static_cast<uint64_t>(tile_rows) * beam_stride);
-        cm_pair_q_.reserve(static_cast<uint64_t>(tile_rows) * b_max * 4);   // up to 4 column ranges per chunk
-        cm_pair_pos_.reserve(static_cast<uint64_t>(tile_rows) * b_max * 4);
+    if (cm) {
+        cm_slot_pos_.reserve(tile * beam_stride);
+        cm_pair_q_.reserve(tile * pairs);
+        cm_pair_pos_.reserve(tile * pairs);
         cm_count_.reserve(chunks_max * 4 + 1);
         cm_bucket_ptr_.reserve(chunks_max * 4 + 1);
         cm_cost_ptr_.reserve(chunks_max * 4 + 1);
     }
-    cand_.reserve(static_cast<uint64_t>(tile_rows) * cand_max);
-    if (sort_max) sortbuf_.reserve(static_cast<uint64_t>(tile_rows) * sort_max);
+    cand_.reserve(tile * cand_max);
+    if (sort_max) sortbuf_.reserve(tile * sort_max);
+    return static_cast<uint32_t>(tile);
 }
 
 // Launches the score kernel of layer d for the beam held in beam_*_[cur] (capacity b_prev slots per query): fills
-// cand_[q * b_prev * c_max + slot_base(j) + c] with the raw scores of every child of every beam node, in prolongation order.
+// cand_[(ws_row + q) * b_prev * c_max + slot_base(j) + c] with the raw scores of every child of every beam node, in prolongation order.
 // Chooses between the chunk-major, query-warp, feature-map, row-list and dense kernels.  Returns the kernel id.
-int XLinearEngine::score_layer_(size_t d, const QueryDev& q, uint32_t b_prev, int cur, bool collect_stats) {
+int XLinearEngine::score_layer_(size_t d, const QueryDev& q, uint32_t b_prev, int cur, uint32_t ws_row, bool collect_stats) {
     const LayerDev& L = layers_[d].view;
     const uint32_t rows = q.rows;
     const bool dense = (q.row_ptr == nullptr);
     const uint32_t c_stride = std::max<uint32_t>(L.c_max, 1u);
     const uint64_t cand_stride_q = static_cast<uint64_t>(b_prev) * c_stride;
+    float* cand = cand_.get() + ws_row * cand_stride_q;
+    const uint32_t* bid = bid_(cur, ws_row);
+    const uint32_t* bcnt = bcnt_(cur, ws_row);
     unsigned long long* stats = collect_stats ? stats_dev_.get() + 8 * d : nullptr;
     // spread the beam slots evenly: b = 10 -> 10 warps x 1 slot, b = 20 -> 10 warps x 2 slots
     const uint32_t rounds = (b_prev + kWarpsMax - 1) / kWarpsMax;
@@ -1181,7 +1186,7 @@ int XLinearEngine::score_layer_(size_t d, const QueryDev& q, uint32_t b_prev, in
     const uint32_t hdr_cap = b_prev <= 128u ? b_prev : 0u;  // beam chunk headers cached in shared memory
     const size_t smem1 = chunk_kernel_smem(warps, lookup, q_cap, sb_cap, hdr_cap);
     auto launch = [&](auto kernel) {
-        kernel<<<grid, block, smem1, stream_>>>(L, q, bid_(cur), bcnt_(cur), beam_stride_, cand_at_(cand_stride_q),
+        kernel<<<grid, block, smem1, stream_>>>(L, q, bid, bcnt, beam_stride_, cand,
                                                cand_stride_q, c_stride, stats, q_cap, sb_cap, hdr_cap);
     };
     // One warp per query over the whole beam (feature-major).  It wins when the beam consists of MANY NARROW chunks
@@ -1205,11 +1210,11 @@ int XLinearEngine::score_layer_(size_t d, const QueryDev& q, uint32_t b_prev, in
         CmWork w{cm_slot_pos_.get(), cm_count_.get(), cm_bucket_ptr_.get(), cm_cost_ptr_.get(), cm_pair_q_.get(), cm_pair_pos_.get()};
         PB200_CUDA(cudaMemsetAsync(w.count, 0, (static_cast<uint64_t>(n_vc) + 1) * 4, stream_));
         const uint32_t warp_grid = (rows * 32u + 127u) / 128u;
-        xl_cm_count_kernel<<<warp_grid, 128, 0, stream_>>>(L, q, bid_(cur), bcnt_(cur), beam_stride_, rows, w, shape.vc_ptr);
+        xl_cm_count_kernel<<<warp_grid, 128, 0, stream_>>>(L, q, bid, bcnt, beam_stride_, rows, w, shape.vc_ptr);
         xl_cm_scan_kernel<<<1, 1024, 0, stream_>>>(n_vc, w, layers_[d].cm_images.get(), shape.img_bytes, L.w_rows);
-        xl_cm_scatter_kernel<<<warp_grid, 128, 0, stream_>>>(L, bid_(cur), bcnt_(cur), beam_stride_, rows, w, shape.vc_ptr);
+        xl_cm_scatter_kernel<<<warp_grid, 128, 0, stream_>>>(L, bid, bcnt, beam_stride_, rows, w, shape.vc_ptr);
         auto launch_cm = [&](auto kernel) {
-            kernel<<<cm.grid, cm.warps * 32, cm.smem, stream_>>>(L, q, w, shape, layers_[d].cm_images.get(), cand_at_(cand_stride_q), cand_stride_q);
+            kernel<<<cm.grid, cm.warps * 32, cm.smem, stream_>>>(L, q, w, shape, layers_[d].cm_images.get(), cand, cand_stride_q);
         };
         if (shape.direct) { if (shape.stages == 4) launch_cm(xl_cm_scores_kernel<true, 4>); else launch_cm(xl_cm_scores_kernel<true, 2>); }
         else { if (shape.stages == 4) launch_cm(xl_cm_scores_kernel<false, 4>); else launch_cm(xl_cm_scores_kernel<false, 2>); }
@@ -1221,10 +1226,10 @@ int XLinearEngine::score_layer_(size_t d, const QueryDev& q, uint32_t b_prev, in
         const dim3 qw_grid((rows + kQwWarps - 1) / kQwWarps);
         if (collect_stats)
             xl_query_warp_scores_kernel<true><<<qw_grid, kQwWarps * 32, qw_smem, stream_>>>(
-                L, q, bid_(cur), bcnt_(cur), beam_stride_, cand_at_(cand_stride_q), cand_stride_q, stats, qw_qcap, qw_ncap, rows);
+                L, q, bid, bcnt, beam_stride_, cand, cand_stride_q, stats, qw_qcap, qw_ncap, rows);
         else
             xl_query_warp_scores_kernel<false><<<qw_grid, kQwWarps * 32, qw_smem, stream_>>>(
-                L, q, bid_(cur), bcnt_(cur), beam_stride_, cand_at_(cand_stride_q), cand_stride_q, stats, qw_qcap, qw_ncap, rows);
+                L, q, bid, bcnt, beam_stride_, cand, cand_stride_q, stats, qw_qcap, qw_ncap, rows);
     } else if (dense) {
         if (collect_stats) launch(xl_chunk_scores_kernel<true, true, false>);
         else launch(xl_chunk_scores_kernel<true, false, false>);
@@ -1241,19 +1246,15 @@ int XLinearEngine::score_layer_(size_t d, const QueryDev& q, uint32_t b_prev, in
     return layer_profile_[d].scores_kernel;
 }
 
-// Runs every layer over one tile of queries.  The last layer writes into res_*_dev_ (shard_*_ in an index-sharded run) at
-// row offset res_rows_.
-// ext_beam: beam_*_[0] already hold the beam entering the first layer (single-layer entry point); combine_first: that
-// layer combines its scores with the beam values (a previous prediction was given).
-void XLinearEngine::run_tile_(const QueryDev& q, const std::vector<LayerPlan>& plan, bool collect_stats, bool ext_beam,
-                              int combine_first, size_t d_begin, size_t d_end) {
+// Runs layers [d_begin, d_end) over one tile of queries; the last layer of the plan writes into `out`.
+void XLinearEngine::run_tile_(const QueryDev& q, const std::vector<LayerPlan>& plan, const OutTarget& out, uint32_t ws_row,
+                              bool collect_stats, bool ext_beam, int combine_first, size_t d_begin, size_t d_end) {
     const uint32_t rows = q.rows;
     if (rows == 0) return;
-    const bool dense = (q.row_ptr == nullptr);
     int cur = static_cast<int>(d_begin & 1);  // every layer flips the ping-pong beam buffers once
     if (!ext_beam && d_begin == 0) {
-        xl_init_beam_kernel<<<(rows + 255) / 256, 256, 0, stream_>>>(bid_(cur), bval_(cur),
-                                                                     bcnt_(cur), beam_stride_, rows);
+        xl_init_beam_kernel<<<(rows + 255) / 256, 256, 0, stream_>>>(bid_(cur, ws_row), bval_(cur, ws_row),
+                                                                     bcnt_(cur, ws_row), beam_stride_, rows);
         ++launches_;
     }
     const size_t depth = plan.size();
@@ -1264,31 +1265,19 @@ void XLinearEngine::run_tile_(const QueryDev& q, const std::vector<LayerPlan>& p
         const int combine = (d == 0) ? combine_first : 1;
         const uint32_t c_stride = std::max<uint32_t>(L.c_max, 1u);
         const uint64_t cand_stride_q = static_cast<uint64_t>(lp.b_prev) * c_stride;
+        const float* cand = cand_.get() + ws_row * cand_stride_q;
+        const uint32_t* bid = bid_(cur, ws_row);
+        const float* bval = bval_(cur, ws_row);
+        const uint32_t* bcnt = bcnt_(cur, ws_row);
         unsigned long long* stats = collect_stats ? stats_dev_.get() + 8 * d : nullptr;
         if (profile_) PB200_CUDA(cudaEventRecord(ev_[0], stream_));
         const dim3 grid(rows);
-        const bool chunk_major = score_layer_(d, q, lp.b_prev, cur, collect_stats) == 4;
-        (void)chunk_major;
+        score_layer_(d, q, lp.b_prev, cur, ws_row, collect_stats);
         if (profile_) PB200_CUDA(cudaEventRecord(ev_[1], stream_));
 
-        const bool last = (d + 1 == depth);
-        uint32_t* o_id; float* o_val; uint32_t* o_cnt; uint32_t o_stride;
-        unsigned long long* o_key = nullptr;
-        if (last && shard_run_) {  // index-sharded run: the local top-k, with keys, to be packed into exchange records
-            o_id = shard_ids_.get() + static_cast<uint64_t>(res_rows_) * res_stride_;
-            o_val = shard_vals_.get() + static_cast<uint64_t>(res_rows_) * res_stride_;
-            o_cnt = shard_cnt_.get() + res_rows_;
-            o_key = shard_keys_.get() + static_cast<uint64_t>(res_rows_) * res_stride_;
-            o_stride = res_stride_;
-        } else if (last) {
-            o_id = res_ids_dev_.get() + static_cast<uint64_t>(res_rows_) * res_stride_;
-            o_val = res_vals_dev_.get() + static_cast<uint64_t>(res_rows_) * res_stride_;
-            o_cnt = res_cnt_dev_.get() + res_rows_;
-            o_stride = res_stride_;
-        } else {
-            o_id = bid_(cur ^ 1); o_val = bval_(cur ^ 1); o_cnt = bcnt_(cur ^ 1);
-            o_stride = beam_stride_;
-        }
+        const OutTarget o = (d + 1 == depth) ? out
+                                             : OutTarget{bid_(cur ^ 1, ws_row), bval_(cur ^ 1, ws_row), bcnt_(cur ^ 1, ws_row),
+                                                         nullptr, beam_stride_};
         const uint64_t sort_stride = next_pow2_host(cand_stride_q);
         const bool warp_select = !force_block_topk_ && lp.b_prev <= static_cast<uint32_t>(kSelSlots) &&
                                  cand_stride_q <= static_cast<uint64_t>(kSelKeysMax) && lp.k <= static_cast<uint32_t>(kSelK);
@@ -1301,19 +1290,19 @@ void XLinearEngine::run_tile_(const QueryDev& q, const std::vector<LayerPlan>& p
             const uint32_t key_cap = static_cast<uint32_t>((cand_stride_q + 127) & ~static_cast<uint64_t>(127));
             const size_t flt_smem = kFltWarps * flt_warp_bytes(key_cap);
             xl_topk_filter_kernel<<<(rows + kFltWarps - 1) / kFltWarps, kFltWarps * 32, flt_smem, stream_>>>(
-                L, lp.pp.kind, lp.pp.p, combine, lp.k, bid_(cur), bval_(cur), bcnt_(cur),
-                beam_stride_, cand_at_(cand_stride_q), cand_stride_q, o_id, o_val, o_cnt, o_stride, rows, stats, o_key, key_cap);
+                L, lp.pp.kind, lp.pp.p, combine, lp.k, bid, bval, bcnt,
+                beam_stride_, cand, cand_stride_q, o.ids, o.vals, o.cnt, o.stride, rows, stats, o.keys, key_cap);
         } else if (warp_select) {
             const uint32_t key_cap = static_cast<uint32_t>((cand_stride_q + 31) & ~static_cast<uint64_t>(31));
             const size_t sel_smem = kSelWarps * ((sel_warp_bytes(key_cap) + 15) & ~static_cast<size_t>(15));
             xl_topk_warp_kernel<<<(rows + kSelWarps - 1) / kSelWarps, kSelWarps * 32, sel_smem, stream_>>>(
-                L, lp.pp.kind, lp.pp.p, combine, lp.k, bid_(cur), bval_(cur), bcnt_(cur),
-                beam_stride_, cand_at_(cand_stride_q), cand_stride_q, c_stride, o_id, o_val, o_cnt, o_stride, rows, stats, o_key, key_cap);
+                L, lp.pp.kind, lp.pp.p, combine, lp.k, bid, bval, bcnt,
+                beam_stride_, cand, cand_stride_q, c_stride, o.ids, o.vals, o.cnt, o.stride, rows, stats, o.keys, key_cap);
         } else {
             xl_topk_kernel<<<grid, kTopkThreads, topk_kernel_smem(lp.b_prev), stream_>>>(
-                L, lp.pp.kind, lp.pp.p, combine, lp.k, bid_(cur), bval_(cur), bcnt_(cur),
-                beam_stride_, cand_at_(cand_stride_q), cand_stride_q, c_stride, o_id, o_val, o_cnt, o_stride, sortbuf_.get(), sort_stride,
-                lp.b_prev, stats, o_key);
+                L, lp.pp.kind, lp.pp.p, combine, lp.k, bid, bval, bcnt,
+                beam_stride_, cand, cand_stride_q, c_stride, o.ids, o.vals, o.cnt, o.stride, sortbuf_.get(), sort_stride,
+                lp.b_prev, stats, o.keys);
         }
         PB200_CUDA(cudaGetLastError());
         ++launches_;
@@ -1352,29 +1341,76 @@ XLinearEngine::Result XLinearEngine::finish_result_(uint32_t rows, uint32_t stri
     return r;
 }
 
-XLinearEngine::Result XLinearEngine::predict_csr(const uint64_t* row_ptr, const uint32_t* col_idx, const float* val,
-                                                 uint32_t rows, uint32_t cols, uint32_t beam_size,
-                                                 const char* post_processor, uint32_t only_topk) {
-    PB200_CUDA(cudaSetDevice(device_));
-    const auto plan = make_plan_(beam_size, post_processor, only_topk);
-    const uint32_t tile = pick_tile_rows_(plan, rows);
-    ensure_workspace_(plan, tile);
-    const uint32_t stride = plan.back().k_cap;
-    res_stride_ = stride;
+XLinearEngine::OutTarget XLinearEngine::reserve_results_(uint32_t rows, uint32_t stride) {
     res_ids_dev_.reserve(static_cast<uint64_t>(rows) * stride + 1);
     res_vals_dev_.reserve(static_cast<uint64_t>(rows) * stride + 1);
     res_cnt_dev_.reserve(static_cast<uint64_t>(rows) + 1);
-    // Whole batch fits the workspace (the common case): the rows are uploaded in `parts` chunks on the copy stream into ONE
-    // staging set; the UPPER layers (cheap) run per chunk as it lands, overlapping the rest of the upload, and the LAST layer
-    // -- where the time goes, and where the chunk-major kernel wants as many pairs per launch as it can get -- runs once over
-    // the whole batch.
-    if (pipeline_uploads_ && rows >= 4096u && tile >= rows) {
+    return OutTarget{res_ids_dev_.get(), res_vals_dev_.get(), res_cnt_dev_.get(), nullptr, stride};
+}
+
+void XLinearEngine::for_each_tile_(uint32_t tile, const HostMatrix* x, const TileFn& run) {
+    const uint32_t rows = x ? x->rows : resident_.rows;
+    for (uint32_t r0 = 0; r0 < rows; r0 += tile) {
+        const uint32_t tr = std::min(tile, rows - r0);
+        QueryDev q = resident_;
+        if (!x) {
+            q.row_ptr = resident_.row_ptr + r0;
+            q.rows = tr;
+        } else if (x->dense) {
+            x_val_.upload(x->dense + static_cast<uint64_t>(r0) * x->cols, static_cast<uint64_t>(tr) * x->cols, stream_);
+            q = QueryDev{nullptr, nullptr, x_val_.get(), 0, tr, x->cols, x->cols};
+        } else {
+            const uint64_t base = x->row_ptr[r0], end = x->row_ptr[r0 + tr];
+            x_row_ptr_.upload(x->row_ptr + r0, static_cast<uint64_t>(tr) + 1, stream_);
+            x_col_idx_.upload(x->col_idx + base, end - base, stream_);
+            x_val_.upload(x->val + base, end - base, stream_);
+            q = QueryDev{x_row_ptr_.get(), x_col_idx_.get(), x_val_.get(), base, tr, x->cols, max_row_nnz(x->row_ptr + r0, tr)};
+        }
+        run(q, r0);
+    }
+}
+
+void XLinearEngine::stage_beam_(uint32_t rows, bool with_vals, const BeamFn& fill) {
+    PB200_CUDA(cudaStreamSynchronize(stream_));  // the pinned staging area may still feed the previous copy
+    const uint64_t n = static_cast<uint64_t>(rows) * beam_stride_;
+    beam_id_host_.reserve(n + 1);
+    if (with_vals) beam_val_host_.reserve(n + 1);
+    beam_cnt_host_.reserve(static_cast<uint64_t>(rows) + 1);
+    for (uint32_t r = 0; r < rows; ++r) {
+        const uint64_t o = static_cast<uint64_t>(r) * beam_stride_;
+        beam_cnt_host_.get()[r] = fill(r, beam_id_host_.get() + o, with_vals ? beam_val_host_.get() + o : nullptr);
+    }
+    PB200_CUDA(cudaMemcpyAsync(beam_id_[0].get(), beam_id_host_.get(), n * 4, cudaMemcpyHostToDevice, stream_));
+    if (with_vals) PB200_CUDA(cudaMemcpyAsync(beam_val_[0].get(), beam_val_host_.get(), n * 4, cudaMemcpyHostToDevice, stream_));
+    PB200_CUDA(cudaMemcpyAsync(beam_cnt_[0].get(), beam_cnt_host_.get(), static_cast<uint64_t>(rows) * 4, cudaMemcpyHostToDevice, stream_));
+}
+
+XLinearEngine::Result XLinearEngine::predict(const HostMatrix& x, uint32_t beam_size, const char* post_processor, uint32_t only_topk) {
+    PB200_CUDA(cudaSetDevice(device_));
+    const auto plan = make_plan_(beam_size, post_processor, only_topk);
+    const uint32_t rows = x.rows, cols = x.cols, stride = plan.back().k_cap;
+    const OutTarget out = reserve_results_(rows, stride);
+    if (x.dense) {
+        for_each_tile_(ensure_workspace_(plan, rows, cols), &x,
+                       [&](const QueryDev& q, uint32_t r0) { run_tile_(q, plan, out.at(r0)); });
+        return finish_result_(rows, stride);
+    }
+    // CSR: the uploads overlap the scoring.  Batches of >= 4096 rows are cut into sub-tiles of about a quarter of the batch.
+    const uint64_t* row_ptr = x.row_ptr;
+    const uint32_t* col_idx = x.col_idx;
+    const float* val = x.val;
+    const uint32_t tile = ensure_workspace_(plan, rows, 0);
+    const uint32_t part = ((rows + 3u) / 4u + 31u) & ~31u;
+    // Whole batch fits the workspace (the common case): the sub-tiles are uploaded on the copy stream into ONE staging set;
+    // the UPPER layers (cheap) run per sub-tile as it lands, overlapping the rest of the upload, and the LAST layer -- where
+    // the time goes, and where the chunk-major kernel wants as many pairs per launch as it can get -- runs once over the
+    // whole batch.
+    if (rows >= 4096u && tile >= rows) {
         const size_t depth = plan.size();
         const uint64_t nnz0 = row_ptr[0], nnz = row_ptr[rows] - nnz0;
         x_row_ptr_.reserve(static_cast<uint64_t>(rows) + 1);
         x_col_idx_.reserve(nnz);
         x_val_.reserve(nnz);
-        const uint32_t part = ((rows + pipeline_parts_ - 1u) / pipeline_parts_ + 31u) & ~31u;
         std::vector<cudaEvent_t> evs;
         for (uint32_t r0 = 0; r0 < rows; r0 += part) {
             const uint32_t tr = std::min(part, rows - r0);
@@ -1393,26 +1429,18 @@ XLinearEngine::Result XLinearEngine::predict_csr(const uint64_t* row_ptr, const 
             PB200_CUDA(cudaStreamWaitEvent(stream_, evs[t], 0));
             if (depth > 1) {
                 QueryDev q{x_row_ptr_.get() + r0, x_col_idx_.get(), x_val_.get(), nnz0, tr, cols, max_row_nnz(row_ptr + r0, tr)};
-                row_off_ = r0;
-                res_rows_ = r0;
-                run_tile_(q, plan, false, false, 0, 0, depth - 1);
+                run_tile_(q, plan, out.at(r0), r0, false, false, 0, 0, depth - 1);
             }
         }
-        row_off_ = 0;
-        res_rows_ = 0;
         QueryDev q{x_row_ptr_.get(), x_col_idx_.get(), x_val_.get(), nnz0, rows, cols, max_row_nnz(row_ptr, rows)};
-        run_tile_(q, plan, false, false, 0, depth - 1, depth);
+        run_tile_(q, plan, out, 0, false, false, 0, depth - 1, depth);
         Result r = finish_result_(rows, stride);
         for (auto ev : evs) cudaEventDestroy(ev);
         return r;
     }
-    // Host buffers: the batch is cut into sub-tiles whose uploads (copy stream, two staging sets) overlap the scoring of
-    // the previous sub-tile; results stay on the device until the last sub-tile is done.
-    uint32_t sub = tile;
-    if (pipeline_uploads_ && rows >= 4096u) {
-        const uint32_t part = ((rows + pipeline_parts_ - 1u) / pipeline_parts_ + 31u) & ~31u;
-        sub = std::min(tile, std::max<uint32_t>(1024u, part));
-    }
+    // Otherwise the sub-tiles' uploads (copy stream, two staging sets) overlap the scoring of the previous sub-tile; results
+    // stay on the device until the last sub-tile is done.
+    const uint32_t sub = rows >= 4096u ? std::min(tile, std::max<uint32_t>(1024u, part)) : tile;
     uint64_t max_nnz = 0;
     for (uint32_t r0 = 0; r0 < rows; r0 += sub) max_nnz = std::max(max_nnz, row_ptr[r0 + std::min(sub, rows - r0)] - row_ptr[r0]);
     DeviceBuffer<uint64_t>* s_rp[2] = {&x_row_ptr_, &x2_row_ptr_};
@@ -1439,128 +1467,61 @@ XLinearEngine::Result XLinearEngine::predict_csr(const uint64_t* row_ptr, const 
             PB200_CUDA(cudaStreamWaitEvent(stream_, up_ev_[b], 0));
         }
         QueryDev q{s_rp[b]->get(), s_ci[b]->get(), s_va[b]->get(), base, tr, cols, max_row_nnz(row_ptr + r0, tr)};
-        res_rows_ = r0;
-        run_tile_(q, plan, false);
+        run_tile_(q, plan, out.at(r0));
         if (two_sets) PB200_CUDA(cudaEventRecord(use_ev_[b], stream_));
     }
     return finish_result_(rows, stride);
 }
 
-XLinearEngine::Result XLinearEngine::predict_drm(const float* dense, uint32_t rows, uint32_t cols, uint32_t beam_size,
-                                                 const char* post_processor, uint32_t only_topk) {
-    PB200_CUDA(cudaSetDevice(device_));
-    const auto plan = make_plan_(beam_size, post_processor, only_topk);
-    uint32_t tile = pick_tile_rows_(plan, rows);
-    const uint64_t max_dense_rows = std::max<uint64_t>(1, (4ull << 30) / (static_cast<uint64_t>(std::max<uint32_t>(cols, 1u)) * 4));
-    tile = static_cast<uint32_t>(std::min<uint64_t>(tile, max_dense_rows));
-    ensure_workspace_(plan, tile);
-    const uint32_t stride = plan.back().k_cap;
-    res_stride_ = stride;
-    res_ids_dev_.reserve(static_cast<uint64_t>(rows) * stride + 1);
-    res_vals_dev_.reserve(static_cast<uint64_t>(rows) * stride + 1);
-    res_cnt_dev_.reserve(static_cast<uint64_t>(rows) + 1);
-    for (uint32_t r0 = 0; r0 < rows; r0 += tile) {
-        const uint32_t tr = std::min(tile, rows - r0);
-        x_val_.upload(dense + static_cast<uint64_t>(r0) * cols, static_cast<uint64_t>(tr) * cols, stream_);
-        QueryDev q{nullptr, nullptr, x_val_.get(), 0, tr, cols, cols};
-        res_rows_ = r0;
-        run_tile_(q, plan, false);
-        if (r0 + tr < rows) PB200_CUDA(cudaStreamSynchronize(stream_));
-    }
-    return finish_result_(rows, stride);
-}
-
-XLinearEngine::Result XLinearEngine::predict_single_layer(const uint64_t* row_ptr, const uint32_t* col_idx, const float* val,
-                                                          const float* dense, uint32_t rows, uint32_t cols,
-                                                          const uint64_t* codes_row_ptr, const uint32_t* codes_col_idx,
-                                                          const float* codes_val, const char* post_processor,
+XLinearEngine::Result XLinearEngine::predict_single_layer(const HostMatrix& x, const HostMatrix& codes, const char* post_processor,
                                                           uint32_t only_topk) {
     PB200_CUDA(cudaSetDevice(device_));
     if (host_->layers.size() != 1) throw std::runtime_error("pecos_b200: predict_single_layer needs a one-layer model");
     const auto& HL = host_->layers[0];
-    const bool have_codes = codes_row_ptr != nullptr;
+    const uint32_t rows = x.rows;
+    const bool have_codes = codes.row_ptr != nullptr;
     // beam entering the layer: the given previous prediction, or every parent with value 1 (libpecos.cpp:209-219)
     uint32_t b_prev = have_codes ? 1u : std::max<uint32_t>(HL.n_chunks, 1u);
     if (have_codes) {
         for (uint32_t r = 0; r < rows; ++r)
-            b_prev = std::max<uint32_t>(b_prev, static_cast<uint32_t>(std::min<uint64_t>(codes_row_ptr[r + 1] - codes_row_ptr[r], 0xFFFFFFFFull)));
-        const uint64_t n = codes_row_ptr[rows] - codes_row_ptr[0];
+            b_prev = std::max<uint32_t>(b_prev, static_cast<uint32_t>(std::min<uint64_t>(codes.row_ptr[r + 1] - codes.row_ptr[r], 0xFFFFFFFFull)));
+        const uint64_t n = codes.row_ptr[rows] - codes.row_ptr[0];
         for (uint64_t i = 0; i < n; ++i)
-            if (codes_col_idx[codes_row_ptr[0] + i] >= HL.n_chunks)
+            if (codes.col_idx[codes.row_ptr[0] + i] >= HL.n_chunks)
                 throw std::runtime_error("pecos_b200: csr_codes column index >= C.cols");
     }
-    std::vector<LayerPlan> plan(1);
-    plan[0].k = only_topk;  // only_topk_to_use = overridden > 0 ? overridden : metadata.only_topk, both = this argument
-    plan[0].pp = parse_post_processor(post_processor ? post_processor : HL.post_processor_name.c_str());
-    plan[0].b_prev = b_prev;
-    const uint64_t cand_max = static_cast<uint64_t>(b_prev) * std::max<uint32_t>(HL.c_max, 1u);
-    plan[0].k_cap = static_cast<uint32_t>(std::max<uint64_t>(1, std::min<uint64_t>(only_topk, cand_max)));
-    if (topk_kernel_smem(b_prev) > 200u * 1024u || b_prev > 32768u)
-        throw std::runtime_error("pecos_b200: beam of " + std::to_string(b_prev) + " nodes exceeds the supported maximum");
+    // only_topk_to_use = overridden > 0 ? overridden : metadata.only_topk, both = this argument
+    const auto plan = make_plan_(0, post_processor, only_topk, {b_prev});
     const uint32_t stride = plan[0].k_cap;
-    res_stride_ = stride;
-    res_ids_dev_.reserve(static_cast<uint64_t>(rows) * stride + 1);
-    res_vals_dev_.reserve(static_cast<uint64_t>(rows) * stride + 1);
-    res_cnt_dev_.reserve(static_cast<uint64_t>(rows) + 1);
+    const OutTarget out = reserve_results_(rows, stride);
     if (only_topk == 0) {  // sorted_csr keeps min(nnz, 0) entries per row (inference.hpp:1237)
         if (rows) PB200_CUDA(cudaMemsetAsync(res_cnt_dev_.get(), 0, static_cast<uint64_t>(rows) * 4, stream_));
         return finish_result_(rows, stride);
     }
-    uint32_t tile = pick_tile_rows_(plan, rows);
-    if (dense) {
-        const uint64_t max_dense_rows = std::max<uint64_t>(1, (4ull << 30) / (static_cast<uint64_t>(std::max<uint32_t>(cols, 1u)) * 4));
-        tile = static_cast<uint32_t>(std::min<uint64_t>(tile, max_dense_rows));
-    }
-    ensure_workspace_(plan, tile);
-    beam_id_host_.reserve(static_cast<uint64_t>(tile) * beam_stride_ + 1);
-    beam_val_host_.reserve(static_cast<uint64_t>(tile) * beam_stride_ + 1);
-    beam_cnt_host_.reserve(static_cast<uint64_t>(tile) + 1);
-    for (uint32_t r0 = 0; r0 < rows; r0 += tile) {
-        const uint32_t tr = std::min(tile, rows - r0);
-        for (uint32_t r = 0; r < tr; ++r) {
-            uint32_t* ids = beam_id_host_.get() + static_cast<uint64_t>(r) * beam_stride_;
-            float* vals = beam_val_host_.get() + static_cast<uint64_t>(r) * beam_stride_;
+    for_each_tile_(ensure_workspace_(plan, rows, x.dense ? x.cols : 0u), &x, [&](const QueryDev& q, uint32_t r0) {
+        stage_beam_(q.rows, true, [&](uint32_t r, uint32_t* ids, float* vals) {
             if (have_codes) {
-                const uint64_t b = codes_row_ptr[r0 + r], e = codes_row_ptr[r0 + r + 1];
-                const uint32_t n = static_cast<uint32_t>(e - b);
-                std::memcpy(ids, codes_col_idx + b, static_cast<size_t>(n) * 4);
-                std::memcpy(vals, codes_val + b, static_cast<size_t>(n) * 4);
-                beam_cnt_host_.get()[r] = n;
-            } else {
-                for (uint32_t j = 0; j < HL.n_chunks; ++j) { ids[j] = j; vals[j] = 1.0f; }
-                beam_cnt_host_.get()[r] = HL.n_chunks;
+                const uint64_t b = codes.row_ptr[r0 + r], e = codes.row_ptr[r0 + r + 1];
+                std::memcpy(ids, codes.col_idx + b, (e - b) * 4);
+                std::memcpy(vals, codes.val + b, (e - b) * 4);
+                return static_cast<uint32_t>(e - b);
             }
-        }
-        PB200_CUDA(cudaMemcpyAsync(beam_id_[0].get(), beam_id_host_.get(), static_cast<uint64_t>(tr) * beam_stride_ * 4, cudaMemcpyHostToDevice, stream_));
-        PB200_CUDA(cudaMemcpyAsync(beam_val_[0].get(), beam_val_host_.get(), static_cast<uint64_t>(tr) * beam_stride_ * 4, cudaMemcpyHostToDevice, stream_));
-        PB200_CUDA(cudaMemcpyAsync(beam_cnt_[0].get(), beam_cnt_host_.get(), static_cast<uint64_t>(tr) * 4, cudaMemcpyHostToDevice, stream_));
-        QueryDev q{};
-        if (dense) {
-            x_val_.upload(dense + static_cast<uint64_t>(r0) * cols, static_cast<uint64_t>(tr) * cols, stream_);
-            q = QueryDev{nullptr, nullptr, x_val_.get(), 0, tr, cols, cols};
-        } else {
-            const uint64_t base = row_ptr[r0], end = row_ptr[r0 + tr];
-            x_row_ptr_.upload(row_ptr + r0, static_cast<uint64_t>(tr) + 1, stream_);
-            x_col_idx_.upload(col_idx + base, end - base, stream_);
-            x_val_.upload(val + base, end - base, stream_);
-            q = QueryDev{x_row_ptr_.get(), x_col_idx_.get(), x_val_.get(), base, tr, cols, max_row_nnz(row_ptr + r0, tr)};
-        }
-        res_rows_ = r0;
-        run_tile_(q, plan, false, /*ext_beam=*/true, /*combine_first=*/have_codes ? 1 : 0);
-        PB200_CUDA(cudaStreamSynchronize(stream_));  // the pinned beam staging area is refilled by the next tile
-    }
+            for (uint32_t j = 0; j < HL.n_chunks; ++j) { ids[j] = j; vals[j] = 1.0f; }
+            return HL.n_chunks;
+        });
+        run_tile_(q, plan, out.at(r0), 0, false, /*ext_beam=*/true, /*combine_first=*/have_codes ? 1 : 0);
+    });
     return finish_result_(rows, stride);
 }
 
-void XLinearEngine::resident_upload_csr(const uint64_t* row_ptr, const uint32_t* col_idx, const float* val, uint32_t rows,
-                                        uint32_t cols) {
+void XLinearEngine::resident_upload_csr(const HostMatrix& x) {
     PB200_CUDA(cudaSetDevice(device_));
-    const uint64_t nnz = row_ptr[rows];
-    x_row_ptr_.upload(row_ptr, static_cast<uint64_t>(rows) + 1, stream_);
-    x_col_idx_.upload(col_idx, nnz, stream_);
-    x_val_.upload(val, nnz, stream_);
+    const uint64_t nnz = x.row_ptr[x.rows];
+    x_row_ptr_.upload(x.row_ptr, static_cast<uint64_t>(x.rows) + 1, stream_);
+    x_col_idx_.upload(x.col_idx, nnz, stream_);
+    x_val_.upload(x.val, nnz, stream_);
     PB200_CUDA(cudaStreamSynchronize(stream_));
-    resident_ = QueryDev{x_row_ptr_.get(), x_col_idx_.get(), x_val_.get(), 0, rows, cols, max_row_nnz(row_ptr, rows)};
+    resident_ = QueryDev{x_row_ptr_.get(), x_col_idx_.get(), x_val_.get(), 0, x.rows, x.cols, max_row_nnz(x.row_ptr, x.rows)};
     has_resident_ = true;
 }
 
@@ -1568,32 +1529,19 @@ double XLinearEngine::resident_predict(uint32_t beam_size, const char* post_proc
     if (!has_resident_) throw std::runtime_error("pecos_b200: no resident query batch uploaded");
     PB200_CUDA(cudaSetDevice(device_));
     const auto plan = make_plan_(beam_size, post_processor, only_topk);
-    const uint32_t rows = resident_.rows;
-    const uint32_t tile = pick_tile_rows_(plan, rows);
-    ensure_workspace_(plan, tile);
-    const uint32_t stride = plan.back().k_cap;
-    res_stride_ = stride;
-    res_ids_dev_.reserve(static_cast<uint64_t>(rows) * stride + 1);
-    res_vals_dev_.reserve(static_cast<uint64_t>(rows) * stride + 1);
-    res_cnt_dev_.reserve(static_cast<uint64_t>(rows) + 1);
+    resident_stride_ = plan.back().k_cap;
+    const OutTarget out = reserve_results_(resident_.rows, resident_stride_);
+    const uint32_t tile = ensure_workspace_(plan, resident_.rows, 0);
     if (collect_stats) PB200_CUDA(cudaMemsetAsync(stats_dev_.get(), 0, stats_dev_.bytes(), stream_));
     PB200_CUDA(cudaEventRecord(ev_[3], stream_));
     cudaEvent_t stop;
     PB200_CUDA(cudaEventCreate(&stop));
-    for (uint32_t r0 = 0; r0 < rows; r0 += tile) {
-        const uint32_t tr = std::min(tile, rows - r0);
-        QueryDev q = resident_;
-        q.row_ptr = resident_.row_ptr + r0;
-        q.rows = tr;
-        res_rows_ = r0;
-        run_tile_(q, plan, collect_stats);
-    }
+    for_each_tile_(tile, nullptr, [&](const QueryDev& q, uint32_t r0) { run_tile_(q, plan, out.at(r0), 0, collect_stats); });
     PB200_CUDA(cudaEventRecord(stop, stream_));
     PB200_CUDA(cudaEventSynchronize(stop));
     float ms = 0.f;
     PB200_CUDA(cudaEventElapsedTime(&ms, ev_[3], stop));
     cudaEventDestroy(stop);
-    res_rows_ = rows;
     if (collect_stats) {
         std::vector<unsigned long long> h(8 * layers_.size());
         PB200_CUDA(cudaMemcpy(h.data(), stats_dev_.get(), h.size() * 8, cudaMemcpyDeviceToHost));
@@ -1607,39 +1555,20 @@ double XLinearEngine::resident_predict(uint32_t beam_size, const char* post_proc
     return static_cast<double>(ms);
 }
 
-uint32_t XLinearEngine::sharded_local_csr_packed(const uint64_t* row_ptr, const uint32_t* col_idx, const float* val, uint32_t rows,
-                                                 uint32_t cols, uint32_t beam_size, const char* post_processor, uint32_t only_topk,
+uint32_t XLinearEngine::sharded_local_csr_packed(const HostMatrix& x, uint32_t beam_size, const char* post_processor, uint32_t only_topk,
                                                  uint32_t stride_capacity, void* rec_dev) {
     PB200_CUDA(cudaSetDevice(device_));
     const auto plan = make_plan_(beam_size, post_processor, only_topk);
-    const uint32_t stride = plan.back().k_cap;
+    const uint32_t rows = x.rows, stride = plan.back().k_cap;
     if (stride > stride_capacity) throw std::runtime_error("pecos_b200: sharded output buffers are too narrow for this top-k");
-    const uint32_t tile = pick_tile_rows_(plan, rows);
-    ensure_workspace_(plan, tile);
     const uint64_t n = static_cast<uint64_t>(rows) * stride;
     shard_keys_.reserve(n + 1);
     shard_ids_.reserve(n + 1);
     shard_vals_.reserve(n + 1);
     shard_cnt_.reserve(static_cast<uint64_t>(rows) + 1);
-    res_stride_ = stride;
-    shard_run_ = true;
-    try {
-        for (uint32_t r0 = 0; r0 < rows; r0 += tile) {
-            const uint32_t tr = std::min(tile, rows - r0);
-            const uint64_t base = row_ptr[r0], end = row_ptr[r0 + tr];
-            x_row_ptr_.upload(row_ptr + r0, static_cast<uint64_t>(tr) + 1, stream_);
-            x_col_idx_.upload(col_idx + base, end - base, stream_);
-            x_val_.upload(val + base, end - base, stream_);
-            QueryDev q{x_row_ptr_.get(), x_col_idx_.get(), x_val_.get(), base, tr, cols, max_row_nnz(row_ptr + r0, tr)};
-            res_rows_ = r0;
-            run_tile_(q, plan, false);
-            PB200_CUDA(cudaStreamSynchronize(stream_));
-        }
-    } catch (...) {
-        shard_run_ = false;
-        throw;
-    }
-    shard_run_ = false;
+    const OutTarget out{shard_ids_.get(), shard_vals_.get(), shard_cnt_.get(), shard_keys_.get(), stride};
+    for_each_tile_(ensure_workspace_(plan, rows, 0), &x,
+                   [&](const QueryDev& q, uint32_t r0) { run_tile_(q, plan, out.at(r0)); });
     if (n) {
         xl_shard_pack_kernel<<<static_cast<uint32_t>((n + 255) / 256), 256, 0, stream_>>>(
             shard_keys_.get(), shard_ids_.get(), shard_vals_.get(), shard_cnt_.get(), rows, stride, static_cast<ShardRecord*>(rec_dev));
@@ -1657,13 +1586,10 @@ XLinearEngine::Result XLinearEngine::sharded_merge_packed(uint32_t world, uint32
         throw std::runtime_error("pecos_b200: world * top-k exceeds the merge kernel's capacity");
     const uint32_t k = only_topk ? only_topk : static_cast<uint32_t>(host_->layers.back().only_topk);
     const uint32_t k_out = std::min<uint32_t>(k, world * stride);
-    res_stride_ = k_out;
-    res_ids_dev_.reserve(static_cast<uint64_t>(rows) * k_out + 1);
-    res_vals_dev_.reserve(static_cast<uint64_t>(rows) * k_out + 1);
-    res_cnt_dev_.reserve(static_cast<uint64_t>(rows) + 1);
+    const OutTarget out = reserve_results_(rows, k_out);
     if (rows) {
         xl_merge_packed_kernel<<<(rows + kSelWarps - 1) / kSelWarps, kSelWarps * 32, 0, stream_>>>(
-            static_cast<const ShardRecord*>(g_rec), world, rows, stride, k_out, res_ids_dev_.get(), res_vals_dev_.get(), res_cnt_dev_.get());
+            static_cast<const ShardRecord*>(g_rec), world, rows, stride, k_out, out.ids, out.vals, out.cnt);
         PB200_CUDA(cudaGetLastError());
         ++launches_;
     }
@@ -1672,12 +1598,234 @@ XLinearEngine::Result XLinearEngine::sharded_merge_packed(uint32_t world, uint32
 
 XLinearEngine::Result XLinearEngine::resident_fetch() {
     PB200_CUDA(cudaSetDevice(device_));
-    return finish_result_(resident_.rows, res_stride_);
+    return finish_result_(resident_.rows, resident_stride_);
 }
 
-#define PB200_SELECTED_ENGINE
-#include "xlinear_selected.cuh"
-#undef PB200_SELECTED_ENGINE
+// predict_on_selected_outputs on the device (SURVEY 8f-2).
+//
+// Replaces HierarchicalMLModel::predict_on_selected_outputs (pecos/core/xmc/inference.hpp:2507-2571), per layer
+// MLModel::predict_on_selected_outputs_internal (:2129-2180) with prolongate_sparse_predictions (:1302-1358); C ABI
+// c_xlinear_predict_on_selected_outputs_{csr,drm}_f32 (pecos/core/libpecos.cpp:179-198).
+//
+// What the reference computes: the scores of exactly the given (query, label) pairs pushed through the hierarchy, no
+// top-k.  The selected set of layer l-1 is the SORTED set of parents of layer l's selected set; a row of layer l holds,
+// for every entry of the previous layer's row IN ORDER, its children in C's column order that belong to the layer's
+// selected set; value = transform(raw score) combined with the parent's value (not at layer 0).
+//
+// Split used here: everything STRUCTURAL (selected sets, entry order, which candidate position and which parent entry an
+// entry reads) depends only on C and the selected pattern, so the host computes it per query; the device does the
+// arithmetic with the SAME validated score kernels as beam search -- the previous layer's entry list plays the beam's
+// role, so cand[] holds every child of every listed parent in prolongation order -- followed by one small gather kernel
+// (xl_selected_gather_kernel: transform + combine of the selected candidates).  Raw scores are therefore bit-identical
+// to predict()'s.
+XLinearEngine::SelectedResult XLinearEngine::predict_selected(const HostMatrix& x, const HostMatrix& sel, const char* post_processor,
+                                                              const HostMatrix& codes) {
+    PB200_CUDA(cudaSetDevice(device_));
+    // codes (single-layer handles only, c_mlmodel_predict_on_selected_outputs_*): the previous layer's prediction; its
+    // rows replace the root as the first layer's parent list and its values are combined with the first layer's scores
+    const bool have_codes = codes.row_ptr != nullptr;
+    if (have_codes && layers_.size() != 1) throw std::runtime_error("pecos_b200: csr_codes needs a one-layer model");
+    const size_t depth = layers_.size();
+    const auto& HL = host_->layers;
+    const uint32_t rows = x.rows;
+    const uint64_t* sel_ptr = sel.row_ptr;
+    const uint32_t* sel_idx = sel.col_idx;
+    if (sel.cols != HL.back().out_cols) throw std::runtime_error("pecos_b200: selected_outputs_csr.cols != nr_labels");
+    if (sel_index_.empty()) {  // label (original numbering of the layer) -> the chunk (= parent node) and column offset that holds it
+        sel_index_.resize(depth);
+        for (size_t d = 0; d < depth; ++d) {
+            const auto& L = HL[d];
+            SelIndex& ix = sel_index_[d];
+            ix.chunk_of_label.assign(L.out_cols, 0xFFFFFFFFu);  // 0xFFFFFFFF: the label has no parent (pruned tree)
+            ix.offset_of_label.assign(L.out_cols, 0u);
+            for (uint32_t p = 0; p < L.n_chunks; ++p) {
+                const ChunkHeader& h = L.chunks[p];
+                for (uint32_t j = 0; j < h.n_cols; ++j) {
+                    const uint32_t col = h.col_begin + j;
+                    const uint32_t label = L.reordered ? L.label_of_col[col] : col;
+                    if (label < L.out_cols) { ix.chunk_of_label[label] = p; ix.offset_of_label[label] = j; }
+                }
+            }
+        }
+    }
+    SelectedResult out;
+    out.rows = rows;
+    out.cols = sel.cols;
+    out.indptr.assign(sel_ptr, sel_ptr + rows + 1);
+    const uint64_t sel_base = sel_ptr[0];
+    for (auto& v : out.indptr) v -= sel_base;
+    const uint64_t total = out.indptr[rows];
+    out.indices.assign(total, 0u);
+    out.data.assign(total, 0.0f);
+    if (rows == 0) return out;
+
+    // ---- structure, per query (host threads): entry lists of every layer
+    struct Lists {
+        std::vector<uint64_t> ptr;       // [rows + 1]
+        std::vector<uint32_t> id;        // label of the entry (original numbering of the layer)
+        std::vector<uint32_t> pos;       // candidate position inside the query's row of this layer
+        std::vector<uint32_t> parent;    // index of the parent entry inside the query's row of the previous layer
+    };
+    std::vector<Lists> lists(depth);
+    {
+        std::vector<std::vector<uint32_t>> q_id(static_cast<size_t>(rows) * depth), q_pos(static_cast<size_t>(rows) * depth),
+            q_par(static_cast<size_t>(rows) * depth);
+        const unsigned hw = std::max(1u, std::min(32u, std::thread::hardware_concurrency()));
+        const unsigned n_thr = static_cast<unsigned>(std::min<uint64_t>(hw, std::max<uint64_t>(1, rows / 64)));
+        std::vector<std::thread> pool;
+        std::atomic<uint32_t> next{0};
+        std::vector<std::exception_ptr> errs(n_thr);
+        auto work = [&](unsigned t) {
+            try {
+                std::vector<std::vector<uint32_t>> sel(depth);
+                for (;;) {
+                    const uint32_t q0 = next.fetch_add(64);
+                    if (q0 >= rows) break;
+                    for (uint32_t q = q0; q < std::min(rows, q0 + 64); ++q) {
+                        // selected sets, leaf upwards (sorted, unique)
+                        sel[depth - 1].assign(sel_idx + sel_ptr[q], sel_idx + sel_ptr[q + 1]);
+                        for (uint32_t lab : sel[depth - 1])
+                            if (lab >= HL.back().out_cols) throw std::runtime_error("pecos_b200: selected label id out of range");
+                        std::sort(sel[depth - 1].begin(), sel[depth - 1].end());
+                        for (size_t d = depth - 1; d > 0; --d) {
+                            auto& up = sel[d - 1];
+                            up.clear();
+                            for (uint32_t lab : sel[d]) {
+                                const uint32_t par = sel_index_[d].chunk_of_label[lab];
+                                if (par != 0xFFFFFFFFu) up.push_back(par);
+                            }
+                            std::sort(up.begin(), up.end());
+                            up.erase(std::unique(up.begin(), up.end()), up.end());
+                        }
+                        // entry lists, root downwards; first parent list: the given codes row, else every code of the first
+                        // layer (= the root for a hierarchical model; ones(rows x nr_codes) for a single layer, libpecos.cpp:96-99)
+                        std::vector<uint32_t> prev_id;
+                        if (have_codes) prev_id.assign(codes.col_idx + codes.row_ptr[q], codes.col_idx + codes.row_ptr[q + 1]);
+                        else { prev_id.resize(HL[0].n_chunks); for (uint32_t p = 0; p < HL[0].n_chunks; ++p) prev_id[p] = p; }
+                        for (size_t d = 0; d < depth; ++d) {
+                            auto& ids = q_id[static_cast<size_t>(q) * depth + d];
+                            auto& pos = q_pos[static_cast<size_t>(q) * depth + d];
+                            auto& par = q_par[static_cast<size_t>(q) * depth + d];
+                            const auto& L = HL[d];
+                            const auto& S = sel[d];
+                            uint32_t slot_base = 0;
+                            for (uint32_t i = 0; i < prev_id.size(); ++i) {
+                                const uint32_t p = prev_id[i];
+                                if (p >= L.n_chunks) throw std::runtime_error("pecos_b200: selected outputs: parent id out of range");
+                                const ChunkHeader& h = L.chunks[p];
+                                for (uint32_t j = 0; j < h.n_cols; ++j) {
+                                    const uint32_t col = h.col_begin + j;
+                                    const uint32_t label = L.reordered ? L.label_of_col[col] : col;
+                                    if (ids.size() >= S.size() || !std::binary_search(S.begin(), S.end(), label)) continue;
+                                    ids.push_back(label);
+                                    pos.push_back(slot_base + j);
+                                    par.push_back(i);
+                                }
+                                slot_base += h.n_cols;
+                            }
+                            prev_id = ids;
+                        }
+                    }
+                }
+            } catch (...) { errs[t] = std::current_exception(); }
+        };
+        for (unsigned t = 1; t < n_thr; ++t) pool.emplace_back(work, t);
+        work(0);
+        for (auto& th : pool) th.join();
+        for (auto& e : errs) if (e) std::rethrow_exception(e);
+        for (size_t d = 0; d < depth; ++d) {
+            auto& Ls = lists[d];
+            Ls.ptr.assign(static_cast<size_t>(rows) + 1, 0);
+            for (uint32_t q = 0; q < rows; ++q) Ls.ptr[q + 1] = Ls.ptr[q] + q_id[static_cast<size_t>(q) * depth + d].size();
+            Ls.id.resize(Ls.ptr[rows]);
+            Ls.pos.resize(Ls.ptr[rows]);
+            Ls.parent.resize(Ls.ptr[rows]);
+            for (uint32_t q = 0; q < rows; ++q) {
+                const size_t k = static_cast<size_t>(q) * depth + d;
+                std::copy(q_id[k].begin(), q_id[k].end(), Ls.id.begin() + Ls.ptr[q]);
+                std::copy(q_pos[k].begin(), q_pos[k].end(), Ls.pos.begin() + Ls.ptr[q]);
+                std::copy(q_par[k].begin(), q_par[k].end(), Ls.parent.begin() + Ls.ptr[q]);
+            }
+        }
+    }
+
+    // ---- plan: the beam entering layer d is the entry list of layer d - 1 (layer 0: the codes rows, else every parent)
+    std::vector<uint32_t> b_in(depth, 1u);
+    for (size_t d = 0; d < depth; ++d) {
+        uint32_t& b = b_in[d];
+        if (d > 0)
+            for (uint32_t q = 0; q < rows; ++q) b = std::max<uint32_t>(b, static_cast<uint32_t>(lists[d - 1].ptr[q + 1] - lists[d - 1].ptr[q]));
+        else if (have_codes)
+            for (uint32_t q = 0; q < rows; ++q) b = std::max<uint32_t>(b, static_cast<uint32_t>(codes.row_ptr[q + 1] - codes.row_ptr[q]));
+        else
+            b = std::max<uint32_t>(1u, HL[0].n_chunks);
+    }
+    const auto plan = make_plan_(1, post_processor, 1, b_in, /*topk=*/false);
+
+    DeviceBuffer<uint64_t> d_ptr[2];
+    DeviceBuffer<uint32_t> d_pos, d_par;
+    DeviceBuffer<float> d_val[2];
+    std::vector<uint64_t> rel_ptr;
+    std::vector<float> leaf_vals;
+    for_each_tile_(ensure_workspace_(plan, rows, x.dense ? x.cols : 0u), &x, [&](const QueryDev& qd, uint32_t r0) {
+        const uint32_t tr = qd.rows;
+        int cur = 0;  // which d_ptr / d_val set holds the previous layer
+        if (have_codes) {  // the given previous prediction plays "layer -1"
+            const uint64_t c0 = codes.row_ptr[r0], c1 = codes.row_ptr[r0 + tr];
+            rel_ptr.resize(static_cast<size_t>(tr) + 1);
+            for (uint32_t r = 0; r <= tr; ++r) rel_ptr[r] = codes.row_ptr[r0 + r] - c0;
+            d_ptr[cur].upload(rel_ptr.data(), rel_ptr.size(), stream_);
+            d_val[cur].upload(codes.val + c0, c1 - c0, stream_);
+        }
+        for (size_t d = 0; d < depth; ++d) {
+            // beam = the previous layer's entry list (layer 0: the codes rows, else every parent); also waits for the
+            // previous layer, whose uploads came from rel_ptr
+            stage_beam_(tr, false, [&](uint32_t r, uint32_t* ids, float*) {
+                const uint64_t* ptr = d > 0 ? lists[d - 1].ptr.data() : have_codes ? codes.row_ptr : nullptr;
+                if (!ptr) {
+                    for (uint32_t p = 0; p < HL[0].n_chunks; ++p) ids[p] = p;
+                    return HL[0].n_chunks;
+                }
+                const uint64_t b = ptr[r0 + r], n = ptr[r0 + r + 1] - b;
+                std::memcpy(ids, (d > 0 ? lists[d - 1].id.data() : codes.col_idx) + b, n * 4);
+                return static_cast<uint32_t>(n);
+            });
+            score_layer_(d, qd, plan[d].b_prev, 0, 0, false);
+            const auto& Ls = lists[d];
+            const uint64_t e0 = Ls.ptr[r0], e1 = Ls.ptr[r0 + tr];
+            rel_ptr.resize(static_cast<size_t>(tr) + 1);
+            for (uint32_t r = 0; r <= tr; ++r) rel_ptr[r] = Ls.ptr[r0 + r] - e0;
+            const int nxt = cur ^ 1;
+            d_ptr[nxt].upload(rel_ptr.data(), rel_ptr.size(), stream_);
+            d_pos.upload(Ls.pos.data() + e0, e1 - e0, stream_);
+            d_par.upload(Ls.parent.data() + e0, e1 - e0, stream_);
+            d_val[nxt].reserve(std::max<uint64_t>(e1 - e0, 1));
+            const uint64_t cand_stride_q = static_cast<uint64_t>(plan[d].b_prev) * std::max<uint32_t>(layers_[d].view.c_max, 1u);
+            xl_selected_gather_kernel<<<tr, 128, 0, stream_>>>(cand_.get(), cand_stride_q, d_ptr[nxt].get(), d_pos.get(), d_par.get(),
+                                                             d_ptr[cur].get(), d_val[cur].get(), d_val[nxt].get(), plan[d].pp.kind,
+                                                             plan[d].pp.p, (d > 0 || have_codes) ? 1 : 0);
+            PB200_CUDA(cudaGetLastError());
+            ++launches_;
+            cur = nxt;
+        }
+        // leaf values of this tile -> result rows (the reference copies the selected row's LENGTH; entries it could not reach
+        // -- labels without a path to the root -- stay zero, inference.hpp:2560-2568)
+        const auto& Lf = lists[depth - 1];
+        const uint64_t e0 = Lf.ptr[r0], e1 = Lf.ptr[r0 + tr];
+        leaf_vals.resize(e1 - e0);
+        PB200_CUDA(cudaStreamSynchronize(stream_));
+        if (e1 > e0) PB200_CUDA(cudaMemcpy(leaf_vals.data(), d_val[cur].get(), (e1 - e0) * 4, cudaMemcpyDeviceToHost));
+        for (uint32_t r = 0; r < tr; ++r) {
+            const uint64_t ob = out.indptr[r0 + r], on = out.indptr[r0 + r + 1] - ob;
+            const uint64_t lb = Lf.ptr[r0 + r], ln = Lf.ptr[r0 + r + 1] - lb;
+            for (uint64_t i = 0; i < std::min(on, ln); ++i) {
+                out.indices[ob + i] = Lf.id[lb + i];
+                out.data[ob + i] = leaf_vals[lb - e0 + i];
+            }
+        }
+    });
+    return out;
+}
 
 }  // namespace pb200
 

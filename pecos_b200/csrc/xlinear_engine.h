@@ -10,6 +10,7 @@
 //     reorder_prediction ................ :1919-1923   (label_of_col lookup in xl_topk_kernel)
 #pragma once
 
+#include <functional>
 #include <memory>
 #include <string>
 #include <vector>
@@ -60,6 +61,17 @@ struct QueryDev {
     uint32_t max_row_nnz;     // longest row of the batch (sizes the shared-memory staging of the query)
 };
 
+// Host view of a caller's matrix (queries, codes or a selected-outputs pattern): CSR (row_ptr/col_idx/val, absolute
+// offsets) or row-major dense (dense).  An empty HostMatrix stands for "not given".
+struct HostMatrix {
+    const uint64_t* row_ptr = nullptr;
+    const uint32_t* col_idx = nullptr;
+    const float* val = nullptr;
+    const float* dense = nullptr;
+    uint32_t rows = 0;
+    uint32_t cols = 0;
+};
+
 struct XLinearStats {  // algorithmic-byte counters of SURVEY.md section 8(d), accumulated by the STATS kernel variant
     unsigned long long chunks;      // (query, chunk) products evaluated
     unsigned long long chunk_rows;  // sum R_p
@@ -95,35 +107,29 @@ public:
         const uint32_t* cnt = nullptr;
     };
 
-    // Host-buffer entry points (H2D + kernels + D2H inside). Exactly one of (row_ptr/col_idx/val) or dense is used.
-    Result predict_csr(const uint64_t* row_ptr, const uint32_t* col_idx, const float* val, uint32_t rows, uint32_t cols,
-                       uint32_t beam_size, const char* post_processor, uint32_t only_topk);
-    Result predict_drm(const float* dense, uint32_t rows, uint32_t cols, uint32_t beam_size, const char* post_processor,
-                       uint32_t only_topk);
+    // Host-buffer entry points (H2D + kernels + D2H inside).
+    Result predict(const HostMatrix& x, uint32_t beam_size, const char* post_processor, uint32_t only_topk);
 
     // One layer of the python prediction chain (c_xlinear_single_layer_predict_*, pecos/core/libpecos.cpp:201-235): the
-    // engine must hold a one-layer model.  Queries: CSR (row_ptr != nullptr) or row-major dense.  codes_*: the previous
-    // layer's prediction as CSR rows x n_chunks, consumed in stored order (nullptr: ones(rows x n_chunks), no combine).
-    Result predict_single_layer(const uint64_t* row_ptr, const uint32_t* col_idx, const float* val, const float* dense,
-                                uint32_t rows, uint32_t cols, const uint64_t* codes_row_ptr, const uint32_t* codes_col_idx,
-                                const float* codes_val, const char* post_processor, uint32_t only_topk);
+    // engine must hold a one-layer model.  codes: the previous layer's prediction as CSR rows x n_chunks, consumed in stored
+    // order (no row_ptr: ones(rows x n_chunks), no combine).
+    Result predict_single_layer(const HostMatrix& x, const HostMatrix& codes, const char* post_processor, uint32_t only_topk);
 
     // predict_on_selected_outputs (c_xlinear_predict_on_selected_outputs_*, pecos/core/libpecos.cpp:179-198): scores of exactly
-    // the (query, label) pairs of the CSR pattern `sel_*` (rows x nr_labels), pushed through the hierarchy, no top-k.
-    // Result rows have the selected rows' lengths; entry order = the reference's (see xlinear_selected.cuh).
+    // the (query, label) pairs of the CSR pattern `sel` (rows x nr_labels), pushed through the hierarchy, no top-k.
+    // Result rows have the selected rows' lengths; entry order = the reference's (see predict_selected in xlinear_engine.cu).
+    // codes (one-layer models only): as for predict_single_layer.
     struct SelectedResult {
         uint32_t rows = 0, cols = 0;
         std::vector<uint64_t> indptr;
         std::vector<uint32_t> indices;
         std::vector<float> data;
     };
-    SelectedResult predict_selected(const uint64_t* row_ptr, const uint32_t* col_idx, const float* val, const float* dense,
-                                    uint32_t rows, uint32_t cols, const uint64_t* sel_ptr, const uint32_t* sel_idx,
-                                    uint32_t sel_cols, const char* post_processor, const uint64_t* codes_ptr = nullptr,
-                                    const uint32_t* codes_idx = nullptr, const float* codes_val = nullptr);
+    SelectedResult predict_selected(const HostMatrix& x, const HostMatrix& sel, const char* post_processor,
+                                    const HostMatrix& codes = {});
 
     // Device-resident queries (bench "value" leg: inputs already in HBM when the timed region starts).
-    void resident_upload_csr(const uint64_t* row_ptr, const uint32_t* col_idx, const float* val, uint32_t rows, uint32_t cols);
+    void resident_upload_csr(const HostMatrix& x);
     // Runs all layers over the resident batch; results stay in HBM (fetch with resident_fetch). Returns device ms.
     double resident_predict(uint32_t beam_size, const char* post_processor, uint32_t only_topk, bool collect_stats);
     Result resident_fetch();
@@ -133,9 +139,8 @@ public:
     // as 16-byte {u64 key, u32 id, f32 value} records [rows][stride] (key == 0: empty slot), so the exchange is a single
     // all-gather; returns the stride used.  sharded_merge_packed reduces the gathered [world][rows][stride] records to the
     // global top-k.
-    uint32_t sharded_local_csr_packed(const uint64_t* row_ptr, const uint32_t* col_idx, const float* val, uint32_t rows, uint32_t cols,
-                                      uint32_t beam_size, const char* post_processor, uint32_t only_topk, uint32_t stride_capacity,
-                                      void* rec_dev);
+    uint32_t sharded_local_csr_packed(const HostMatrix& x, uint32_t beam_size, const char* post_processor, uint32_t only_topk,
+                                      uint32_t stride_capacity, void* rec_dev);
     Result sharded_merge_packed(uint32_t world, uint32_t rows, uint32_t stride, uint32_t only_topk, const void* g_rec);
 
     void set_profile(bool on) { profile_ = on; }
@@ -169,18 +174,46 @@ private:
         LayerDev view{};
     };
 
-    std::vector<LayerPlan> make_plan_(uint32_t beam_size, const char* post_processor, uint32_t only_topk) const;
-    void ensure_workspace_(const std::vector<LayerPlan>& plan, uint32_t tile_rows);
-    uint32_t pick_tile_rows_(const std::vector<LayerPlan>& plan, uint32_t rows) const;
-    // layers [d_begin, d_end) over one tile of queries; the tile's beam / candidate rows start at row_off_ of the workspace
-    void run_tile_(const QueryDev& q, const std::vector<LayerPlan>& plan, bool collect_stats, bool ext_beam = false,
-                   int combine_first = 0, size_t d_begin = 0, size_t d_end = static_cast<size_t>(-1));
-    uint32_t* bid_(int b) const { return beam_id_[b].get() + static_cast<uint64_t>(row_off_) * beam_stride_; }
-    float* bval_(int b) const { return beam_val_[b].get() + static_cast<uint64_t>(row_off_) * beam_stride_; }
-    uint32_t* bcnt_(int b) const { return beam_cnt_[b].get() + row_off_; }
-    float* cand_at_(uint64_t stride_q) const { return cand_.get() + static_cast<uint64_t>(row_off_) * stride_q; }
-    uint32_t row_off_ = 0;
-    int score_layer_(size_t d, const QueryDev& q, uint32_t b_prev, int cur, bool collect_stats);
+    // Where the last layer of a tile writes its top-k: rows [0, tile) of these arrays (keys only in an index-sharded run).
+    struct OutTarget {
+        uint32_t* ids;
+        float* vals;
+        uint32_t* cnt;
+        unsigned long long* keys;
+        uint32_t stride;
+        OutTarget at(uint32_t row) const {
+            const uint64_t o = static_cast<uint64_t>(row) * stride;
+            return {ids + o, vals + o, cnt + row, keys ? keys + o : nullptr, stride};
+        }
+    };
+    using TileFn = std::function<void(const QueryDev& q, uint32_t r0)>;
+    using BeamFn = std::function<uint32_t(uint32_t row, uint32_t* ids, float* vals)>;
+
+    // b_in[d] (where given and > 0): the beam capacity entering layer d, set by the caller (single layer: the codes rows or
+    // every parent; selected outputs: the previous layer's entry lists); otherwise the previous layer's k_cap (root: 1).
+    // topk = false: no top-k kernel runs on the plan (selected outputs).
+    std::vector<LayerPlan> make_plan_(uint32_t beam_size, const char* post_processor, uint32_t only_topk,
+                                      const std::vector<uint32_t>& b_in = {}, bool topk = true) const;
+    // Sizes the tiles of a `rows`-query call so that the workspace of one tile stays within PB200_WORKSPACE_MB, allocates
+    // that workspace and returns the tile's rows.  dense_cols > 0: dense queries, whose staged tile is also capped at 4 GiB.
+    uint32_t ensure_workspace_(const std::vector<LayerPlan>& plan, uint32_t rows, uint32_t dense_cols);
+    // Tiled pass over the queries x (host CSR or dense; nullptr: the resident batch) in tiles of `tile` rows (from
+    // ensure_workspace_): stages every tile on the device and calls run(q, first row of the tile).
+    void for_each_tile_(uint32_t tile, const HostMatrix* x, const TileFn& run);
+    // The beam entering the first layer of a tile (rows [0, rows) of beam_*_[0]), from fill(row, ids, vals) = its length;
+    // vals is nullptr unless with_vals.
+    void stage_beam_(uint32_t rows, bool with_vals, const BeamFn& fill);
+    // Layers [d_begin, d_end) over one tile of queries whose beam / candidate rows start at row ws_row of the workspace.
+    // ext_beam: beam_*_[0] already hold the beam entering the first layer; combine_first: that layer combines its scores
+    // with the beam values (single layer with a given previous prediction).
+    void run_tile_(const QueryDev& q, const std::vector<LayerPlan>& plan, const OutTarget& out, uint32_t ws_row = 0,
+                   bool collect_stats = false, bool ext_beam = false, int combine_first = 0, size_t d_begin = 0,
+                   size_t d_end = static_cast<size_t>(-1));
+    uint32_t* bid_(int b, uint32_t row) const { return beam_id_[b].get() + static_cast<uint64_t>(row) * beam_stride_; }
+    float* bval_(int b, uint32_t row) const { return beam_val_[b].get() + static_cast<uint64_t>(row) * beam_stride_; }
+    uint32_t* bcnt_(int b, uint32_t row) const { return beam_cnt_[b].get() + row; }
+    int score_layer_(size_t d, const QueryDev& q, uint32_t b_prev, int cur, uint32_t ws_row, bool collect_stats);
+    OutTarget reserve_results_(uint32_t rows, uint32_t stride);
     Result finish_result_(uint32_t rows, uint32_t stride);
 
     struct SelIndex {  // per layer: label -> (chunk, column offset); built on the first predict_selected call
@@ -201,35 +234,31 @@ private:
     DeviceBuffer<float> cand_;
     DeviceBuffer<unsigned long long> sortbuf_;
     DeviceBuffer<unsigned long long> stats_dev_;
-    int final_buf_ = 0;  // which ping-pong buffer holds the last layer's output
     uint32_t beam_stride_ = 0;
 
     // staged inputs (host-buffer path) and resident batch
     DeviceBuffer<uint64_t> x_row_ptr_;
     DeviceBuffer<uint32_t> x_col_idx_;
     DeviceBuffer<float> x_val_;
-    // second staging set + copy stream: predict_csr uploads sub-tile t+1 while sub-tile t is being scored
+    // second staging set + copy stream: predict() uploads sub-tile t+1 of a CSR batch while sub-tile t is being scored
     DeviceBuffer<uint64_t> x2_row_ptr_;
     DeviceBuffer<uint32_t> x2_col_idx_;
     DeviceBuffer<float> x2_val_;
     cudaStream_t copy_stream_ = nullptr;
     cudaEvent_t up_ev_[2] = {nullptr, nullptr};   // staging set uploaded
     cudaEvent_t use_ev_[2] = {nullptr, nullptr};  // staging set consumed by the score kernels
-    bool pipeline_uploads_ = true;
-    PinnedBuffer<uint32_t> beam_id_host_;   // single-layer entry point: the given beam, staged per tile
+    PinnedBuffer<uint32_t> beam_id_host_;   // stage_beam_: the given beam, staged per tile
     PinnedBuffer<float> beam_val_host_;
     PinnedBuffer<uint32_t> beam_cnt_host_;
-    uint32_t pipeline_parts_ = 4;
     QueryDev resident_{};
     bool has_resident_ = false;
     DeviceBuffer<uint32_t> res_ids_dev_;
     DeviceBuffer<float> res_vals_dev_;
     DeviceBuffer<uint32_t> res_cnt_dev_;
-    uint32_t res_rows_ = 0, res_stride_ = 0;
+    uint32_t resident_stride_ = 0;  // top-k stride of the last resident_predict
     DeviceBuffer<unsigned long long> shard_keys_;  // local top-k of an index-sharded run before packing
     DeviceBuffer<uint32_t> shard_ids_, shard_cnt_;
     DeviceBuffer<float> shard_vals_;
-    bool shard_run_ = false;  // the last layer writes into shard_*_ (inside sharded_local_csr_packed)
 
     // host result staging (pinned)
     PinnedBuffer<uint32_t> out_ids_;

@@ -1,6 +1,6 @@
 """GPU parity tests for c_xlinear_predict_on_selected_outputs_{csr,drm}_f32 (pecos/core/libpecos.cpp:179-198; SURVEY 8f-2).
 
-CUDA path (pecos_b200/csrc/xlinear_selected.cuh) vs the C restatement (pinned bit-for-bit against the reference library in
+CUDA path (XLinearEngine::predict_selected in pecos_b200/csrc/xlinear_engine.cu) vs the C restatement (pinned bit-for-bit against the reference library in
 tests/test_oracle_cpu.py) and, where oracle/_ref is present, vs the reference library itself (CSC handle).  Bar: same entry
 order and label ids, scores 1e-5 relative.  Mirrors test/pecos/xmc/xlinear/test_xlinear.py:1059-1137.
 """
