@@ -265,6 +265,22 @@ void pb200_hnsw_get_counters(void* model_ptr, uint64_t* out);
 /* sparse (csr) indices: resident csr batch; stored entries (8 bytes each) of the base rows evaluated by the last search */
 void pb200_hnsw_resident_upload_csr(void* model_ptr, const ScipyCsrF32* pX);
 uint64_t pb200_hnsw_sparse_entries(void* model_ptr);
+/* HNSW index sharding (pecos_b200.hnsw_build.build_hnsw_shards: one independent index per contiguous row range, one process
+ * per GPU).  model_ptr is a c_ann_hnsw_load_* handle of this rank's shard; only its primary engine is used.
+ *   local:  searches the shard and writes its top-k as 16-byte records {u64 key, u32 id, f32 value}[rows][topk] into the
+ *           CALLER-OWNED DEVICE buffer rec_dev (the send buffer of ONE all-gather).  id = id_offset + local id (the shard's
+ *           first global row), value = distance, key = (~orderable(distance) << 32) | ~(rank * topk + slot); key 0 marks an
+ *           empty slot.  Requires (rank + 1) * topk <= 1024.
+ *   merge:  gathered [world][rows][topk] records g_rec -> ret_idx / ret_val [rows][topk] (host), ordered by distance, then
+ *           shard rank, then slot; rows with fewer than topk results end in zeros, like c_ann_hnsw_predict_*.
+ *           Requires world * topk <= 1024.
+ * The result equals, bit for bit, the merge by that order of the per-shard c_ann_hnsw_predict_* results. */
+void pb200_hnsw_sharded_local_packed_drm(void* model_ptr, const ScipyDrmF32* pX, uint32_t efS, uint32_t topk, uint32_t rank,
+                                         uint32_t id_offset, void* rec_dev);
+void pb200_hnsw_sharded_local_packed_csr(void* model_ptr, const ScipyCsrF32* pX, uint32_t efS, uint32_t topk, uint32_t rank,
+                                         uint32_t id_offset, void* rec_dev);
+void pb200_hnsw_sharded_merge_packed(void* model_ptr, uint32_t world, uint32_t rows, uint32_t topk, const void* g_rec,
+                                     uint32_t* ret_idx, float* ret_val);
 /* libpecos.cpp:482-490  c_ann_hnsw_save_drm_{ip,l2}_f32(model_ptr, model_dir): for an index loaded by THIS library the saved
  * form is what it was loaded from (config.json + index.mmap_store are copied to model_dir).
  *

@@ -466,6 +466,12 @@ class B200CoreLib(object):
         fp(c.pb200_hnsw_sparse_entries, c_uint64, [c_void_p])
         fp(c.pb200_hnsw_resident_predict, c_double, [c_void_p, c_uint32, c_uint32])
         fp(c.pb200_hnsw_resident_fetch, None, [c_void_p, POINTER(c_uint32), POINTER(c_float)])
+        fp(c.pb200_hnsw_sharded_local_packed_drm, None, [c_void_p, POINTER(ScipyDrmF32), c_uint32, c_uint32, c_uint32, c_uint32,
+                                                         c_void_p])
+        fp(c.pb200_hnsw_sharded_local_packed_csr, None, [c_void_p, POINTER(ScipyCsrF32), c_uint32, c_uint32, c_uint32, c_uint32,
+                                                         c_void_p])
+        fp(c.pb200_hnsw_sharded_merge_packed, None, [c_void_p, c_uint32, c_uint32, c_uint32, c_void_p, POINTER(c_uint32),
+                                                     POINTER(c_float)])
         fp(c.pb200_hnsw_get_counters, None, [c_void_p, POINTER(c_uint64)])
         fp(c.pb200_hnsw_set_stages, c_int, [c_void_p, c_int])
         fp(c.pb200_hnsw_get_info, None, [c_void_p, POINTER(c_uint64)])

@@ -1092,6 +1092,32 @@ void pb200_hnsw_resident_fetch(void* model_ptr, uint32_t* ret_idx, float* ret_va
     PB200_API_END("pb200_hnsw_resident_fetch")
 }
 
+// index sharding: the handle's primary engine holds one shard (PB200_DEVICES replicas are not used)
+void pb200_hnsw_sharded_local_packed_drm(void* model_ptr, const ScipyDrmF32* pX, uint32_t efS, uint32_t topk, uint32_t rank,
+                                         uint32_t id_offset, void* rec_dev) {
+    PB200_API_BEGIN
+    PB200_LOCK_HNSW(model_ptr)
+    hnsw_of(model_ptr).sharded_local_packed(pX->val, pX->rows, pX->cols, efS, topk, rank, id_offset, rec_dev);
+    PB200_API_END("pb200_hnsw_sharded_local_packed_drm")
+}
+
+void pb200_hnsw_sharded_local_packed_csr(void* model_ptr, const ScipyCsrF32* pX, uint32_t efS, uint32_t topk, uint32_t rank,
+                                         uint32_t id_offset, void* rec_dev) {
+    PB200_API_BEGIN
+    PB200_LOCK_HNSW(model_ptr)
+    hnsw_of(model_ptr).sharded_local_packed_csr(pX->row_ptr, pX->col_idx, pX->val, pX->rows, pX->cols, efS, topk, rank, id_offset,
+                                                rec_dev);
+    PB200_API_END("pb200_hnsw_sharded_local_packed_csr")
+}
+
+void pb200_hnsw_sharded_merge_packed(void* model_ptr, uint32_t world, uint32_t rows, uint32_t topk, const void* g_rec,
+                                     uint32_t* ret_idx, float* ret_val) {
+    PB200_API_BEGIN
+    PB200_LOCK_HNSW(model_ptr)
+    hnsw_of(model_ptr).sharded_merge_packed(world, rows, topk, g_rec, ret_idx, ret_val);
+    PB200_API_END("pb200_hnsw_sharded_merge_packed")
+}
+
 int pb200_hnsw_set_stages(void* model_ptr, int stages) {
     PB200_API_BEGIN
     PB200_LOCK_HNSW(model_ptr)

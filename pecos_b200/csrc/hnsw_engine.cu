@@ -20,6 +20,7 @@
 //
 // HBM traffic per query (SURVEY 8d): n_dist * 4d + n_expand * 4(1+maxM0) + hops * 4(1+maxM) + 4d + 8k.
 #include "hnsw_engine.h"
+#include "shard_merge.cuh"
 #include "sparse_distance.cuh"
 
 #include <algorithm>
@@ -532,6 +533,27 @@ hnsw_search_kernel(const HnswDev ix, const float* __restrict__ Q, const HnswSpar
     }
 }
 
+// Index sharding: this shard's [nq][topk] search results -> exchange records.  An empty slot (out_idx == 0xFFFFFFFF, the fill
+// of the sharded path) gets key 0.  key = (~orderable(dist) << 32) | ~(rank * topk + slot): the merge orders by distance
+// ascending, then shard rank, then slot, so one shard's own order (ties included) is kept; the low word is never 0 while
+// (rank + 1) * topk <= kSelKeys.
+__global__ void hnsw_shard_pack_kernel(const uint32_t* __restrict__ idx, const float* __restrict__ val, const uint64_t n,
+                                       const uint32_t topk, const uint32_t rank, const uint32_t id_offset,
+                                       ShardRecord* __restrict__ rec) {
+    const uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint32_t slot = static_cast<uint32_t>(i % topk);
+    const uint32_t id = idx[i];
+    ShardRecord out{0ull, 0u, 0.0f};
+    if (id != 0xFFFFFFFFu) {
+        const float d = val[i];
+        out.key = (static_cast<unsigned long long>(~orderable(d)) << 32) | static_cast<unsigned long long>(~(rank * topk + slot));
+        out.id = id_offset + id;
+        out.val = d;
+    }
+    rec[i] = out;
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -719,7 +741,7 @@ void HnswEngine::ensure_scratch_(uint32_t ef) {
     }
 }
 
-double HnswEngine::launch_once_(const float* q_dev, uint32_t nq, uint32_t efS, uint32_t topk, bool* overflow) {
+double HnswEngine::launch_once_(const float* q_dev, uint32_t nq, uint32_t efS, uint32_t topk, int idx_fill, bool* overflow) {
     const HnswHostIndex& H = *host_;
     const uint32_t ef = std::max(efS, topk);
     if (ef == 0) throw std::runtime_error("pecos_b200: efS and topk are both zero");
@@ -729,7 +751,7 @@ double HnswEngine::launch_once_(const float* q_dev, uint32_t nq, uint32_t efS, u
     const uint32_t per_warp = per_warp_smem_(ef, &nbmax);
     const uint32_t words = static_cast<uint32_t>((static_cast<uint64_t>(H.num_node) + 31) / 32);
     PB200_CUDA(cudaMemsetAsync(ctrl_.get(), 0, 8 * sizeof(unsigned long long), stream_));
-    PB200_CUDA(cudaMemsetAsync(out_idx_.get(), 0, static_cast<uint64_t>(nq) * topk * 4, stream_));
+    PB200_CUDA(cudaMemsetAsync(out_idx_.get(), idx_fill, static_cast<uint64_t>(nq) * topk * 4, stream_));
     PB200_CUDA(cudaMemsetAsync(out_val_.get(), 0, static_cast<uint64_t>(nq) * topk * 4, stream_));
     const uint32_t ctas = std::max<uint32_t>(1, std::min<uint32_t>(n_ctas_, (nq + warps_per_cta_ - 1) / warps_per_cta_));
     const size_t smem = static_cast<size_t>(warps_per_cta_) * per_warp;
@@ -761,10 +783,10 @@ double HnswEngine::launch_once_(const float* q_dev, uint32_t nq, uint32_t efS, u
 // A query whose candidate queue outgrows the per-warp scratch (vcap entries) flags an overflow; the batch is then re-run with
 // twice the capacity (at most num_node + 1 entries, which can never overflow: a node enters the queue at most once), instead
 // of aborting the host process.
-double HnswEngine::launch_(const float* q_dev, uint32_t nq, uint32_t efS, uint32_t topk) {
+double HnswEngine::launch_(const float* q_dev, uint32_t nq, uint32_t efS, uint32_t topk, int idx_fill) {
     for (;;) {
         bool overflow = false;
-        const double ms = launch_once_(q_dev, nq, efS, topk, &overflow);
+        const double ms = launch_once_(q_dev, nq, efS, topk, idx_fill, &overflow);
         if (!overflow) return ms;
         const uint64_t cap_max = static_cast<uint64_t>(host_->num_node) + 1;
         if (vcap_ >= cap_max) throw std::runtime_error("pecos_b200: HNSW candidate queue overflow at full capacity (internal error)");
@@ -857,6 +879,70 @@ void HnswEngine::resident_fetch(uint32_t* ret_idx, float* ret_val) {
     PB200_CUDA(cudaSetDevice(device_));
     PB200_CUDA(cudaMemcpy(ret_idx, out_idx_.get(), static_cast<uint64_t>(res_nq_) * res_topk_ * 4, cudaMemcpyDeviceToHost));
     PB200_CUDA(cudaMemcpy(ret_val, out_val_.get(), static_cast<uint64_t>(res_nq_) * res_topk_ * 4, cudaMemcpyDeviceToHost));
+}
+
+// search into out_idx_ / out_val_ (empty slots 0xFFFFFFFF), then pack the records into the caller's device buffer
+void HnswEngine::shard_pack_(uint32_t nq, uint32_t efS, uint32_t topk, uint32_t rank, uint32_t id_offset, void* rec_dev) {
+    const uint64_t n = static_cast<uint64_t>(nq) * topk;
+    out_idx_.reserve(n);
+    out_val_.reserve(n);
+    launch_(q_dev_.get(), nq, efS, topk, 0xFF);
+    hnsw_shard_pack_kernel<<<static_cast<uint32_t>((n + 255) / 256), 256, 0, stream_>>>(out_idx_.get(), out_val_.get(), n, topk, rank,
+                                                                                      id_offset, static_cast<ShardRecord*>(rec_dev));
+    PB200_CUDA(cudaGetLastError());
+    ++launches_;
+    PB200_CUDA(cudaStreamSynchronize(stream_));
+}
+
+static void check_shard_slots(uint32_t rank, uint32_t topk) {
+    if ((static_cast<uint64_t>(rank) + 1) * topk > static_cast<uint64_t>(kSelKeys))
+        throw std::runtime_error("pecos_b200: (rank + 1) * topk exceeds the shard merge capacity of 1024 records per query");
+}
+
+void HnswEngine::sharded_local_packed(const float* X, uint32_t nq, uint32_t d, uint32_t efS, uint32_t topk, uint32_t rank,
+                                      uint32_t id_offset, void* rec_dev) {
+    PB200_CUDA(cudaSetDevice(device_));
+    if (host_->sparse) throw std::runtime_error("pecos_b200: dense queries against a sparse (csr) HNSW index");
+    if (d != host_->feat_dim) throw std::runtime_error("pecos_b200: query dimension != index dimension");
+    check_shard_slots(rank, topk);
+    if (nq == 0 || topk == 0) return;
+    q_dev_.upload(X, static_cast<uint64_t>(nq) * d, stream_);
+    shard_pack_(nq, efS, topk, rank, id_offset, rec_dev);
+}
+
+void HnswEngine::sharded_local_packed_csr(const uint64_t* row_ptr, const uint32_t* col_idx, const float* val, uint32_t nq,
+                                          uint32_t cols, uint32_t efS, uint32_t topk, uint32_t rank, uint32_t id_offset,
+                                          void* rec_dev) {
+    PB200_CUDA(cudaSetDevice(device_));
+    if (!host_->sparse) throw std::runtime_error("pecos_b200: csr queries against a dense HNSW index");
+    if (cols != host_->feat_dim) throw std::runtime_error("pecos_b200: query dimension != index dimension");
+    check_shard_slots(rank, topk);
+    if (nq == 0 || topk == 0) return;
+    upload_csr_(row_ptr, col_idx, val, nq);
+    shard_pack_(nq, efS, topk, rank, id_offset, rec_dev);
+}
+
+void HnswEngine::sharded_merge_packed(uint32_t world, uint32_t rows, uint32_t topk, const void* g_rec, uint32_t* ret_idx,
+                                      float* ret_val) {
+    PB200_CUDA(cudaSetDevice(device_));
+    if (world == 0) throw std::runtime_error("pecos_b200: world must be >= 1");
+    if (static_cast<uint64_t>(world) * topk > static_cast<uint64_t>(kSelKeys))
+        throw std::runtime_error("pecos_b200: world * topk exceeds the shard merge capacity of 1024 records per query");
+    if (rows == 0 || topk == 0) return;
+    const uint64_t n = static_cast<uint64_t>(rows) * topk;
+    out_idx_.reserve(n);
+    out_val_.reserve(n);
+    merge_cnt_.reserve(rows);
+    // the merge writes each row's first min(topk, records) entries; the tail keeps these zeros (libpecos.cpp:554-558)
+    PB200_CUDA(cudaMemsetAsync(out_idx_.get(), 0, n * 4, stream_));
+    PB200_CUDA(cudaMemsetAsync(out_val_.get(), 0, n * 4, stream_));
+    shard_merge_packed_kernel<<<(rows + kSelWarps - 1) / kSelWarps, kSelWarps * 32, 0, stream_>>>(
+        static_cast<const ShardRecord*>(g_rec), world, rows, topk, topk, out_idx_.get(), out_val_.get(), merge_cnt_.get());
+    PB200_CUDA(cudaGetLastError());
+    ++launches_;
+    PB200_CUDA(cudaMemcpyAsync(ret_idx, out_idx_.get(), n * 4, cudaMemcpyDeviceToHost, stream_));
+    PB200_CUDA(cudaMemcpyAsync(ret_val, out_val_.get(), n * 4, cudaMemcpyDeviceToHost, stream_));
+    PB200_CUDA(cudaStreamSynchronize(stream_));
 }
 
 HnswCounters HnswEngine::counters() {

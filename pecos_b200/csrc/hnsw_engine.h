@@ -66,6 +66,17 @@ public:
     double resident_predict(uint32_t efS, uint32_t topk);  // returns device ms of the search kernel
     void resident_fetch(uint32_t* ret_idx, float* ret_val);
 
+    // Index sharding (one graph per shard, one engine per rank).  sharded_local_packed{,_csr} search this shard and write
+    // [nq][topk] 16-byte ShardRecords (shard_merge.cuh) to the caller-owned device buffer rec_dev:
+    //   key = (~orderable(dist) << 32) | ~(rank * topk + slot), id = id_offset + local id, val = dist; key 0 = empty slot.
+    // sharded_merge_packed merges the all-gathered [world][rows][topk] records into ret arrays rows x topk; rows with fewer
+    // than topk results keep zeros, as in predict.
+    void sharded_local_packed(const float* X, uint32_t nq, uint32_t d, uint32_t efS, uint32_t topk, uint32_t rank,
+                              uint32_t id_offset, void* rec_dev);
+    void sharded_local_packed_csr(const uint64_t* row_ptr, const uint32_t* col_idx, const float* val, uint32_t nq, uint32_t cols,
+                                  uint32_t efS, uint32_t topk, uint32_t rank, uint32_t id_offset, void* rec_dev);
+    void sharded_merge_packed(uint32_t world, uint32_t rows, uint32_t topk, const void* g_rec, uint32_t* ret_idx, float* ret_val);
+
     HnswCounters counters();
     uint64_t launches() const { return launches_; }
     uint32_t vcap_retries() const { return vcap_retries_; }  // batches re-run after a candidate-queue overflow
@@ -78,8 +89,11 @@ public:
 private:
     void ensure_scratch_(uint32_t ef);
     uint32_t per_warp_smem_(uint32_t ef, uint32_t* nbmax_out) const;
-    double launch_(const float* q_dev, uint32_t nq, uint32_t efS, uint32_t topk);
-    double launch_once_(const float* q_dev, uint32_t nq, uint32_t efS, uint32_t topk, bool* overflow);
+    // idx_fill: byte value out_idx_ is filled with before the search (0: the reference's zeros; 0xFF: empty slots read
+    // 0xFFFFFFFF, which no node id can be, for the shard pack kernel)
+    double launch_(const float* q_dev, uint32_t nq, uint32_t efS, uint32_t topk, int idx_fill = 0);
+    double launch_once_(const float* q_dev, uint32_t nq, uint32_t efS, uint32_t topk, int idx_fill, bool* overflow);
+    void shard_pack_(uint32_t nq, uint32_t efS, uint32_t topk, uint32_t rank, uint32_t id_offset, void* rec_dev);
 
     std::unique_ptr<HnswHostIndex> host_;
     int device_ = 0;
@@ -111,6 +125,7 @@ private:
     DeviceBuffer<float> q_dev_;
     DeviceBuffer<uint32_t> out_idx_;
     DeviceBuffer<float> out_val_;
+    DeviceBuffer<uint32_t> merge_cnt_;  // per-query result counts of the shard merge
     uint32_t res_nq_ = 0, res_d_ = 0, res_topk_ = 0;
     PinnedBuffer<uint32_t> stage_idx_;
     PinnedBuffer<float> stage_val_;

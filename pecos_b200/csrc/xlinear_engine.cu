@@ -18,6 +18,7 @@
 // No FMA contraction anywhere on the score path: products use __fmul_rn, sums use __fadd_rn (the reference build has
 // no -march flag, so its XR-Linear loops are scalar mulss/addss).
 #include "xlinear_engine.h"
+#include "shard_merge.cuh"
 
 #include <algorithm>
 #include <atomic>
@@ -631,9 +632,7 @@ xl_topk_kernel(const LayerDev L, const int pp_kind, const int pp_p, const int co
 // Narrow-beam variant: one WARP per query (kSelWarps queries per CTA).  The keys of the <= kSelKeys candidates sit in the
 // warp's shared-memory slice; the top-k is extracted by k rounds of warp arg-max on the 64-bit composite key (keys are
 // unique because they embed the candidate position), the winning lane rescanning only its own stride-32 subset.
-// Same keys, same order, same values as xl_topk_kernel.
-constexpr int kSelWarps = 4;
-constexpr int kSelKeys = 1024;   // merge kernel capacity (static shared memory)
+// Same keys, same order, same values as xl_topk_kernel.  (kSelWarps queries per CTA: shard_merge.cuh.)
 constexpr int kSelKeysMax = 4096; // warp top-k capacity (dynamic shared memory, sized per launch)
 constexpr int kSelSlots = 64;
 constexpr int kSelK = 64;
@@ -797,16 +796,9 @@ xl_selected_gather_kernel(const float* __restrict__ cand, const uint64_t cand_st
     }
 }
 
-// Packed exchange records for index sharding: ONE 16-byte {key, id, value} record per (query, rank) slot, key == 0 marks an
-// empty slot (a valid key is never 0: its low word is ~position), so the per-query counts need not travel: the whole exchange
-// is a single all-gather of one buffer.
-struct __align__(16) ShardRecord {
-    unsigned long long key;
-    uint32_t id;
-    float val;
-};
-static_assert(sizeof(ShardRecord) == 16, "shard record must stay 16 bytes");
-
+// Packed exchange records for index sharding (ShardRecord, shard_merge.cuh): ONE record per (query, rank) slot, key == 0
+// marks an empty slot (a valid key is never 0: its low word is ~position), so the per-query counts need not travel: the
+// whole exchange is a single all-gather of one buffer.
 __global__ void xl_shard_pack_kernel(const unsigned long long* __restrict__ keys, const uint32_t* __restrict__ ids,
                                      const float* __restrict__ vals, const uint32_t* __restrict__ cnt, const uint32_t rows,
                                      const uint32_t stride, ShardRecord* __restrict__ rec) {
@@ -816,57 +808,6 @@ __global__ void xl_shard_pack_kernel(const unsigned long long* __restrict__ keys
     ShardRecord out{0ull, 0u, 0.0f};
     if (r < cnt[q]) { out.key = keys[i]; out.id = ids[i]; out.val = vals[i]; }
     rec[i] = out;
-}
-
-// Merge of the per-GPU top-k records gathered by ONE all-gather ([world][rows][stride]) into the global top-k.  Keys are
-// globally unique (they embed the candidate's position in the full prolongated row), so the merge is an exact arg-max
-// selection: for each output rank, the lane holding the warp's largest key finds its slot and emits that record.
-__global__ void __launch_bounds__(kSelWarps * 32)
-xl_merge_packed_kernel(const ShardRecord* __restrict__ g_rec, const uint32_t world, const uint32_t rows, const uint32_t stride,
-                       const uint32_t k, uint32_t* __restrict__ out_id, float* __restrict__ out_val, uint32_t* __restrict__ out_cnt) {
-    __shared__ unsigned long long s_keys[kSelWarps][kSelKeys];
-    const int lane = threadIdx.x & 31;
-    const int warp = threadIdx.x >> 5;
-    const uint32_t q = blockIdx.x * kSelWarps + warp;
-    if (q >= rows) return;
-    unsigned long long* keys = s_keys[warp];
-    const uint32_t n = world * stride;
-    unsigned long long best = 0ull;
-    uint32_t total = 0;
-    for (uint32_t i = lane; i < n; i += 32) {
-        const uint32_t g = i / stride, r = i - g * stride;
-        const unsigned long long key = g_rec[(static_cast<uint64_t>(g) * rows + q) * stride + r].key;
-        if (key) ++total;
-        keys[i] = key;
-        best = key > best ? key : best;
-    }
-#pragma unroll
-    for (int d = 16; d > 0; d >>= 1) total += __shfl_xor_sync(kFull, total, d);
-    __syncwarp();
-    const uint32_t kk = min(k, total);
-    if (lane == 0) out_cnt[q] = kk;
-    for (uint32_t rnk = 0; rnk < kk; ++rnk) {
-        unsigned long long top = best;
-#pragma unroll
-        for (int d = 16; d > 0; d >>= 1) {
-            const unsigned long long o = __shfl_xor_sync(kFull, top, d);
-            top = o > top ? o : top;
-        }
-        uint32_t slot = 0xFFFFFFFFu;
-        if (best == top) {
-            for (uint32_t i = lane; i < n; i += 32) if (keys[i] == top) { slot = i; break; }
-        }
-        if (slot != 0xFFFFFFFFu) {
-            const uint32_t g = slot / stride, r = slot - g * stride;
-            const ShardRecord rc = g_rec[(static_cast<uint64_t>(g) * rows + q) * stride + r];
-            out_id[static_cast<uint64_t>(q) * k + rnk] = rc.id;
-            out_val[static_cast<uint64_t>(q) * k + rnk] = rc.val;
-            keys[slot] = 0ull;
-            best = 0ull;
-            for (uint32_t i = lane; i < n; i += 32) { const unsigned long long key = keys[i]; best = key > best ? key : best; }
-        }
-        __syncwarp();
-    }
 }
 
 // Row extents as one 8-byte record per chunk row, derived on the device from the row_ptr array of the chunk (the score
@@ -1588,7 +1529,7 @@ XLinearEngine::Result XLinearEngine::sharded_merge_packed(uint32_t world, uint32
     const uint32_t k_out = std::min<uint32_t>(k, world * stride);
     const OutTarget out = reserve_results_(rows, k_out);
     if (rows) {
-        xl_merge_packed_kernel<<<(rows + kSelWarps - 1) / kSelWarps, kSelWarps * 32, 0, stream_>>>(
+        shard_merge_packed_kernel<<<(rows + kSelWarps - 1) / kSelWarps, kSelWarps * 32, 0, stream_>>>(
             static_cast<const ShardRecord*>(g_rec), world, rows, stride, k_out, out.ids, out.vals, out.cnt);
         PB200_CUDA(cudaGetLastError());
         ++launches_;

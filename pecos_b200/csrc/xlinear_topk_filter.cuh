@@ -57,11 +57,7 @@ __device__ __forceinline__ float xl_transform_estimate(float v, int kind, int p)
     }
 }
 
-__device__ __forceinline__ uint32_t xl_orderable(float v) {
-    const uint32_t u = __float_as_uint(v);
-    return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-}
-
+// inverse of orderable (shard_merge.cuh)
 __device__ __forceinline__ float xl_from_orderable(uint32_t o) {
     return __uint_as_float((o & 0x80000000u) ? (o ^ 0x80000000u) : ~o);
 }
@@ -172,7 +168,7 @@ xl_topk_filter_kernel(const LayerDev L, const int pp_kind, const int pp_p, const
                 if (s_colbeg[slot] != 0xFFFFFFFFu) {
                     float s = xl_transform_estimate(r[u], pp_kind, pp_p);
                     if (combine) s = xl_combine(s, s_pval[slot], pp_kind);
-                    key = max(xl_orderable(s), 1u);
+                    key = max(orderable(s), 1u);
                 }
             }
             if (i < n_pad) keys[i] = key;
@@ -193,7 +189,7 @@ xl_topk_filter_kernel(const LayerDev L, const int pp_kind, const int pp_p, const
     uint32_t cut = 1;
     if (tkey != 0) {
         const float T = xl_from_orderable(tkey);
-        if (isfinite(T)) cut = max(xl_orderable(T - (1e-3f * fabsf(T) + 1e-30f)), 1u);
+        if (isfinite(T)) cut = max(orderable(T - (1e-3f * fabsf(T) + 1e-30f)), 1u);
     }
     __syncwarp();
 

@@ -1,6 +1,6 @@
-"""Multi-GPU XR-Linear prediction, one process per GPU (``torch.distributed``; NCCL on GPUs, gloo in CPU tests).
+"""Multi-GPU XR-Linear prediction and HNSW search, one process per GPU (``torch.distributed``; NCCL on GPUs, gloo in CPU tests).
 
-Two layouts (SURVEY.md section 8e):
+Two layouts for XR-Linear (SURVEY.md section 8e):
 
 * **query sharding** -- model replicated, rows of ``X`` split across ranks; no data-path collective
   (:func:`split_rows_by_nnz`, used by ``bench.py`` and by callers that scatter their own batches).
@@ -9,14 +9,20 @@ Two layouts (SURVEY.md section 8e):
   a local top-k as ``(key, label, score)`` with ``key = (orderable(score) << 32) | ~global_position``; ONE all-gather of
   those lists and a merge kernel give the global top-k, bit-identical to the single-GPU result.
 
+HNSW index sharding (:class:`ShardedHNSW`): one independent graph per contiguous row range, each rank searches its own shard
+and keeps its top-k as ``(key, global id, distance)`` with ``key = (~orderable(distance) << 32) | ~(rank * topk + slot)``; the
+same ONE all-gather and merge kernel give the top-k of the union, bit-identical to merging the per-shard searches.
+
 The reference has no inference-time model sharding (its parallelism is OpenMP threads inside one call,
 pecos/core/xmc/inference.hpp:969-1005); this module is the multi-GPU counterpart of that loop.
 """
+import dataclasses as dc
 import json
 import os
-from ctypes import byref, c_uint32, c_void_p
+from ctypes import POINTER, byref, c_float, c_uint32, c_void_p
 
 import numpy as np
+import scipy.sparse as smat
 
 from .core import ScipyCompressedSparseAllocator, ScipyCsrF32, XLINEAR_INFERENCE_MODEL_TYPES, get_clib
 
@@ -120,3 +126,91 @@ class ShardedXLinearModel(object):
         alloc = ScipyCompressedSparseAllocator()
         c.pb200_xlinear_sharded_merge_packed(self.model_chain, self.world, rows, stride, only_topk or 0, g_rec.data_ptr(), alloc.cfunc)
         return alloc.get()
+
+
+class ShardedHNSW(object):
+    """HNSW index sharded by rows (``hnsw_build.build_hnsw_shards``): rank r searches only ``shard-<r>``; ``predict`` returns the
+    same result on every rank.
+
+    The result is NOT the search of one graph over all rows (each shard is its own graph: recall level against it); it is,
+    bit for bit, the merge of the per-shard searches ordered by (distance, shard rank, slot within the shard), with global
+    ids ``row_begin[r] + local id``.  At world 1 it is the unsharded search."""
+
+    MERGE_CAPACITY = 1024  # world * topk records per query (kSelKeys in csrc/shard_merge.cuh)
+
+    def __init__(self, index, manifest, rank, world, comm, clib):
+        self.index = index
+        self.manifest = manifest
+        self.rank, self.world = rank, world
+        self.comm = comm
+        self._clib = clib
+        self.row_begin = [int(b) for b in manifest["row_begin"]]
+        self.num_item, self.feat_dim = int(manifest["num_item"]), int(manifest["feat_dim"])
+        self.data_type, self.metric_type = manifest["data_type"], manifest["metric_type"]
+        self.pred_params = index.PredParams.from_dict(manifest.get("pred_kwargs"))
+        self.last_exchange_bytes = 0
+        self.last_phase_ms = {}
+
+    @classmethod
+    def load(cls, folder, comm=None, device=None):
+        from .hnsw import HNSW
+        from .hnsw_build import SHARDS_MANIFEST
+
+        with open(os.path.join(folder, SHARDS_MANIFEST), "r", encoding="utf-8") as f:
+            manifest = json.load(f)
+        comm = comm or _TorchComm()
+        if int(manifest["world"]) != comm.world:
+            raise ValueError(f"{folder} holds {manifest['world']} shards, the communicator has {comm.world} ranks")
+        clib = get_clib()
+        clib.require_gpu()
+        if device is not None:
+            clib.set_device(device)
+        index = HNSW.load(os.path.join(folder, f"shard-{comm.rank}"))
+        rb = manifest["row_begin"]
+        if index.num_item != rb[comm.rank + 1] - rb[comm.rank] or index.feat_dim != manifest["feat_dim"]:
+            raise ValueError(f"shard-{comm.rank} of {folder} does not match its manifest")
+        return cls(index, manifest, comm.rank, comm.world, comm, clib)
+
+    def get_pred_params(self):
+        return dc.replace(self.pred_params)
+
+    def predict(self, X, pred_params=None, ret_csr=True):
+        """Every rank passes the same ``X``.  Same arguments and return types as ``HNSW.predict``: CSR (rows x num_item,
+        distances as values) or ``(indices, distances)`` arrays rows x topk; slots beyond a row's results hold zeros."""
+        import time
+
+        import torch
+
+        params = pred_params if pred_params is not None else self.get_pred_params()
+        view, kind = self.index.create_pymat(X)
+        if kind != self.data_type:
+            raise ValueError(f"{kind} queries cannot be searched in a {self.data_type} index")
+        if view.cols != self.feat_dim:
+            raise ValueError(f"query dimension {view.cols} != index dimension {self.feat_dim}")
+        n, k = int(view.rows), int(params.topk)
+        if self.world * k > self.MERGE_CAPACITY:
+            raise ValueError(f"world * topk = {self.world * k} exceeds the merge capacity of {self.MERGE_CAPACITY} records per query")
+        idx = np.zeros((n, k), dtype=np.uint32)
+        dist = np.zeros((n, k), dtype=np.float32)
+        if n and k:
+            c = self._clib.clib_float32
+            dev = torch.device("cuda", c.pb200_get_device())
+            # send buffer of the exchange: 16-byte {u64 key, u32 id, f32 distance} records, viewed as int64 pairs for torch
+            rec = torch.empty((n, k, 2), dtype=torch.int64, device=dev)
+            torch.cuda.synchronize(dev)
+            t0 = time.perf_counter()
+            local = c.pb200_hnsw_sharded_local_packed_drm if kind == "drm" else c.pb200_hnsw_sharded_local_packed_csr
+            local(self.index.model_ptr, byref(view), int(params.efS), k, self.rank, self.row_begin[self.rank], rec.data_ptr())
+            t1 = time.perf_counter()
+            g_rec = self.comm.all_gather(rec)  # THE exchange: one all-gather of one buffer
+            torch.cuda.synchronize(dev)
+            t2 = time.perf_counter()
+            c.pb200_hnsw_sharded_merge_packed(self.index.model_ptr, self.world, n, k, g_rec.data_ptr(),
+                                              idx.ctypes.data_as(POINTER(c_uint32)), dist.ctypes.data_as(POINTER(c_float)))
+            t3 = time.perf_counter()
+            self.last_exchange_bytes = int(rec.numel() * 8)
+            self.last_phase_ms = {"local": 1e3 * (t1 - t0), "exchange": 1e3 * (t2 - t1), "merge": 1e3 * (t3 - t2)}
+        if not ret_csr:
+            return idx, dist
+        row_starts = np.arange(n + 1, dtype=np.int64) * k
+        return smat.csr_matrix((dist.ravel(), idx.ravel().astype(np.int64), row_starts), shape=(n, self.num_item), dtype=np.float32)

@@ -38,6 +38,9 @@ Algorithm:
    (sparse GraphL0 records are variable-size FeatVecSparse records located by byte offsets).
 
 torch is used for device memory and the GEMM / top-k primitives; nothing here is on the search path.
+
+``build_hnsw_shards`` splits the rows into contiguous ranges and builds one such index per range (an index larger than one GPU,
+built in parallel on several); ``pecos_b200.distributed.ShardedHNSW`` searches it.
 """
 import contextlib
 import json
@@ -363,6 +366,12 @@ def _reverse_pools(torch, ids, pos, dist, cand, keep, cap):
 
 
 # ------------------------------------------------------------------------------------------------ public entry point
+def _pred_kwargs(pred_kwargs):
+    pk = {"efS": 100, "topk": 10, "threads": 1}
+    pk.update(pred_kwargs or {})
+    return pk
+
+
 def build_hnsw_index(X, folder, M=32, efC=100, metric="ip", seed=0, max_level_upper_bound=-1, device=None, pred_kwargs=None,
                      q_tile=4096, c_tile=65536, h_tile=None, allow_tf32=False):
     """Builds the index for the rows of ``X`` and writes it to ``folder`` in the reference's format.  ``X``: float32 [N, d]
@@ -463,12 +472,10 @@ def build_hnsw_index(X, folder, M=32, efC=100, metric="ip", seed=0, max_level_up
         json.dump({"hnsw_t": (_HNSW_T_SPARSE if sparse else _HNSW_T)[metric], "version": "v2.0",
                    "train_params": {"num_node": N, "maxM": maxM, "maxM0": maxM0, "efC": int(efC), "max_level": max_level,
                                     "init_node": init_node}}, f, indent=4)
-    pk = {"efS": 100, "topk": 10, "threads": 1}
-    pk.update(pred_kwargs or {})
     with open(os.path.join(folder, "param.json"), "w", encoding="utf-8") as f:
         json.dump({"model": "HNSW", "data_type": "csr" if sparse else "drm", "metric_type": metric, "num_item": N, "feat_dim": d,
                    "train_kwargs": {"M": maxM, "efC": int(efC), "builder": "pecos_b200.hnsw_build (batch, exact kNN + heuristic)"},
-                   "pred_kwargs": pk}, f, indent=1)
+                   "pred_kwargs": _pred_kwargs(pred_kwargs)}, f, indent=1)
     phase_ms = timer.totals_ms()
     phase_ms["write"] = (time.perf_counter() - t0) * 1e3
     stats = {"num_node": N, "feat_dim": d, "max_level": max_level, "init_node": init_node,
@@ -477,6 +484,53 @@ def build_hnsw_index(X, folder, M=32, efC=100, metric="ip", seed=0, max_level_up
         work = sp.work.cpu().tolist()
         stats["block_postings"], stats["candidate_entries"] = int(work[0]), int(work[1])
     return stats
+
+
+SHARDS_MANIFEST = "shards.json"
+
+
+def build_hnsw_shards(X, folder, world, ranks=None, device=None, seed=0, **build_kwargs):
+    """Builds a sharded index: the rows of ``X`` split into ``world`` contiguous ranges, one independent index per range in
+    ``<folder>/shard-<r>/`` (an ordinary index folder written by :func:`build_hnsw_index` with seed ``seed + r``), and the
+    manifest ``<folder>/shards.json``.  Shard r's node j is global id ``row_begin[r] + j``.  Ranges: equal row counts for dense
+    ``X``, ``distributed.split_rows_by_nnz`` of the csr indptr for sparse ``X``.
+
+    Only the shards listed in ``ranks`` (default: all) are built, so under torchrun every rank builds its own with
+    ``ranks=[rank]`` on its GPU.  The manifest depends only on X's shape (or indptr), ``world``, ``seed`` and the build
+    arguments, so every caller writes the same file.  ``pecos_b200.distributed.ShardedHNSW`` searches the result.  Returns
+    ``{"manifest": ..., "shards": {rank: build statistics}}``."""
+    import scipy.sparse as smat
+
+    from .distributed import split_rows_by_nnz
+
+    world = int(world)
+    if world < 1:
+        raise ValueError(f"world must be >= 1, got {world}")
+    ranks = list(range(world)) if ranks is None else [int(r) for r in ranks]
+    if any(r < 0 or r >= world for r in ranks):
+        raise ValueError(f"ranks {ranks} are outside 0..{world - 1}")
+    sparse = smat.issparse(X)
+    if sparse:
+        X = smat.csr_matrix(X)
+        row_begin = [int(b) for b in split_rows_by_nnz(X.indptr, world)]
+    else:
+        X = np.ascontiguousarray(X, dtype=np.float32)
+        row_begin = [X.shape[0] * r // world for r in range(world + 1)]
+    if any(row_begin[r + 1] <= row_begin[r] for r in range(world)):
+        raise ValueError(f"{X.shape[0]} rows cannot fill {world} non-empty shards (row ranges {row_begin})")
+    manifest = {"world": world, "num_item": int(X.shape[0]), "feat_dim": int(X.shape[1]), "data_type": "csr" if sparse else "drm",
+                "metric_type": build_kwargs.get("metric", "ip"), "row_begin": row_begin,
+                "seeds": [int(seed) + r for r in range(world)], "pred_kwargs": _pred_kwargs(build_kwargs.get("pred_kwargs"))}
+    shards = {}
+    for r in ranks:
+        shards[r] = build_hnsw_index(X[row_begin[r]:row_begin[r + 1]], os.path.join(folder, f"shard-{r}"), seed=int(seed) + r,
+                                     device=device, **build_kwargs)
+    os.makedirs(folder, exist_ok=True)
+    tmp = os.path.join(folder, f".{SHARDS_MANIFEST}.{os.getpid()}")
+    with open(tmp, "w", encoding="utf-8") as f:
+        json.dump(manifest, f, indent=1)
+    os.replace(tmp, os.path.join(folder, SHARDS_MANIFEST))  # atomic: concurrent writers leave one complete copy
+    return {"manifest": manifest, "shards": shards}
 
 
 def _sparse_records(head, X):

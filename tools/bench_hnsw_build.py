@@ -42,17 +42,28 @@ def card():
 
 
 def exact_top10(X, Q, metric, tile=512):
-    """Exact top-10 by the reference's sparse distance order (ip: 1 - <q,x>; l2: -2<q,x>: both = descending dot) on the GPU."""
+    """Exact top-10 by the reference's distance order on the GPU.  Sparse X (csr): ip 1 - <q,x> and the reference's l2 -2<q,x>,
+    both = descending dot.  Dense X (float32 array): ip 1 - <q,x> (descending dot), l2 |q - x|^2 (descending 2<q,x> - |x|^2)."""
+    import scipy.sparse as smat
     import torch
 
     dev = torch.device("cuda", 0)
-    Xt = torch.sparse_csr_tensor(torch.from_numpy(X.indptr.astype(np.int64)), torch.from_numpy(X.indices.astype(np.int64)),
-                                 torch.from_numpy(X.data), size=X.shape).to(dev)
+    sparse = smat.issparse(X)
+    if sparse:
+        Xt = torch.sparse_csr_tensor(torch.from_numpy(X.indptr.astype(np.int64)), torch.from_numpy(X.indices.astype(np.int64)),
+                                     torch.from_numpy(X.data), size=X.shape).to(dev)
+    else:
+        Xt = torch.from_numpy(np.ascontiguousarray(X, dtype=np.float32)).to(dev)
+        sq = (Xt * Xt).sum(1) if metric == "l2" else None
     out = np.empty((Q.shape[0], 10), dtype=np.int64)
     for q0 in range(0, Q.shape[0], tile):
         q1 = min(Q.shape[0], q0 + tile)
-        Qd = torch.from_numpy(Q[q0:q1].toarray()).to(dev)
-        dot = (Xt @ Qd.T).T                                   # [tile, N]
+        if sparse:
+            dot = (Xt @ torch.from_numpy(Q[q0:q1].toarray()).to(dev).T).T   # [tile, N]
+        else:
+            dot = torch.from_numpy(np.ascontiguousarray(Q[q0:q1], dtype=np.float32)).to(dev) @ Xt.T
+            if sq is not None:
+                dot = 2.0 * dot - sq
         out[q0:q1] = torch.topk(dot, 10, dim=1, largest=True, sorted=True).indices.cpu().numpy()
     return out
 
