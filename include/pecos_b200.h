@@ -235,8 +235,12 @@ void pb200_xlinear_set_profile(void* ptr, int on);
  * warp per chunk in place of the query-warp kernel, 3 = as 1 but the query-warp kernel wherever it is eligible and the
  * chunk-major kernel is not chosen, 4 = as 1 but the warp top-k evaluates the post-processor for every candidate (no
  * single-precision estimate filter), 5 = as 1 plus the chunk-major kernel on every layer with chunk images (its reuse and
- * occupancy heuristics ignored), 6 = as 1 without the chunk-major kernel (query-major kernels only).  Any other value
- * behaves as 1.
+ * occupancy heuristics ignored, and the prefix kernel below on tiles of any size), 6 = as 1 without the chunk-major kernel
+ * (query-major kernels only, no prefix kernel), 7 = as 1 without the prefix kernel.  Any other value behaves as 1.
+ * Prefix kernel (modes 1 - 5): where layer 0 is one chunk, every query's beam holds all of layer 0, neither upper layer is
+ * rearranged, both share their bias and their merged image fits in shared memory, a sparse tile of enough queries scores
+ * layers 0 and 1 in ONE chunk-major launch (kernel id 4 in layer 0's score slot; layer 0's top-k slot and layer 1's score
+ * slot then read 0 ms).  Results are identical with and without it.
  * Returns 1 when every layer has a feature map (PB200_FEATMAP_MB caps their total size at load time, default 32768). */
 int pb200_xlinear_set_lookup(void* ptr, int on);
 void pb200_xlinear_reset_profile(void* ptr);
@@ -335,6 +339,9 @@ void pb200_sparse_candidate_distances(int device, int metric, const void* row_pt
 void* pb200_xlinear_host_load(const char* model_path, int kind);
 /* host-only: the one-layer model c_xlinear_single_layer_predict_* builds from in-memory W / C (same handle type) */
 void* pb200_xlinear_host_from_csc(const ScipyCscF32* W, const ScipyCscF32* C, float bias);
+/* host-only: a new one-layer handle holding the merged layer that scores layers 0 and 1 of hptr in one pass (W = [W0 | W1],
+ * one chunk, one shared bias row); hptr must have depth >= 2, neither layer rearranged, both over the same features */
+void* pb200_xlinear_host_prefix_layer(void* hptr);
 void pb200_xlinear_host_free(void* hptr);
 uint32_t pb200_xlinear_host_depth(void* hptr);
 void pb200_xlinear_host_layer_dims(void* hptr, uint32_t layer, uint64_t* out);

@@ -481,6 +481,7 @@ class B200CoreLib(object):
         fp(c.pb200_sparse_candidate_distances, None, [c_int, c_int, c_void_p, c_void_p, c_void_p, c_uint32, c_uint32, c_void_p,
                                                       c_void_p, c_void_p])
         fp(c.pb200_xlinear_host_load, c_void_p, [c_char_p, c_int])
+        fp(c.pb200_xlinear_host_prefix_layer, c_void_p, [c_void_p])
         fp(c.pb200_xlinear_host_free, None, [c_void_p])
         fp(c.pb200_xlinear_host_depth, c_uint32, [c_void_p])
         fp(c.pb200_xlinear_host_layer_dims, None, [c_void_p, c_uint32, POINTER(c_uint64)])
@@ -517,6 +518,16 @@ class B200CoreLib(object):
         c = self.clib_float32
         h = c_void_p(c.pb200_xlinear_host_load(model_path.encode("utf-8"), 1 if is_mmap else 0))
         return self._export_host_model(h)
+
+    def host_prefix_layer_layout(self, model_path):
+        """Host-only: the merged one-chunk layer that scores layers 0 and 1 of an npz model folder in one pass."""
+        c = self.clib_float32
+        h = c_void_p(c.pb200_xlinear_host_load(model_path.encode("utf-8"), 0))
+        try:
+            m = c_void_p(c.pb200_xlinear_host_prefix_layer(h))
+        finally:
+            c.pb200_xlinear_host_free(h)
+        return self._export_host_model(m)[0]
 
     def _export_host_model(self, h):
         c = self.clib_float32

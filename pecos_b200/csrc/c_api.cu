@@ -827,6 +827,17 @@ void* pb200_xlinear_host_from_csc(const ScipyCscF32* W, const ScipyCscF32* C, fl
     PB200_API_END("pb200_xlinear_host_from_csc")
 }
 
+void* pb200_xlinear_host_prefix_layer(void* hptr) {
+    PB200_API_BEGIN
+    const auto& H = *static_cast<pb200::XLinearHostModel*>(hptr);
+    if (H.depth() < 2) throw std::runtime_error("pecos_b200: the prefix layer needs a model of depth >= 2");
+    auto m = std::make_unique<pb200::XLinearHostModel>();
+    m->layers.resize(1);
+    pb200::build_prefix_layer(H.layers[0], H.layers[1], m->layers[0]);
+    return m.release();
+    PB200_API_END("pb200_xlinear_host_prefix_layer")
+}
+
 void pb200_xlinear_host_free(void* hptr) { delete static_cast<pb200::XLinearHostModel*>(hptr); }
 
 uint32_t pb200_xlinear_host_depth(void* hptr) { return static_cast<pb200::XLinearHostModel*>(hptr)->depth(); }

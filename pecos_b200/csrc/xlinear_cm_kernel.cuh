@@ -56,6 +56,25 @@ struct CmPlan {  // per call
     size_t smem = 0;
 };
 
+// PREFIX mode of xl_cm_scores_kernel: the image is the merged one-chunk layer of layers 0 and 1 (layer 0's n0 columns, then
+// layer 1's columns in layer-1 column order, see build_prefix_layer) and pair i is query i of the tile.  A query's layer-0
+// beam holds all n0 candidates, so layer 0's top-k is a sort of its n0 transformed scores, and layer 1's beam slots are every
+// layer-1 chunk in that order.  The epilogue writes the layer-0 beam and layer 1's raw scores at the candidate positions
+// layer 1's top-k kernel reads.
+constexpr uint32_t kCmPrefixTop0 = 8;       // widest layer 0 the prefix takes (its keys are sorted in registers)
+struct CmPrefixOut {
+    uint32_t rows = 0;                      // queries of the tile
+    uint32_t n0 = 0;                        // layer 0's columns (<= kCmPrefixTop0)
+    int pp_kind = 0, pp_p = 0;              // layer 0's post-processor
+    const ChunkHeader* chunks1 = nullptr;   // layer 1's chunks: chunk j = the children of layer-0 column j
+    uint32_t* beam_id = nullptr;            // layer 0's beam [rows x beam_stride], best first
+    float* beam_val = nullptr;
+    uint32_t* beam_cnt = nullptr;
+    uint32_t beam_stride = 0;
+    float* cand1 = nullptr;                 // layer 1's candidate rows [rows x cand1_stride]
+    uint64_t cand1_stride = 0;
+};
+
 __host__ __device__ inline uint32_t cm_align16(uint32_t x) { return (x + 15u) & ~15u; }
 
 __host__ __device__ inline size_t cm_warp_bytes(uint32_t acc_cols, uint32_t stages) {
@@ -426,10 +445,12 @@ struct CmTrace {
 };
 #endif
 
-template <bool DIRECT, int STAGES>
+// PREFIX: see CmPrefixOut (w, cand and cand_stride_q are unused; a CTA takes an equal slice of the tile's rows and stages the
+// one image once).  Otherwise P is unused.
+template <bool DIRECT, int STAGES, bool PREFIX = false>
 __global__ void __launch_bounds__(kCmMaxWarps * 32, 1)
 xl_cm_scores_kernel(const LayerDev L, const QueryDev X, const CmWork w, const CmShape S, const unsigned char* __restrict__ images,
-                    float* __restrict__ cand, const uint64_t cand_stride_q) {
+                    float* __restrict__ cand, const uint64_t cand_stride_q, const CmPrefixOut P) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     unsigned char* img = smem_raw;                                   // the staged image of one virtual chunk
     // the image is only ever written by the bulk copy (async proxy), never by this kernel's stores: __restrict__ lets the
@@ -462,14 +483,20 @@ xl_cm_scores_kernel(const LayerDev L, const QueryDev X, const CmWork w, const Cm
 
     // ---- this CTA's contiguous share of the (virtual-)chunk-sorted pair list: an equal share of the estimated WORK
     const uint32_t n_vc = S.n_vc;
-    const uint32_t begin = cm_share_begin(w, n_vc, blockIdx.x, gridDim.x);
-    const uint32_t end = cm_share_begin(w, n_vc, blockIdx.x + 1u, gridDim.x);
+    uint32_t begin, end;
+    if constexpr (PREFIX) {  // every pair costs the same: equal slices of the rows
+        begin = static_cast<uint32_t>(static_cast<uint64_t>(P.rows) * blockIdx.x / gridDim.x);
+        end = static_cast<uint32_t>(static_cast<uint64_t>(P.rows) * (blockIdx.x + 1u) / gridDim.x);
+    } else {
+        begin = cm_share_begin(w, n_vc, blockIdx.x, gridDim.x);
+        end = cm_share_begin(w, n_vc, blockIdx.x + 1u, gridDim.x);
+    }
     if (begin >= end) {
         trace.flush(warp, lane);
         return;
     }
-    uint32_t c;
-    {
+    uint32_t c = 0;
+    if constexpr (!PREFIX) {
         uint32_t lo = 0, hi = n_vc;  // largest c with bucket_ptr[c] <= begin (then skip empty buckets forward)
         while (hi - lo > 1) {
             const uint32_t mid = (lo + hi) >> 1;
@@ -534,8 +561,11 @@ xl_cm_scores_kernel(const LayerDev L, const QueryDev X, const CmWork w, const Cm
     };
 
     for (uint32_t i = begin; i < end;) {
-        while (w.bucket_ptr[c + 1] <= i) ++c;                        // virtual chunk holding pair i
-        const uint32_t run_end = min(end, w.bucket_ptr[c + 1]);
+        uint32_t run_end = end;
+        if constexpr (!PREFIX) {
+            while (w.bucket_ptr[c + 1] <= i) ++c;                    // virtual chunk holding pair i
+            run_end = min(end, w.bucket_ptr[c + 1]);
+        }
         // ---- stage the image: ONE bulk copy (every warp has left the previous image: barrier first)
         __syncthreads();
         if (threadIdx.x == 0) cm_bulk_load(static_cast<uint32_t>(__cvta_generic_to_shared(img)), images + static_cast<uint64_t>(c) * S.img_bytes, S.img_bytes, mbar);
@@ -552,8 +582,12 @@ xl_cm_scores_kernel(const LayerDev L, const QueryDev X, const CmWork w, const Cm
             uint32_t q = 0, pos = 0, qn = 0;
             uint64_t qb = 0;
             if (have) {
-                q = w.pair_q[pidx];
-                pos = w.pair_pos[pidx];
+                if constexpr (PREFIX) {
+                    q = pidx;
+                } else {
+                    q = w.pair_q[pidx];
+                    pos = w.pair_pos[pidx];
+                }
                 qb = X.row_ptr[q] - X.nnz_base;
                 qn = static_cast<uint32_t>(X.row_ptr[q + 1] - X.nnz_base - qb);
             }
@@ -657,8 +691,39 @@ xl_cm_scores_kernel(const LayerDev L, const QueryDev X, const CmWork w, const Cm
             }
             trace.mark(kCmPhAccumulate);
             if (have) {
-                float* dst = cand + static_cast<uint64_t>(q) * cand_stride_q + pos;
-                for (uint32_t col = 0; col < n_cols; ++col) dst[col] = my_acc[col * 32];
+                if constexpr (PREFIX) {
+                    // layer 0 keeps all n0 candidates: its top-k is the descending order of their exact keys (unused keys
+                    // are 0 and sort last; a real key never is 0)
+                    unsigned long long key[kCmPrefixTop0];
+#pragma unroll
+                    for (uint32_t j = 0; j < kCmPrefixTop0; ++j)
+                        key[j] = j < P.n0 ? xl_exact_key(xl_transform(my_acc[j * 32], P.pp_kind, P.pp_p), j) : 0ull;
+#pragma unroll
+                    for (uint32_t a = 1; a < kCmPrefixTop0; ++a)
+#pragma unroll
+                        for (uint32_t b = a; b > 0; --b)
+                            if (key[b] > key[b - 1]) { const unsigned long long t = key[b]; key[b] = key[b - 1]; key[b - 1] = t; }
+                    // layer 1's beam slot r is the chunk of layer-0 rank r: its children's raw scores go to the next
+                    // positions of the candidate row, in column order
+                    const uint64_t o = static_cast<uint64_t>(q) * P.beam_stride;
+                    float* dst = P.cand1 + static_cast<uint64_t>(q) * P.cand1_stride;
+#pragma unroll
+                    for (uint32_t r = 0; r < kCmPrefixTop0; ++r) {
+                        if (r < P.n0) {
+                            const uint32_t j = xl_exact_key_pos(key[r]);
+                            P.beam_id[o + r] = j;
+                            P.beam_val[o + r] = xl_exact_key_value(key[r]);
+                            const ChunkHeader h = P.chunks1[j];
+                            const float* src = my_acc + (P.n0 + h.col_begin) * 32u;
+                            for (uint32_t col = 0; col < h.n_cols; ++col) dst[col] = src[col * 32];
+                            dst += h.n_cols;
+                        }
+                    }
+                    P.beam_cnt[q] = P.n0;
+                } else {
+                    float* dst = cand + static_cast<uint64_t>(q) * cand_stride_q + pos;
+                    for (uint32_t col = 0; col < n_cols; ++col) dst[col] = my_acc[col * 32];
+                }
             }
             trace.mark(kCmPhSlice);
         }

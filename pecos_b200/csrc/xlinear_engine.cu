@@ -495,6 +495,24 @@ __device__ __forceinline__ unsigned long long xl_make_key(float v, uint32_t pos)
     return (static_cast<unsigned long long>(u) << 32) | static_cast<unsigned long long>(0xFFFFFFFFu - pos);
 }
 
+// Selection key that also carries the value's exact bits: orderable(score) << 32 | ~((pos << 1) | neg_zero).  Same order as
+// xl_make_key (-0.0 ties with +0.0, and ties go to the lower position); xl_exact_key_value gives back the bits, -0.0 included.
+__device__ __forceinline__ unsigned long long xl_exact_key(float v, uint32_t pos) {
+    uint32_t u = __float_as_uint(v);
+    const uint32_t neg_zero = (u == 0x80000000u) ? 1u : 0u;  // -0.0 compares equal to +0.0 but keeps its bits
+    if ((u & 0x7FFFFFFFu) == 0u) u = 0u;
+    u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+    return (static_cast<unsigned long long>(u) << 32) | static_cast<unsigned long long>(0xFFFFFFFFu - ((pos << 1) | neg_zero));
+}
+__device__ __forceinline__ uint32_t xl_exact_key_pos(unsigned long long key) {
+    return (0xFFFFFFFFu - static_cast<uint32_t>(key & 0xFFFFFFFFull)) >> 1;
+}
+__device__ __forceinline__ float xl_exact_key_value(unsigned long long key) {
+    const uint32_t hi = static_cast<uint32_t>(key >> 32);
+    const uint32_t bits = (hi & 0x80000000u) ? (hi ^ 0x80000000u) : ~hi;
+    return __uint_as_float(((0xFFFFFFFFu - static_cast<uint32_t>(key & 0xFFFFFFFFull)) & 1u) ? 0x80000000u : bits);
+}
+
 #include "xlinear_qw_kernel.cuh"
 #include "xlinear_cm_kernel.cuh"
 
@@ -976,6 +994,47 @@ XLinearEngine::XLinearEngine(std::unique_ptr<XLinearHostModel> host, int device)
         model_bytes_ += src.chunks.size() * sizeof(ChunkHeader) + src.meta.size() * 4 + src.entries.size() * 8 +
                         src.label_of_col.size() * 4;
     }
+    // The prefix image: layers 0 and 1 merged into one chunk (build_prefix_layer) when layer 0 is one narrow chunk, neither
+    // layer is rearranged or index-sharded, both share features and bias, and the merged chunk fits a direct-table image.
+    if (layers_.size() >= 2 && layers_[0].view.featmap && layers_[1].view.featmap) {
+        const ChunkedLayerHost& H0 = host_->layers[0];
+        const ChunkedLayerHost& H1 = host_->layers[1];
+        bool ok = H0.n_chunks == 1 && H0.n_cols >= 1 && H0.n_cols <= kCmPrefixTop0 && H1.n_chunks == H0.n_cols &&
+                  !H0.reordered && !H1.reordered && H0.w_rows == H1.w_rows && H0.w_rows <= kCmDirectRows &&
+                  std::memcmp(&H0.bias, &H1.bias, sizeof(float)) == 0 && H0.n_cols + H1.n_cols <= 256u;
+        for (const ChunkHeader& ch : H0.chunks) ok = ok && !(ch.has_bias & kChunkAbsent);
+        for (const ChunkHeader& ch : H1.chunks) ok = ok && !(ch.has_bias & kChunkAbsent);
+        if (ok) {
+            ChunkedLayerHost M;
+            build_prefix_layer(H0, H1, M);
+            const uint32_t fm_words = static_cast<uint32_t>((static_cast<uint64_t>(M.w_rows) + 31) / 32);
+            const uint64_t n_ent = M.entries.size();
+            CmShape shape = n_ent < 65535u ? cm_shape(fm_words, M.w_rows, M.r_max, static_cast<uint32_t>(n_ent), M.c_max, 1, 1) : CmShape{};
+            if (shape.ok && shape.direct && shape.img_bytes <= cmimg_budget) {
+                LayerStore& P = prefix_;
+                P.chunks.upload(M.chunks.data(), M.chunks.size(), stream_);
+                P.meta.upload(M.meta.data(), M.meta.size(), stream_);
+                P.entries.upload(reinterpret_cast<const uint2*>(M.entries.data()), M.entries.size(), stream_);
+                const uint32_t vc_ptr[2] = {0u, 1u};
+                P.cm_vc_ptr.upload(vc_ptr, 2, stream_);
+                P.view.chunks = P.chunks.get();
+                P.view.meta = P.meta.get();
+                P.view.entries = P.entries.get();
+                P.view.n_cols = M.n_cols;
+                P.view.n_chunks = 1;
+                P.view.c_max = M.c_max;
+                P.view.w_rows = M.w_rows;
+                P.view.bias = M.bias;
+                shape.vc_ptr = P.cm_vc_ptr.get();
+                P.cm_shape = shape;
+                P.cm_images.reserve(shape.img_bytes);
+                xl_cm_build_images_kernel<<<1, 256, 0, stream_>>>(P.view, shape, P.cm_images.get());
+                PB200_CUDA(cudaGetLastError());
+                PB200_CUDA(cudaStreamSynchronize(stream_));  // M's host arrays go out of scope
+                model_bytes_ += shape.img_bytes + M.chunks.size() * sizeof(ChunkHeader) + M.meta.size() * 4 + M.entries.size() * 8 + 8;
+            }
+        }
+    }
     PB200_CUDA(cudaStreamSynchronize(stream_));
     // host copies of the big arrays are no longer needed
     for (auto& l : host_->layers) {
@@ -996,6 +1055,8 @@ XLinearEngine::XLinearEngine(std::unique_ptr<XLinearHostModel> host, int device)
     PB200_CUDA(cudaFuncSetAttribute(xl_cm_scores_kernel<true, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kCmSmemBudget)));
     PB200_CUDA(cudaFuncSetAttribute(xl_cm_scores_kernel<false, 2>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kCmSmemBudget)));
     PB200_CUDA(cudaFuncSetAttribute(xl_cm_scores_kernel<false, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kCmSmemBudget)));
+    PB200_CUDA(cudaFuncSetAttribute(xl_cm_scores_kernel<true, 2, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kCmSmemBudget)));
+    PB200_CUDA(cudaFuncSetAttribute(xl_cm_scores_kernel<true, 4, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(kCmSmemBudget)));
     PB200_CUDA(cudaFuncSetAttribute(xl_query_warp_scores_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
     PB200_CUDA(cudaFuncSetAttribute(xl_query_warp_scores_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
     stats_dev_.reserve(8 * layers_.size());
@@ -1020,7 +1081,8 @@ void XLinearEngine::set_kernel_mode(int mode) {
     // 2: feature-map lookups with one warp per chunk (no query-warp kernel); 3: query-warp kernel wherever eligible;
     // 4: as 1 but the warp top-k evaluates the post-processor for every candidate (no estimate filter);
     // 5: as 1, and the chunk-major score kernel wherever it FITS (its reuse / occupancy heuristics ignored; tests);
-    // 6: as 1 WITHOUT the chunk-major score kernel (query-major kernels only, for A/B tests)
+    // 6: as 1 WITHOUT the chunk-major score kernel (query-major kernels only, no prefix kernel, for A/B tests);
+    // 7: as 1 without the prefix kernel (layers 0 and 1 scored and selected one by one, for A/B tests)
     const bool on = mode != 0;
     for (auto& l : layers_) l.view.featmap = (on && l.featmap.capacity()) ? l.featmap.get() : nullptr;
     force_block_topk_ = !on;
@@ -1029,6 +1091,7 @@ void XLinearEngine::set_kernel_mode(int mode) {
     no_topk_filter_ = (mode == 4);
     chunk_major_ = on && (mode != 6);
     cm_force_ = (mode == 5);
+    no_prefix_ = (mode == 7);
 }
 
 bool XLinearEngine::has_feature_maps() const {
@@ -1155,7 +1218,8 @@ int XLinearEngine::score_layer_(size_t d, const QueryDev& q, uint32_t b_prev, in
         xl_cm_scan_kernel<<<1, 1024, 0, stream_>>>(n_vc, w, layers_[d].cm_images.get(), shape.img_bytes, L.w_rows);
         xl_cm_scatter_kernel<<<warp_grid, 128, 0, stream_>>>(L, bid, bcnt, beam_stride_, rows, w, shape.vc_ptr);
         auto launch_cm = [&](auto kernel) {
-            kernel<<<cm.grid, cm.warps * 32, cm.smem, stream_>>>(L, q, w, shape, layers_[d].cm_images.get(), cand, cand_stride_q);
+            kernel<<<cm.grid, cm.warps * 32, cm.smem, stream_>>>(L, q, w, shape, layers_[d].cm_images.get(), cand, cand_stride_q,
+                                                                 CmPrefixOut{});
         };
         if (shape.direct) { if (shape.stages == 4) launch_cm(xl_cm_scores_kernel<true, 4>); else launch_cm(xl_cm_scores_kernel<true, 2>); }
         else { if (shape.stages == 4) launch_cm(xl_cm_scores_kernel<false, 4>); else launch_cm(xl_cm_scores_kernel<false, 2>); }
@@ -1187,20 +1251,75 @@ int XLinearEngine::score_layer_(size_t d, const QueryDev& q, uint32_t b_prev, in
     return layer_profile_[d].scores_kernel;
 }
 
+// The prefix launch needs the merged image, sparse queries, a layer-0 top-k that keeps every layer-0 node (so that layer 1's
+// beam is all of layer 1, in layer 0's rank order) and enough rows to fill the GPU: a small tile leaves most SMs idle in
+// the one-pass kernel, while the per-layer kernels spread its pairs wider (kernel mode 5 ignores the row count, for tests).
+bool XLinearEngine::use_prefix_(const QueryDev& q, const std::vector<LayerPlan>& plan) const {
+    if (!prefix_.cm_shape.ok || !chunk_major_ || no_prefix_ || q.row_ptr == nullptr || !layers_[0].view.featmap || plan.size() < 2)
+        return false;
+    if (plan[0].k < host_->layers[0].n_cols) return false;
+    if (static_cast<uint64_t>(q.rows) * std::max<uint32_t>(q.max_row_nnz, 1u) >= (1ull << 32)) return false;  // 32-bit feature offsets
+    return cm_force_ || q.rows >= kCmMinPairsPerSm * n_sm_;
+}
+
+void XLinearEngine::launch_prefix_(const QueryDev& q, const std::vector<LayerPlan>& plan, uint32_t ws_row) {
+    const CmShape& S = prefix_.cm_shape;
+    const uint32_t rows = q.rows;
+    const uint32_t grid = std::min<uint32_t>(n_sm_, (rows + 31u) / 32u);
+    const uint32_t share = (rows + grid - 1) / grid;
+    const uint32_t warps = std::max<uint32_t>(1u, std::min<uint32_t>(S.warps_fit, (share + 31u) / 32u));
+    const size_t smem = S.img_bytes + warps * cm_warp_bytes(S.acc_cols, S.stages) + 64;
+    CmPrefixOut P;
+    P.rows = rows;
+    P.n0 = host_->layers[0].n_cols;
+    P.pp_kind = plan[0].pp.kind;
+    P.pp_p = plan[0].pp.p;
+    P.chunks1 = layers_[1].view.chunks;
+    P.beam_id = bid_(1, ws_row);
+    P.beam_val = bval_(1, ws_row);
+    P.beam_cnt = bcnt_(1, ws_row);
+    P.beam_stride = beam_stride_;
+    P.cand1_stride = static_cast<uint64_t>(plan[1].b_prev) * std::max<uint32_t>(layers_[1].view.c_max, 1u);
+    P.cand1 = cand_.get() + ws_row * P.cand1_stride;
+    auto launch = [&](auto kernel) {
+        kernel<<<grid, warps * 32, smem, stream_>>>(prefix_.view, q, CmWork{}, S, prefix_.cm_images.get(), nullptr, 0, P);
+    };
+    if (S.stages == 4) launch(xl_cm_scores_kernel<true, 4, true>);
+    else launch(xl_cm_scores_kernel<true, 2, true>);
+    PB200_CUDA(cudaGetLastError());
+    ++launches_;
+}
+
 // Runs layers [d_begin, d_end) over one tile of queries; the last layer of the plan writes into `out`.
 void XLinearEngine::run_tile_(const QueryDev& q, const std::vector<LayerPlan>& plan, const OutTarget& out, uint32_t ws_row,
                               bool collect_stats, bool ext_beam, int combine_first, size_t d_begin, size_t d_end) {
     const uint32_t rows = q.rows;
     if (rows == 0) return;
     int cur = static_cast<int>(d_begin & 1);  // every layer flips the ping-pong beam buffers once
-    if (!ext_beam && d_begin == 0) {
+    const size_t depth = plan.size();
+    d_end = std::min(d_end, depth);
+    const bool prefix = !ext_beam && d_begin == 0 && d_end >= 2 && combine_first == 0 && !collect_stats && use_prefix_(q, plan);
+    if (!ext_beam && d_begin == 0 && !prefix) {
         xl_init_beam_kernel<<<(rows + 255) / 256, 256, 0, stream_>>>(bid_(cur, ws_row), bval_(cur, ws_row),
                                                                      bcnt_(cur, ws_row), beam_stride_, rows);
         ++launches_;
     }
-    const size_t depth = plan.size();
-    d_end = std::min(d_end, depth);
     for (size_t d = d_begin; d < d_end; ++d) {
+        if (prefix && d == 0) {  // layer 0's scores, beam and layer 1's raw scores: one launch, timed in layer 0's score slot
+            if (profile_) PB200_CUDA(cudaEventRecord(ev_[0], stream_));
+            launch_prefix_(q, plan, ws_row);
+            layer_profile_[0].scores_kernel = 4;
+            if (profile_) {
+                PB200_CUDA(cudaEventRecord(ev_[1], stream_));
+                PB200_CUDA(cudaEventSynchronize(ev_[1]));
+                float a = 0.f;
+                PB200_CUDA(cudaEventElapsedTime(&a, ev_[0], ev_[1]));
+                layer_profile_[0].scores_ms += a;
+                layer_profile_[0].launches += 1;
+            }
+            cur ^= 1;
+            continue;
+        }
         const LayerDev& L = layers_[d].view;
         const LayerPlan& lp = plan[d];
         const int combine = (d == 0) ? combine_first : 1;
@@ -1213,7 +1332,9 @@ void XLinearEngine::run_tile_(const QueryDev& q, const std::vector<LayerPlan>& p
         unsigned long long* stats = collect_stats ? stats_dev_.get() + 8 * d : nullptr;
         if (profile_) PB200_CUDA(cudaEventRecord(ev_[0], stream_));
         const dim3 grid(rows);
-        score_layer_(d, q, lp.b_prev, cur, ws_row, collect_stats);
+        const bool scored = prefix && d == 1;  // by the prefix launch
+        if (scored) layer_profile_[1].scores_kernel = 4;
+        else score_layer_(d, q, lp.b_prev, cur, ws_row, collect_stats);
         if (profile_) PB200_CUDA(cudaEventRecord(ev_[1], stream_));
 
         const OutTarget o = (d + 1 == depth) ? out
@@ -1254,9 +1375,9 @@ void XLinearEngine::run_tile_(const QueryDev& q, const std::vector<LayerPlan>& p
             float a = 0.f, b = 0.f;
             PB200_CUDA(cudaEventElapsedTime(&a, ev_[0], ev_[1]));
             PB200_CUDA(cudaEventElapsedTime(&b, ev_[1], ev_[2]));
-            layer_profile_[d].scores_ms += a;
+            if (!scored) layer_profile_[d].scores_ms += a;  // the slot stays at 0 ms: the prefix launch is layer 0's
             layer_profile_[d].topk_ms += b;
-            layer_profile_[d].launches += 2;
+            layer_profile_[d].launches += scored ? 1 : 2;
         }
         cur ^= 1;
     }

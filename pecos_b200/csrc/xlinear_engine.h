@@ -144,7 +144,7 @@ public:
     Result sharded_merge_packed(uint32_t world, uint32_t rows, uint32_t stride, uint32_t only_topk, const void* g_rec);
 
     void set_profile(bool on) { profile_ = on; }
-    // kernel selection for A/B runs and cross-checks: modes 0 - 6, listed at the definition; any other value behaves as 1
+    // kernel selection for A/B runs and cross-checks: modes 0 - 7, listed at the definition; any other value behaves as 1
     void set_kernel_mode(int mode);
     bool has_feature_maps() const;
     const std::vector<XLinearLayerProfile>& layer_profile() const { return layer_profile_; }
@@ -271,6 +271,15 @@ private:
     bool no_topk_filter_ = false;
     bool chunk_major_ = true;   // chunk-major scoring wherever cm_plan() finds it eligible (kernel mode 6 switches it off)
     bool cm_force_ = false;     // kernel mode 5
+    bool no_prefix_ = false;    // kernel mode 7
+    // Merged one-chunk layer of layers 0 and 1 (build_prefix_layer) and its chunk-major image: scores both layers of a tile
+    // in one launch (prefix_.cm_images empty: the model is not eligible)
+    LayerStore prefix_;
+    // Whether one prefix launch may replace layer 0 and layer 1's scoring for this tile (the caller checks that the tile
+    // enters at layer 0 with the root beam, runs both layers and collects no statistics).
+    bool use_prefix_(const QueryDev& q, const std::vector<LayerPlan>& plan) const;
+    // Layer 0's beam into beam_*_[1] and layer 1's raw scores into its candidate rows, for rows [ws_row, ws_row + q.rows).
+    void launch_prefix_(const QueryDev& q, const std::vector<LayerPlan>& plan, uint32_t ws_row);
     uint32_t n_sm_ = 132;
     DeviceBuffer<uint32_t> cm_slot_pos_, cm_count_, cm_bucket_ptr_, cm_pair_q_, cm_pair_pos_;
     DeviceBuffer<uint64_t> cm_cost_ptr_;

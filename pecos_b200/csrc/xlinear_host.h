@@ -359,6 +359,43 @@ inline void apply_leaf_shard(ChunkedLayerHost& L, uint32_t rank, uint32_t world,
     L.entries.swap(entries);
 }
 
+// The two upper layers as ONE one-chunk layer: W = [W0 | W1] with layer 1's columns in its (contiguous) column order, one
+// shared bias row.  A column's raw score is the sum over its own entries only, so scoring this layer gives both layers'
+// raw scores bit for bit.  Needs the host arrays of both layers, neither rearranged, the same feature space and the same
+// bias.
+inline void build_prefix_layer(const ChunkedLayerHost& L0, const ChunkedLayerHost& L1, ChunkedLayerHost& M) {
+    if (L0.reordered || L1.reordered || L0.w_rows != L1.w_rows) throw std::runtime_error("prefix layer: layers do not merge");
+    CscHost W;
+    W.rows = L0.w_rows;
+    W.cols = L0.n_cols + L1.n_cols;
+    W.col_ptr.assign(static_cast<size_t>(W.cols) + 1, 0);
+    // chunk c of layer l holds merged columns [first + col_begin, first + col_begin + n_cols); its rows ascend, so appending
+    // row by row keeps every column's entries in row order
+    auto for_each_entry = [&](auto&& fn) {
+        uint32_t first = 0;
+        for (const ChunkedLayerHost* L : {&L0, &L1}) {
+            for (const ChunkHeader& h : L->chunks) {
+                const uint32_t* rows = L->meta.data() + h.meta_off;
+                const uint32_t* rp = rows + round_up4(h.nnz_rows);
+                const ChunkEntry* en = L->entries.data() + h.ent_off;
+                for (uint32_t r = 0; r < h.nnz_rows; ++r)
+                    for (uint32_t i = rp[r]; i < rp[r + 1]; ++i) fn(first + h.col_begin + en[i].col_offset, rows[r], en[i].val);
+            }
+            first += L->n_cols;
+        }
+    };
+    for_each_entry([&](uint32_t col, uint32_t, float) { ++W.col_ptr[col + 1]; });
+    for (uint32_t c = 0; c < W.cols; ++c) W.col_ptr[c + 1] += W.col_ptr[c];
+    W.row_idx.resize(W.nnz());
+    W.val.resize(W.nnz());
+    std::vector<uint64_t> fill(W.col_ptr.begin(), W.col_ptr.end() - 1);
+    for_each_entry([&](uint32_t col, uint32_t row, float v) {
+        W.row_idx[fill[col]] = row;
+        W.val[fill[col]++] = v;
+    });
+    build_chunked_layer(W, csc_ones_column(W.cols), L0.bias, M);
+}
+
 // Bytes the feature map of a layer would occupy.
 inline uint64_t feature_map_bytes(const ChunkedLayerHost& L) {
     return static_cast<uint64_t>(L.n_chunks) * ((static_cast<uint64_t>(L.w_rows) + 31) / 32) * 8;

@@ -229,12 +229,7 @@ xl_topk_filter_kernel(const LayerDev L, const int pp_kind, const int pp_p, const
                 const uint32_t j = static_cast<uint32_t>(last_le_u32(s_base, static_cast<int>(cnt), pos));
                 float v = xl_transform(cq[pos], pp_kind, pp_p);
                 if (combine) v = xl_combine(v, s_pval[j], pp_kind);
-                uint32_t u = __float_as_uint(v);
-                const uint32_t neg_zero = (u == 0x80000000u) ? 1u : 0u;  // -0.0 compares equal to +0.0 but keeps its bits
-                if ((u & 0x7FFFFFFFu) == 0u) u = 0u;
-                u = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
-                key = (static_cast<unsigned long long>(u) << 32) |
-                      static_cast<unsigned long long>(0xFFFFFFFFu - ((pos << 1) | neg_zero));
+                key = xl_exact_key(v, pos);
             }
             head = (head + take) & (kFltRing - 1);
             pend -= take;
@@ -247,17 +242,13 @@ xl_topk_filter_kernel(const LayerDev L, const int pp_kind, const int pp_p, const
 
     // ---- results: lane r writes rank r
     if (static_cast<uint32_t>(lane) < kk) {
-        const uint32_t lo = 0xFFFFFFFFu - static_cast<uint32_t>(best & 0xFFFFFFFFull);
-        const uint32_t pos = lo >> 1;
-        const uint32_t hi = static_cast<uint32_t>(best >> 32);
-        uint32_t bits = (hi & 0x80000000u) ? (hi ^ 0x80000000u) : ~hi;
-        if (lo & 1u) bits = 0x80000000u;
+        const uint32_t pos = xl_exact_key_pos(best);
         const uint32_t j = static_cast<uint32_t>(last_le_u32(s_base, static_cast<int>(cnt), pos));
         uint32_t label = s_colbeg[j] + (pos - s_base[j]);
         if (L.label_of_col) label = L.label_of_col[label];
         const uint64_t o = static_cast<uint64_t>(q) * out_stride + lane;
         out_id[o] = label;
-        out_val[o] = __uint_as_float(bits);
-        if (out_key) out_key[o] = (static_cast<unsigned long long>(hi) << 32) | static_cast<unsigned long long>(0xFFFFFFFFu - pos);
+        out_val[o] = xl_exact_key_value(best);
+        if (out_key) out_key[o] = (best & 0xFFFFFFFF00000000ull) | static_cast<unsigned long long>(0xFFFFFFFFu - pos);
     }
 }
