@@ -8,9 +8,9 @@
 // access is a scattered global load (one L1 line each).  Here
 //   * at LOAD time every chunk of an eligible layer is packed into a self-contained IMAGE in HBM (xl_cm_build_images_kernel):
 //     header | lookup structure | entry weights (f32) | entry columns (u8).  Lookup structure: for feature spaces up to
-//     kCmDirectRows a direct table feature -> {first entry, end} (u16 | u16 << 16); else the chunk's feature map (one bit
-//     per feature + a 16-bit row prefix per 32 features: "is f a row, and which one" = one shared-memory word + popcount)
-//     and 16-bit row pointers;
+//     kCmDirectRows a direct table of w_rows + 1 u16 row starts, feature f's entries = [T[f], T[f + 1]) (a feature without a
+//     row gets the next row's start: an empty range); else the chunk's feature map (one bit per feature + a 16-bit row
+//     prefix per 32 features: "is f a row, and which one" = one shared-memory word + popcount) and 16-bit row pointers;
 //   * per call the pairs are bucketed by chunk on the device (count -> scan -> scatter; the reference's b_sort_by_chunk,
 //     pecos/core/xmc/inference.hpp:985-993);
 //   * the score kernel is PERSISTENT: one CTA per SM takes a contiguous share of the chunk-sorted pair list holding 1/grid
@@ -18,10 +18,12 @@
 //     and no CTA is left with the widest chunks' pairs; a chunk's image arrives by ONE bulk asynchronous copy
 //     (cp.async.bulk + mbarrier, the TMA engine's non-tensor form) and serves every pair of the run; warps take 32-pair
 //     slices of the run;
-//   * a lane walks its pair's query features in ascending order (staged global -> shared by cp.async, two rounds of 8 in
+//   * a lane walks its pair's query features in ascending order (staged global -> shared by cp.async, rounds of 8 in
 //     flight), compacts the hits of a round in place as {entry range, x}, then streams the hit rows' entries as one flat
-//     stream, kCmSlots entries per iteration across row boundaries (the warp's trip count follows the lane with the most
-//     entries), into the lane's PRIVATE accumulators acc[column][lane].  That is the reference's marching loop
+//     stream, kCmSlots entries per trip across row boundaries AND across rounds: after round r's lookup the warp runs only
+//     the trips that finish round r - 1's hits, a lane done early going on into round r's, so the trip count follows the
+//     largest backlog of a lane rather than each round's busiest lane; one drain (with the bias row) ends the pair.  The
+//     entries go into the lane's PRIVATE accumulators acc[column][lane].  That is the reference's marching loop
 //     (inference.hpp:788-811): ascending feature order, separate multiply and add, bias row last; a column is only ever
 //     touched by the lane that owns the pair: no compaction across lanes, no conflict resolution.
 //
@@ -77,9 +79,13 @@ struct CmPrefixOut {
 
 __host__ __device__ inline uint32_t cm_align16(uint32_t x) { return (x + 15u) & ~15u; }
 
+// staging buffers of a warp: `stages` rounds of query features in flight or in lookup, plus one that still holds the
+// previous round's compacted hits (carried into the next round's accumulate trips)
+__host__ __device__ constexpr uint32_t cm_buffers(uint32_t stages) { return stages + 1u; }
+
 __host__ __device__ inline size_t cm_warp_bytes(uint32_t acc_cols, uint32_t stages) {
-    return static_cast<size_t>(stages) * 32 * (kCmFeat + 1) * 8   // staging ring: query features / compacted hits, stride 9
-           + static_cast<size_t>(acc_cols) * 32 * 4;              // accumulators [col][lane]
+    return static_cast<size_t>(cm_buffers(stages)) * 32 * (kCmFeat + 1) * 8  // staging ring: query features / compacted hits, stride 9
+           + static_cast<size_t>(acc_cols) * 32 * 4;                        // accumulators [col][lane]
 }
 
 // col_cap: a chunk wider than col_cap columns is cut into ceil(n_cols / col_cap) column ranges of (nearly) equal width, each
@@ -93,7 +99,7 @@ inline CmShape cm_shape(uint32_t fm_words, uint32_t w_rows, uint32_t r_max, uint
     CmShape s;
     if (fm_words == 0 || n_chunks == 0 || col_cap == 0 || col_cap > 256u || r_max >= 65535u || e_max >= 65535u) return s;
     s.direct = w_rows <= kCmDirectRows;
-    s.words = s.direct ? w_rows : fm_words;
+    s.words = s.direct ? w_rows + 1u : fm_words;
     s.col_cap = col_cap;
     s.n_vc = n_vc;
     s.r_cap = r_max; s.e_cap = e_max; s.acc_cols = col_cap;
@@ -101,7 +107,7 @@ inline CmShape cm_shape(uint32_t fm_words, uint32_t w_rows, uint32_t r_max, uint
     // cover the global-memory latency; wide chunks (long accumulate phases) get by with two
     s.stages = s.acc_cols <= 16u ? 4u : 2u;
     uint32_t off = 16;  // header {bias range, n_cols, R, E}
-    s.off_lookup = off; off += cm_align16(s.words * 4u);
+    s.off_lookup = off; off += cm_align16(s.words * (s.direct ? 2u : 4u));
     if (!s.direct) {
         s.off_pre = off; off += cm_align16(s.words * 2u);
         s.off_rp = off;  off += cm_align16((r_max + 2u) * 2u);
@@ -182,7 +188,6 @@ xl_cm_build_images_kernel(const LayerDev L, const CmShape S, unsigned char* __re
     const ChunkHeader h = L.chunks[c];
     unsigned char* img = images + static_cast<uint64_t>(vc) * S.img_bytes;
     uint32_t* hdr = reinterpret_cast<uint32_t*>(img);
-    uint32_t* lookup = reinterpret_cast<uint32_t*>(img + S.off_lookup);
     float* ew = reinterpret_cast<float*>(img + S.off_ew);
     unsigned char* ec = img + S.off_ec;
     for (uint32_t i = threadIdx.x; i < S.img_bytes / 4u; i += blockDim.x) reinterpret_cast<uint32_t*>(img)[i] = 0u;
@@ -200,6 +205,7 @@ xl_cm_build_images_kernel(const LayerDev L, const CmShape S, unsigned char* __re
     const uint2* ent = L.entries + h.ent_off;
     unsigned short* rps = S.direct ? nullptr : reinterpret_cast<unsigned short*>(img + S.off_rp);
     if (!S.direct) {
+        uint32_t* lookup = reinterpret_cast<uint32_t*>(img + S.off_lookup);
         unsigned short* pre = reinterpret_cast<unsigned short*>(img + S.off_pre);
         const uint2* fm = L.featmap + static_cast<uint64_t>(c) * L.fm_words;
         for (uint32_t i = threadIdx.x; i < S.words; i += blockDim.x) {
@@ -241,8 +247,15 @@ xl_cm_build_images_kernel(const LayerDev L, const CmShape S, unsigned char* __re
                 ew[base + i] = __uint_as_float(en.y);
             }
             if (S.direct) {
-                const uint32_t f = ridx[r];
-                if (f < S.words) lookup[f] = base | ((base + len) << 16);  // an empty row reads as "no row": nothing to add
+                // start table: row r starts every feature after the previous row's up to its own (a feature without a row
+                // reads as an empty range, as does a row without entries in this column range); the last row's end
+                // closes the table at T[w_rows].  Rows ascend by feature.
+                unsigned short* starts = reinterpret_cast<unsigned short*>(img + S.off_lookup);
+                const uint32_t w_rows = S.words - 1u;
+                const uint32_t f = min(ridx[r], w_rows);
+                for (uint32_t g = r ? min(ridx[r - 1], w_rows) + 1u : 0u; g <= f; ++g) starts[g] = static_cast<unsigned short>(base);
+                if (r + 1u == R)
+                    for (uint32_t g = f + 1u; g <= w_rows; ++g) starts[g] = static_cast<unsigned short>(base + len);
             } else {
                 rps[r] = static_cast<unsigned short>(base);
             }
@@ -398,13 +411,15 @@ __device__ inline uint32_t cm_share_begin(const CmWork& w, uint32_t n_vc, uint32
 }
 
 // Diagnostics: built with -DPB200_CM_TRACE (tools/profile_cm_kernel.py) the score kernel records, for its last launch, every
-// CTA's %globaltimer start / end and every warp's clock64 cycles by phase in g_cm_trace:
-//   [0] grid, [1] warps per CTA, then per CTA: start ns, end ns, kCmMaxWarps x kCmPhases cycles.
+// CTA's %globaltimer start / end, every warp's clock64 cycles by phase, and its accumulate trips and useful slots (entries
+// added; a trip offers 32 x kCmSlots) in g_cm_trace:
+//   [0] grid, [1] warps per CTA, then per CTA: start ns, end ns, kCmMaxWarps x (kCmPhases cycles, trips, useful slots).
 // Without the define CmTrace is empty and the kernel is unchanged.
 enum { kCmPhImage, kCmPhStaging, kCmPhLookup, kCmPhAccumulate, kCmPhSlice, kCmPhases };
 #ifdef PB200_CM_TRACE
 constexpr uint32_t kCmTraceCtas = 1024;
-constexpr uint32_t kCmTraceCta = 2 + kCmMaxWarps * kCmPhases;
+constexpr uint32_t kCmTraceWarp = kCmPhases + 2;
+constexpr uint32_t kCmTraceCta = 2 + kCmMaxWarps * kCmTraceWarp;
 __device__ unsigned long long g_cm_trace[2 + kCmTraceCtas * kCmTraceCta];
 __device__ __forceinline__ unsigned long long cm_globaltimer() {
     unsigned long long t;
@@ -414,15 +429,21 @@ __device__ __forceinline__ unsigned long long cm_globaltimer() {
 struct CmTrace {
     unsigned long long start;
     long long t, ph[kCmPhases];
+    unsigned long long trips, slots;  // trips: warp-uniform; slots: this lane's
     __device__ void begin() {
         start = cm_globaltimer();
         t = clock64();
         for (int p = 0; p < kCmPhases; ++p) ph[p] = 0;
+        trips = slots = 0;
     }
     __device__ void mark(int p) {
         const long long n = clock64();
         ph[p] += n - t;
         t = n;
+    }
+    __device__ void count(uint32_t n_trips, uint32_t n_slots) {
+        trips += n_trips;
+        slots += n_slots;
     }
     __device__ void flush(int warp, int lane) {  // every thread of the CTA calls it once, last
         __syncthreads();
@@ -433,14 +454,20 @@ struct CmTrace {
             rec[0] = start;
             rec[1] = cm_globaltimer();
         }
-        if (lane == 0)
-            for (int p = 0; p < kCmPhases; ++p) rec[2 + warp * kCmPhases + p] = static_cast<unsigned long long>(ph[p]);
+        for (int d = 16; d > 0; d >>= 1) slots += __shfl_xor_sync(kFull, slots, d);
+        if (lane == 0) {
+            unsigned long long* wr = rec + 2 + warp * kCmTraceWarp;
+            for (int p = 0; p < kCmPhases; ++p) wr[p] = static_cast<unsigned long long>(ph[p]);
+            wr[kCmPhases] = trips;
+            wr[kCmPhases + 1] = slots;
+        }
     }
 };
 #else
 struct CmTrace {
     __device__ void begin() {}
     __device__ void mark(int) {}
+    __device__ void count(uint32_t, uint32_t) {}
     __device__ void flush(int, int) {}
 };
 #endif
@@ -456,7 +483,8 @@ xl_cm_scores_kernel(const LayerDev L, const QueryDev X, const CmWork w, const Cm
     // the image is only ever written by the bulk copy (async proxy), never by this kernel's stores: __restrict__ lets the
     // compiler hoist its loads above the accumulator stores
     const uint32_t* __restrict__ hdr_s = reinterpret_cast<const uint32_t*>(img);
-    const uint32_t* __restrict__ look_s = reinterpret_cast<const uint32_t*>(img + S.off_lookup);   // direct table, or feature-map bits
+    const unsigned short* __restrict__ start_s = reinterpret_cast<const unsigned short*>(img + S.off_lookup);  // direct: row starts
+    const uint32_t* __restrict__ look_s = reinterpret_cast<const uint32_t*>(img + S.off_lookup);   // else feature-map bits
     const unsigned short* __restrict__ pre_s = reinterpret_cast<const unsigned short*>(img + S.off_pre);
     const unsigned short* __restrict__ rp_s = reinterpret_cast<const unsigned short*>(img + S.off_rp);
     const float* __restrict__ ew_s = reinterpret_cast<const float*>(img + S.off_ew);
@@ -466,10 +494,11 @@ xl_cm_scores_kernel(const LayerDev L, const QueryDev X, const CmWork w, const Cm
     const int nwarps = blockDim.x >> 5;
     constexpr int kStride = kCmFeat + 1;
     constexpr int kBuf = 32 * kStride;                               // words per staging array
+    constexpr int kNBuf = static_cast<int>(cm_buffers(STAGES));
     unsigned char* mine = smem_raw + S.img_bytes + static_cast<size_t>(warp) * cm_warp_bytes(S.acc_cols, STAGES);
-    uint32_t* st_idx = reinterpret_cast<uint32_t*>(mine);            // [STAGES][32][kStride]
-    float* st_val = reinterpret_cast<float*>(st_idx + STAGES * kBuf); // [STAGES][32][kStride]
-    float* my_acc = st_val + STAGES * kBuf + lane;                   // [acc_cols][32], this lane's column of it
+    uint32_t* st_idx = reinterpret_cast<uint32_t*>(mine);            // [kNBuf][32][kStride]
+    float* st_val = reinterpret_cast<float*>(st_idx + kNBuf * kBuf); // [kNBuf][32][kStride]
+    float* my_acc = st_val + kNBuf * kBuf + lane;                    // [acc_cols][32], this lane's column of it
 
     __shared__ __align__(8) unsigned long long s_mbar;
     const uint32_t mbar = static_cast<uint32_t>(__cvta_generic_to_shared(&s_mbar));
@@ -511,53 +540,74 @@ xl_cm_scores_kernel(const LayerDev L, const QueryDev X, const CmWork w, const Cm
     const int sub = lane / kCmFeat, fl = lane % kCmFeat;
     uint32_t parity = 0;
 
-    // Adds the entries of this lane's hit rows (hit_r[0, cnt): entry ranges in feature order, hit_x: their x; n_ent entries
-    // in all) to its accumulators.  The rows are ONE stream of entries, kCmSlots per iteration whatever the rows' lengths, so
-    // the warp's trip count follows the lane with the most entries, not (most hits) x (longest row).  Slots of one iteration
-    // may hold entries of different rows, or a column a non-canonical row repeats: a slot whose column an earlier slot of the
-    // iteration also adds to starts from that slot's sum instead of the loaded accumulator, and the stores go out in slot
+    // The accumulate phase.  A lane's hit rows (entry ranges with their x, in feature order) are ONE stream of entries,
+    // kCmSlots per trip whatever the rows' lengths, and the stream runs across rounds: after round r's lookup the warp runs
+    // just enough trips for every lane to finish round r - 1's hits, and a lane that finishes early goes straight on into
+    // round r's.  So the trip count follows the largest BACKLOG of a lane (entries looked up but not yet added), not each
+    // round's busiest lane; one drain after the last round (with the bias row) runs to the busiest lane.  Slots of one trip
+    // may hold entries of different rows, or a column a non-canonical row repeats: a slot whose column an earlier slot of
+    // the trip also adds to starts from that slot's sum instead of the loaded accumulator, and the stores go out in slot
     // order -- every column sees exactly the sequential additions, in feature order (inference.hpp:788-811).
-    // hit_r / hit_x are read one past the last hit (the stride-9 row's spare word).
-    auto add_rows = [&](uint32_t cnt, uint32_t n_ent, const uint32_t* hit_r, const float* hit_x) {
-        const uint32_t trips = __reduce_max_sync(kFull, (n_ent + kCmSlots - 1u) / kCmSlots);
-        uint32_t h = 0, e = 0, ee = 0;
-        float x = 0.0f;
-        uint32_t next_r = hit_r[0];  // the next row's range and x, loaded ahead of their use
-        float next_x = hit_x[0];
+    //
+    // Stream state, carried from round to round: the current row's entries [e, ee) with factor x; hp, the next hit to
+    // take (a word offset in st_idx / st_val), loaded ahead into next_r / next_x; l1_end, one past the previous round's
+    // last hit.  The previous round's hits and the newest round's are read as one list: hp jumps from l1_end to the newest
+    // row.  Two rounds of hits are resident at once, hence the extra staging buffer (cm_buffers).  backlog: entries looked
+    // up but not yet added.
+    uint32_t e = 0, ee = 0, backlog = 0;
+    float x = 0.0f;
+    uint32_t hp = 0, l1_end = 0;  // word offsets in st_idx (and st_val)
+    // row / cnt / n_ent: the newest round's compacted hits (its row in st_idx; the x sit at the same place in st_val),
+    // their count and entries.  drain: run until every lane has added all of them, else only until every lane has
+    // finished the previous round's.
+    auto add_rows = [&](uint32_t row, uint32_t cnt, uint32_t n_ent, bool drain) {
+        const uint32_t l2_end = row + cnt;
+        const uint32_t avail = backlog + n_ent;
+        const uint32_t trips = __reduce_max_sync(kFull, ((drain ? avail : backlog) + kCmSlots - 1u) / kCmSlots);
+        if (hp == l1_end) hp = row;
+        // the next row's range and x, loaded ahead of their use (read one past the last hit: the stride-9 row's spare word)
+        uint32_t next_r = st_idx[hp];
+        float next_x = st_val[hp];
         for (uint32_t t = 0; t < trips; ++t) {
             uint32_t es[kCmSlots], cs[kCmSlots];
-            float xs[kCmSlots], v[kCmSlots];
+            float xs[kCmSlots], a[kCmSlots];
             bool on[kCmSlots];  // true for a prefix of the slots
 #pragma unroll
             for (int u = 0; u < kCmSlots; ++u) {
-                if (e == ee && h < cnt) {
+                if (e == ee && hp != l2_end) {
                     e = next_r & 0xFFFFu;
                     ee = next_r >> 16;
                     x = next_x;
-                    ++h;
-                    next_r = hit_r[h];
-                    next_x = hit_x[h];
+                    ++hp;
+                    if (hp == l1_end) hp = row;
+                    next_r = st_idx[hp];
+                    next_x = st_val[hp];
                 }
                 on[u] = e < ee;
-                es[u] = e;  // an idle slot reads a valid (unused) entry
+                es[u] = e;  // an idle slot (only once the lane's backlog is all added) reads a valid, unused entry
                 xs[u] = x;
                 e += on[u] ? 1u : 0u;
             }
 #pragma unroll
             for (int u = 0; u < kCmSlots; ++u) cs[u] = ec_s[es[u]];
 #pragma unroll
-            for (int u = 0; u < kCmSlots; ++u) v[u] = my_acc[cs[u] * 32u];
+            for (int u = 0; u < kCmSlots; ++u) a[u] = my_acc[cs[u] * 32u];
 #pragma unroll
             for (int u = 0; u < kCmSlots; ++u) {
-                float a = v[u];
+                float sum = a[u];
 #pragma unroll
-                for (int p = 0; p < u; ++p) a = (cs[p] == cs[u]) ? v[p] : a;  // v[p] already holds slot p's sum
-                v[u] = __fadd_rn(a, __fmul_rn(xs[u], ew_s[es[u]]));
+                for (int p = 0; p < u; ++p) sum = (cs[p] == cs[u]) ? a[p] : sum;  // a[p] already holds slot p's sum
+                a[u] = __fadd_rn(sum, __fmul_rn(xs[u], ew_s[es[u]]));
             }
 #pragma unroll
             for (int u = 0; u < kCmSlots; ++u)
-                if (on[u]) my_acc[cs[u] * 32u] = v[u];
+                if (on[u]) my_acc[cs[u] * 32u] = a[u];
         }
+        // every slot of a trip adds an entry while the lane has one, so the previous round's hits are all added now
+        const uint32_t added = min(avail, trips * kCmSlots);
+        backlog = avail - added;
+        trace.count(trips, added);
+        l1_end = l2_end;
     };
 
     for (uint32_t i = begin; i < end;) {
@@ -624,9 +674,13 @@ xl_cm_scores_kernel(const LayerDev L, const QueryDev X, const CmWork w, const Cm
             for (uint32_t col = 0; col < n_cols; ++col) my_acc[col * 32] = 0.0f;
             trace.mark(kCmPhSlice);
             uint32_t prev_f = kCmEmpty;
+            e = ee = backlog = 0;
+            x = 0.0f;
+            hp = l1_end = 0;
             int buf = 0;
-            for (uint32_t t0 = 0; t0 < qn_max; t0 += kCmFeat, buf = (buf + 1 == STAGES) ? 0 : buf + 1) {
-                stage_round(t0 + (STAGES - 1) * kCmFeat, (buf + STAGES - 1) % STAGES);  // refills the buffer consumed last round
+            for (uint32_t t0 = 0; t0 < qn_max; t0 += kCmFeat, buf = (buf + 1 == kNBuf) ? 0 : buf + 1) {
+                // refills the buffer of round r - 2, whose hits the previous round's trips finished
+                stage_round(t0 + (STAGES - 1) * kCmFeat, (buf + STAGES - 1) % kNBuf);
                 cm_cp_async_wait<STAGES - 1>();
                 __syncwarp();
                 trace.mark(kCmPhStaging);
@@ -650,7 +704,7 @@ xl_cm_scores_kernel(const LayerDev L, const QueryDev X, const CmWork w, const Cm
                     uint32_t range = 0;
                     if (static_cast<uint32_t>(k) < n_here && !dup && f < L.w_rows) {
                         if (DIRECT) {
-                            range = look_s[f];
+                            range = static_cast<uint32_t>(start_s[f]) | (static_cast<uint32_t>(start_s[f + 1]) << 16);
                         } else {
                             const uint32_t word = look_s[f >> 5];
                             const uint32_t bit = f & 31u;
@@ -674,20 +728,21 @@ xl_cm_scores_kernel(const LayerDev L, const QueryDev X, const CmWork w, const Cm
                     }
                 }
                 trace.mark(kCmPhLookup);
-                // phase 2: the hit rows' entries, in feature order, into this lane's accumulators
-                add_rows(cnt, n_ent, my_idx, my_val);
+                // phase 2: the rest of the previous round's hit rows, then as much of this round's as the trips hold, in
+                // feature order, into this lane's accumulators
+                add_rows(static_cast<uint32_t>(buf * kBuf + lane * kStride), cnt, n_ent, false);
                 trace.mark(kCmPhAccumulate);
                 __syncwarp();
             }
             cm_cp_async_wait<0>();
-            {  // bias row last (inference.hpp:806-811), through the staging buffer of round 0 (no copy is in flight any more)
-                uint32_t* b_idx = st_idx + lane * kStride;
-                float* b_val = st_val + lane * kStride;
+            {  // drain, bias row last (inference.hpp:806-811): the bias row is the last "round", staged in the buffer after the
+               // last round's (its hits are gone, and no copy is in flight any more)
+                const uint32_t o = static_cast<uint32_t>(buf * kBuf + lane * kStride);
                 const uint32_t b0 = bias_range & 0xFFFFu, b1 = bias_range >> 16;
                 const bool live = have && b1 > b0;
-                b_idx[0] = bias_range;
-                b_val[0] = L.bias;
-                add_rows(live ? 1u : 0u, live ? b1 - b0 : 0u, b_idx, b_val);
+                st_idx[o] = bias_range;
+                st_val[o] = L.bias;
+                add_rows(o, live ? 1u : 0u, live ? b1 - b0 : 0u, true);
             }
             trace.mark(kCmPhAccumulate);
             if (have) {

@@ -39,7 +39,7 @@ struct LayerDev {
 struct CmShape {  // load-time, per layer: geometry of the chunk images
     bool ok = false;
     bool direct = false;
-    uint32_t words = 0;      // direct: w_rows (table entries); else fm_words (feature-map cells)
+    uint32_t words = 0;      // direct: w_rows + 1 (u16 row starts); else fm_words (feature-map cells)
     uint32_t r_cap = 0, e_cap = 0, acc_cols = 0;
     uint32_t stages = 2;     // depth of the per-warp cp.async ring of query-feature rounds
     uint32_t col_cap = 0;    // widest column range: wider chunks are cut into ranges ("virtual chunks"), each with its own image

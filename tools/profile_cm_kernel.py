@@ -5,7 +5,8 @@ the eurlex-4k workload of bench.py (same model and query seeds) through it, and 
 xl_cm_scores_kernel (the leaf layer):
   * per-CTA elapsed time from %globaltimer (max / mean / min over the CTAs, and max / mean);
   * per-warp clock64 cycles by phase: image wait, query staging wait, lookup + compaction, accumulate, slice set-up +
-    output (mean over the warps, and the share of each phase).
+    output (mean over the warps, and the share of each phase);
+  * accumulate trips per warp and lane efficiency: entries added / (trips x 32 lanes x 4 slots).
 The product build never defines PB200_CM_TRACE.
 
     python tools/profile_cm_kernel.py [--queries N] [--json OUT]
@@ -26,6 +27,8 @@ sys.path.insert(0, ROOT)
 PHASES = ["image_wait", "staging_wait", "lookup_compact", "accumulate", "slice_setup_output"]
 MAX_WARPS = 16  # kCmMaxWarps
 TRACE_CTAS = 1024  # kCmTraceCtas
+WARP_FIELDS = len(PHASES) + 2  # kCmTraceWarp: phase cycles, trips, useful slots
+SLOTS = 4  # kCmSlots
 
 
 def build_traced(out_dir):
@@ -68,7 +71,7 @@ def main():
         c.pb200_xlinear_get_kernel_ids(m.model.model_chain, kid)
         if kid[2 * (depth - 1)] != 4:
             raise RuntimeError(f"the leaf layer did not run the chunk-major kernel (score kernel id {kid[2 * (depth - 1)]})")
-        per_cta = 2 + MAX_WARPS * len(PHASES)
+        per_cta = 2 + MAX_WARPS * WARP_FIELDS
         buf = (ctypes.c_ulonglong * (2 + TRACE_CTAS * per_cta))()
         if c.pb200_cm_trace_fetch(buf, len(buf)) != 0:
             raise RuntimeError("pb200_cm_trace_fetch failed")
@@ -76,7 +79,9 @@ def main():
     grid, warps = int(raw[0]), int(raw[1])
     rec = raw[2: 2 + grid * per_cta].reshape(grid, per_cta)
     cta_us = (rec[:, 1].astype(np.float64) - rec[:, 0].astype(np.float64)) / 1e3
-    cyc = rec[:, 2:].reshape(grid, MAX_WARPS, len(PHASES))[:, :warps, :].astype(np.float64)
+    per_warp = rec[:, 2:].reshape(grid, MAX_WARPS, WARP_FIELDS)[:, :warps, :].astype(np.float64)
+    cyc = per_warp[:, :, : len(PHASES)]
+    trips, slots = per_warp[:, :, len(PHASES)], per_warp[:, :, len(PHASES) + 1]
     phase_mean = cyc.mean(axis=(0, 1))
     warp_total = cyc.sum(axis=2)
     out = {
@@ -86,6 +91,8 @@ def main():
         "warp_cycles": {"mean_total": float(warp_total.mean()), "max_total": float(warp_total.max()),
                         "phases_mean": {p: float(v) for p, v in zip(PHASES, phase_mean)},
                         "phases_share": {p: float(v / phase_mean.sum()) for p, v in zip(PHASES, phase_mean)}},
+        "accumulate": {"trips_per_warp": float(trips.mean()), "entries_per_warp": float(slots.mean()),
+                       "lane_efficiency": float(slots.sum() / max(trips.sum() * 32 * SLOTS, 1.0))},
     }
     print(f"leaf: {out['queries']} queries, {grid} CTAs x {warps} warps")
     print("CTA elapsed (us): max %.1f  mean %.1f  min %.1f  max/mean %.3f" % (
@@ -93,6 +100,9 @@ def main():
     print("warp cycles: mean total %.0f, max total %.0f" % (out["warp_cycles"]["mean_total"], out["warp_cycles"]["max_total"]))
     for p in PHASES:
         print("  %-20s %12.0f  %5.1f %%" % (p, out["warp_cycles"]["phases_mean"][p], 100 * out["warp_cycles"]["phases_share"][p]))
+    acc = out["accumulate"]
+    print("accumulate: %.0f trips and %.0f entries per warp, lane efficiency %.3f" % (
+        acc["trips_per_warp"], acc["entries_per_warp"], acc["lane_efficiency"]))
     if args.json:
         with open(args.json, "w") as f:
             json.dump(out, f, indent=1)
