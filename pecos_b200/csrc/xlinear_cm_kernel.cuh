@@ -13,11 +13,12 @@
 //     prefix per 32 features: "is f a row, and which one" = one shared-memory word + popcount) and 16-bit row pointers;
 //   * per call the pairs are bucketed by chunk on the device (count -> scan -> scatter; the reference's b_sort_by_chunk,
 //     pecos/core/xmc/inference.hpp:985-993);
-//   * the score kernel is PERSISTENT: one CTA per SM takes a contiguous share of the chunk-sorted pair list holding 1/grid
-//     of the estimated work (a pair's cost grows with its chunk's entry count: cm_pair_cost), so it meets only a few chunks
-//     and no CTA is left with the widest chunks' pairs; a chunk's image arrives by ONE bulk asynchronous copy
-//     (cp.async.bulk + mbarrier, the TMA engine's non-tensor form) and serves every pair of the run; warps take 32-pair
-//     slices of the run;
+//   * the score kernel is PERSISTENT: one CTA per SM starts on the chunk where its 1/grid share of the estimated work
+//     begins (a pair's cost grows with its chunk's entry count: cm_pair_cost), stages that chunk's image by ONE bulk
+//     asynchronous copy (cp.async.bulk + mbarrier, the TMA engine's non-tensor form), and its warps CLAIM 32-pair slices of
+//     the chunk from a per-chunk cursor (one atomicAdd per slice) until the chunk runs dry; then the CTA moves to the chunk
+//     with the most unclaimed estimated work.  Work moves between SMs at run time, so the launch ends when the last slice
+//     does, not when the CTA with the most expensive static share does;
 //   * a lane walks its pair's query features in ascending order (staged global -> shared by cp.async, rounds of 8 in
 //     flight), compacts the hits of a round in place as {entry range, x}, then streams the hit rows' entries as one flat
 //     stream, kCmSlots entries per trip across row boundaries AND across rounds: after round r's lookup the warp runs only
@@ -50,6 +51,7 @@ struct CmWork {
     uint64_t* cost_ptr;     // [n_chunks + 1] exclusive prefix of the chunks' estimated work (cm_pair_cost x pairs)
     uint32_t* pair_q;       // [pairs] query of a pair, grouped by chunk
     uint32_t* pair_pos;     // [pairs] candidate position of the pair's first column inside the query's row
+    uint32_t* claim;        // [n_chunks] first unclaimed pair of a chunk's bucket (at or past bucket_ptr[c + 1]: none left)
 };
 
 struct CmPlan {  // per call
@@ -324,7 +326,7 @@ __device__ __forceinline__ uint64_t warp_incl_scan64(uint64_t v, int lane) {
 }
 
 // single CTA: exclusive scans of the pair counts (bucket offsets) and of the chunks' estimated work (cost_ptr); count[]
-// becomes the scatter cursor.  A chunk's entry count is read from its image header.
+// becomes the scatter cursor and claim[] the score kernel's claim cursor.  A chunk's entry count is read from its image header.
 __global__ void __launch_bounds__(1024)
 xl_cm_scan_kernel(const uint32_t n_chunks, CmWork w, const unsigned char* __restrict__ images, const uint32_t img_bytes,
                   const uint32_t w_rows) {
@@ -359,6 +361,7 @@ xl_cm_scan_kernel(const uint32_t n_chunks, CmWork w, const unsigned char* __rest
             w.bucket_ptr[c] = ex_p;
             w.cost_ptr[c] = ex_c;
             w.count[c] = ex_p;  // cursor
+            w.claim[c] = ex_p;
         }
         __syncthreads();
         if (threadIdx.x == 1023) { carry_pairs = ex_p + n; carry_cost = ex_c + cost; }
@@ -391,36 +394,34 @@ xl_cm_scatter_kernel(const LayerDev L, const uint32_t* __restrict__ beam_id, con
     }
 }
 
-// First pair of share b of the chunk-sorted pair list when it is cut into `shares` contiguous shares of (nearly) equal
-// estimated work (cost_ptr).  A cut inside a chunk falls on the nearest pair, rounded to a whole 32-pair slice of the chunk.
-// Monotone in b, so the shares tile the list.
-__device__ inline uint32_t cm_share_begin(const CmWork& w, uint32_t n_vc, uint32_t b, uint32_t shares) {
-    if (b >= shares) return w.bucket_ptr[n_vc];
+// The (virtual) chunk CTA b of `shares` starts on: the one where share b begins when the chunk-sorted pair list is cut into
+// shares of equal estimated work (cost_ptr), so the CTAs start spread over the chunks in proportion to their work.
+// n_vc: no pairs at all.
+__device__ inline uint32_t cm_start_chunk(const CmWork& w, uint32_t n_vc, uint32_t b, uint32_t shares) {
     const uint64_t T = w.cost_ptr[n_vc];
-    const uint64_t t = static_cast<uint64_t>(T / shares) * b + (T % shares) * b / shares;  // floor(T * b / shares) without overflow
-    if (t >= T) return w.bucket_ptr[n_vc];
+    if (T == 0) return n_vc;
+    const uint64_t t = static_cast<uint64_t>(T / shares) * b + (T % shares) * b / shares;  // floor(T * b / shares) < T without overflow
     uint32_t lo = 0, hi = n_vc;  // largest c with cost_ptr[c] <= t: a non-empty chunk, as cost_ptr[c + 1] > t
     while (hi - lo > 1) {
         const uint32_t mid = (lo + hi) >> 1;
         if (w.cost_ptr[mid] <= t) lo = mid; else hi = mid;
     }
-    const uint32_t n = w.bucket_ptr[lo + 1] - w.bucket_ptr[lo];
-    const uint64_t unit = (w.cost_ptr[lo + 1] - w.cost_ptr[lo]) / n;  // every pair of a chunk costs the same
-    const uint64_t k = ((t - w.cost_ptr[lo] + unit / 2) / unit + 16u) & ~static_cast<uint64_t>(31);
-    return w.bucket_ptr[lo] + (k < n ? static_cast<uint32_t>(k) : n);
+    return lo;
 }
 
 // Diagnostics: built with -DPB200_CM_TRACE (tools/profile_cm_kernel.py) the score kernel records, for its last launch, every
-// CTA's %globaltimer start / end, every warp's clock64 cycles by phase, and its accumulate trips and useful slots (entries
-// added; a trip offers 32 x kCmSlots) in g_cm_trace:
-//   [0] grid, [1] warps per CTA, then per CTA: start ns, end ns, kCmMaxWarps x (kCmPhases cycles, trips, useful slots).
+// CTA's %globaltimer start / end and images staged, every warp's clock64 cycles by phase, its accumulate trips and useful
+// slots (entries added; a trip offers 32 x kCmSlots), and the slices and pairs it scored, in g_cm_trace:
+//   [0] grid, [1] warps per CTA, [2] pairs of the launch, then per CTA: start ns, end ns, images staged,
+//   kCmMaxWarps x (kCmPhases cycles, trips, useful slots, slices, pairs).
+// The image phase covers a chunk switch: the barrier, the choice of the next chunk and the bulk copy.
 // Without the define CmTrace is empty and the kernel is unchanged.
 enum { kCmPhImage, kCmPhStaging, kCmPhLookup, kCmPhAccumulate, kCmPhSlice, kCmPhases };
 #ifdef PB200_CM_TRACE
 constexpr uint32_t kCmTraceCtas = 1024;
-constexpr uint32_t kCmTraceWarp = kCmPhases + 2;
-constexpr uint32_t kCmTraceCta = 2 + kCmMaxWarps * kCmTraceWarp;
-__device__ unsigned long long g_cm_trace[2 + kCmTraceCtas * kCmTraceCta];
+constexpr uint32_t kCmTraceWarp = kCmPhases + 4;
+constexpr uint32_t kCmTraceCta = 3 + kCmMaxWarps * kCmTraceWarp;
+__device__ unsigned long long g_cm_trace[3 + kCmTraceCtas * kCmTraceCta];
 __device__ __forceinline__ unsigned long long cm_globaltimer() {
     unsigned long long t;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
@@ -430,12 +431,18 @@ struct CmTrace {
     unsigned long long start;
     long long t, ph[kCmPhases];
     unsigned long long trips, slots;  // trips: warp-uniform; slots: this lane's
+    unsigned long long slices, pairs, images;  // slices, pairs: warp-uniform; images: CTA-uniform
     __device__ void begin() {
         start = cm_globaltimer();
         t = clock64();
         for (int p = 0; p < kCmPhases; ++p) ph[p] = 0;
-        trips = slots = 0;
+        trips = slots = slices = pairs = images = 0;
     }
+    __device__ void slice(uint32_t n_pairs) {
+        ++slices;
+        pairs += n_pairs;
+    }
+    __device__ void staged() { ++images; }
     __device__ void mark(int p) {
         const long long n = clock64();
         ph[p] += n - t;
@@ -445,21 +452,24 @@ struct CmTrace {
         trips += n_trips;
         slots += n_slots;
     }
-    __device__ void flush(int warp, int lane) {  // every thread of the CTA calls it once, last
+    __device__ void flush(int warp, int lane, uint32_t launch_pairs) {  // every thread of the CTA calls it once, last
         __syncthreads();
         if (blockIdx.x >= kCmTraceCtas) return;
-        unsigned long long* rec = g_cm_trace + 2 + blockIdx.x * kCmTraceCta;
+        unsigned long long* rec = g_cm_trace + 3 + blockIdx.x * kCmTraceCta;
         if (threadIdx.x == 0) {
-            if (blockIdx.x == 0) { g_cm_trace[0] = gridDim.x; g_cm_trace[1] = blockDim.x >> 5; }
+            if (blockIdx.x == 0) { g_cm_trace[0] = gridDim.x; g_cm_trace[1] = blockDim.x >> 5; g_cm_trace[2] = launch_pairs; }
             rec[0] = start;
             rec[1] = cm_globaltimer();
+            rec[2] = images;
         }
         for (int d = 16; d > 0; d >>= 1) slots += __shfl_xor_sync(kFull, slots, d);
         if (lane == 0) {
-            unsigned long long* wr = rec + 2 + warp * kCmTraceWarp;
+            unsigned long long* wr = rec + 3 + warp * kCmTraceWarp;
             for (int p = 0; p < kCmPhases; ++p) wr[p] = static_cast<unsigned long long>(ph[p]);
             wr[kCmPhases] = trips;
             wr[kCmPhases + 1] = slots;
+            wr[kCmPhases + 2] = slices;
+            wr[kCmPhases + 3] = pairs;
         }
     }
 };
@@ -468,7 +478,9 @@ struct CmTrace {
     __device__ void begin() {}
     __device__ void mark(int) {}
     __device__ void count(uint32_t, uint32_t) {}
-    __device__ void flush(int, int) {}
+    __device__ void slice(uint32_t) {}
+    __device__ void staged() {}
+    __device__ void flush(int, int, uint32_t) {}
 };
 #endif
 
@@ -510,29 +522,6 @@ xl_cm_scores_kernel(const LayerDev L, const QueryDev X, const CmWork w, const Cm
     CmTrace trace;
     trace.begin();
 
-    // ---- this CTA's contiguous share of the (virtual-)chunk-sorted pair list: an equal share of the estimated WORK
-    const uint32_t n_vc = S.n_vc;
-    uint32_t begin, end;
-    if constexpr (PREFIX) {  // every pair costs the same: equal slices of the rows
-        begin = static_cast<uint32_t>(static_cast<uint64_t>(P.rows) * blockIdx.x / gridDim.x);
-        end = static_cast<uint32_t>(static_cast<uint64_t>(P.rows) * (blockIdx.x + 1u) / gridDim.x);
-    } else {
-        begin = cm_share_begin(w, n_vc, blockIdx.x, gridDim.x);
-        end = cm_share_begin(w, n_vc, blockIdx.x + 1u, gridDim.x);
-    }
-    if (begin >= end) {
-        trace.flush(warp, lane);
-        return;
-    }
-    uint32_t c = 0;
-    if constexpr (!PREFIX) {
-        uint32_t lo = 0, hi = n_vc;  // largest c with bucket_ptr[c] <= begin (then skip empty buckets forward)
-        while (hi - lo > 1) {
-            const uint32_t mid = (lo + hi) >> 1;
-            if (w.bucket_ptr[mid] <= begin) lo = mid; else hi = mid;
-        }
-        c = lo;
-    }
     // staging geometry: one warp-wide cp.async instruction copies kCmFeat consecutive features of kPerIter pairs; this lane
     // always serves feature fl of the pairs sub, sub + kPerIter, ...
     constexpr int kPerIter = 32 / kCmFeat;
@@ -610,179 +599,235 @@ xl_cm_scores_kernel(const LayerDev L, const QueryDev X, const CmWork w, const Cm
         l1_end = l2_end;
     };
 
-    for (uint32_t i = begin; i < end;) {
-        uint32_t run_end = end;
-        if constexpr (!PREFIX) {
-            while (w.bucket_ptr[c + 1] <= i) ++c;                    // virtual chunk holding pair i
-            run_end = min(end, w.bucket_ptr[c + 1]);
-        }
-        // ---- stage the image: ONE bulk copy (every warp has left the previous image: barrier first)
-        __syncthreads();
+    // ---- stage the image of virtual chunk c: ONE bulk copy (the caller has made sure every warp has left the previous image)
+    uint32_t bias_range = 0, n_cols = 0;
+    auto stage_image = [&](uint32_t c) {
         if (threadIdx.x == 0) cm_bulk_load(static_cast<uint32_t>(__cvta_generic_to_shared(img)), images + static_cast<uint64_t>(c) * S.img_bytes, S.img_bytes, mbar);
         cm_mbar_wait(mbar, parity);
         parity ^= 1u;
+        trace.staged();
         trace.mark(kCmPhImage);
-        const uint32_t bias_range = hdr_s[0];
-        const uint32_t n_cols = hdr_s[1];
+        bias_range = hdr_s[0];
+        n_cols = hdr_s[1];
+    };
 
-        // ---- warps take 32-pair slices of the run
-        for (uint32_t s0 = i + static_cast<uint32_t>(warp) * 32u; s0 < run_end; s0 += static_cast<uint32_t>(nwarps) * 32u) {
-            const uint32_t pidx = s0 + lane;
-            const bool have = pidx < run_end;
-            uint32_t q = 0, pos = 0, qn = 0;
-            uint64_t qb = 0;
-            if (have) {
-                if constexpr (PREFIX) {
-                    q = pidx;
-                } else {
-                    q = w.pair_q[pidx];
-                    pos = w.pair_pos[pidx];
-                }
-                qb = X.row_ptr[q] - X.nnz_base;
-                qn = static_cast<uint32_t>(X.row_ptr[q + 1] - X.nnz_base - qb);
+    // ---- one warp scores the pairs [s0, s_end) (at most 32, one per lane) of the staged chunk
+    auto score_slice = [&](uint32_t s0, uint32_t s_end) {
+        const uint32_t pidx = s0 + lane;
+        const bool have = pidx < s_end;
+        uint32_t q = 0, pos = 0, qn = 0;
+        uint64_t qb = 0;
+        if (have) {
+            if constexpr (PREFIX) {
+                q = pidx;
+            } else {
+                q = w.pair_q[pidx];
+                pos = w.pair_pos[pidx];
             }
-            const uint32_t qn_max = __reduce_max_sync(kFull, qn);
-            // the pairs this lane copies for: source pointers (feature fl of the pair's row) and row lengths, once per slice
-            uint32_t src_o[kIters], src_n[kIters];  // offsets fit 32 bits: a tile of queries holds < 2^32 non-zeros
-#pragma unroll
-            for (int it = 0; it < kIters; ++it) {
-                const int pi = it * kPerIter + sub;
-                src_o[it] = static_cast<uint32_t>(__shfl_sync(kFull, qb, pi)) + fl;
-                src_n[it] = __shfl_sync(kFull, qn, pi);
-            }
-            // query features travel global -> shared by cp.async through a ring of STAGES buffers: rounds r + 1 .. r + STAGES - 1
-            // are in flight while round r is processed.  Row i of a buffer = the next kCmFeat features of the slice's pair i
-            // (stride 9 words: the lane-per-row reads are bank-conflict free).  A (possibly empty) group is committed for every
-            // round slot, so "all but the newest STAGES - 1 groups are complete" always means "round r has landed".
-            auto stage_round = [&](uint32_t t0, int buf) {
-                if (t0 < qn_max) {
-                    uint32_t* di = st_idx + buf * kBuf + sub * kStride + fl;
-                    float* dv = st_val + buf * kBuf + sub * kStride + fl;
-#pragma unroll
-                    for (int it = 0; it < kIters; ++it) {
-                        if (t0 + fl < src_n[it]) {
-                            cm_cp_async4(di + it * kPerIter * kStride, X.col_idx + src_o[it] + t0);
-                            cm_cp_async4(dv + it * kPerIter * kStride, X.val + src_o[it] + t0);
-                        }
-                    }
-                }
-                cm_cp_async_commit();
-            };
-            __syncwarp();
-#pragma unroll
-            for (int st = 0; st < STAGES - 1; ++st) stage_round(static_cast<uint32_t>(st) * kCmFeat, st);
-            for (uint32_t col = 0; col < n_cols; ++col) my_acc[col * 32] = 0.0f;
-            trace.mark(kCmPhSlice);
-            uint32_t prev_f = kCmEmpty;
-            e = ee = backlog = 0;
-            x = 0.0f;
-            hp = l1_end = 0;
-            int buf = 0;
-            for (uint32_t t0 = 0; t0 < qn_max; t0 += kCmFeat, buf = (buf + 1 == kNBuf) ? 0 : buf + 1) {
-                // refills the buffer of round r - 2, whose hits the previous round's trips finished
-                stage_round(t0 + (STAGES - 1) * kCmFeat, (buf + STAGES - 1) % kNBuf);
-                cm_cp_async_wait<STAGES - 1>();
-                __syncwarp();
-                trace.mark(kCmPhStaging);
-                uint32_t* my_idx = st_idx + buf * kBuf + lane * kStride;
-                float* my_val = st_val + buf * kBuf + lane * kStride;
-                const uint32_t n_here = (qn > t0) ? min(static_cast<uint32_t>(kCmFeat), qn - t0) : 0u;
-                // phase 1: look the features up -- all loads of the round are issued before the first store (eight independent
-                // feature / lookup / value loads in flight per lane) -- then compact the hits IN PLACE as {entry range, x}
-                uint32_t fq[kCmFeat], rq[kCmFeat];
-                float xq[kCmFeat];
-#pragma unroll
-                for (int k = 0; k < kCmFeat; ++k) {
-                    fq[k] = (static_cast<uint32_t>(k) < n_here) ? my_idx[k] : kCmEmpty;
-                    xq[k] = my_val[k];
-                }
-#pragma unroll
-                for (int k = 0; k < kCmFeat; ++k) {
-                    const uint32_t f = fq[k];
-                    const bool dup = (f == prev_f);  // a repeated column index only counts once (the first occurrence)
-                    if (static_cast<uint32_t>(k) < n_here) prev_f = f;
-                    uint32_t range = 0;
-                    if (static_cast<uint32_t>(k) < n_here && !dup && f < L.w_rows) {
-                        if (DIRECT) {
-                            range = static_cast<uint32_t>(start_s[f]) | (static_cast<uint32_t>(start_s[f + 1]) << 16);
-                        } else {
-                            const uint32_t word = look_s[f >> 5];
-                            const uint32_t bit = f & 31u;
-                            if ((word >> bit) & 1u) {
-                                const uint32_t row = static_cast<uint32_t>(pre_s[f >> 5]) + __popc(word & ((1u << bit) - 1u));
-                                range = static_cast<uint32_t>(rp_s[row]) | (static_cast<uint32_t>(rp_s[row + 1]) << 16);
-                            }
-                        }
-                    }
-                    rq[k] = range;
-                }
-                uint32_t cnt = 0, n_ent = 0;
-#pragma unroll
-                for (int k = 0; k < kCmFeat; ++k) {
-                    const uint32_t e0 = rq[k] & 0xFFFFu, e1 = rq[k] >> 16;
-                    if (e1 > e0) {
-                        my_idx[cnt] = rq[k];
-                        my_val[cnt] = xq[k];
-                        ++cnt;
-                        n_ent += e1 - e0;
-                    }
-                }
-                trace.mark(kCmPhLookup);
-                // phase 2: the rest of the previous round's hit rows, then as much of this round's as the trips hold, in
-                // feature order, into this lane's accumulators
-                add_rows(static_cast<uint32_t>(buf * kBuf + lane * kStride), cnt, n_ent, false);
-                trace.mark(kCmPhAccumulate);
-                __syncwarp();
-            }
-            cm_cp_async_wait<0>();
-            {  // drain, bias row last (inference.hpp:806-811): the bias row is the last "round", staged in the buffer after the
-               // last round's (its hits are gone, and no copy is in flight any more)
-                const uint32_t o = static_cast<uint32_t>(buf * kBuf + lane * kStride);
-                const uint32_t b0 = bias_range & 0xFFFFu, b1 = bias_range >> 16;
-                const bool live = have && b1 > b0;
-                st_idx[o] = bias_range;
-                st_val[o] = L.bias;
-                add_rows(o, live ? 1u : 0u, live ? b1 - b0 : 0u, true);
-            }
-            trace.mark(kCmPhAccumulate);
-            if (have) {
-                if constexpr (PREFIX) {
-                    // layer 0 keeps all n0 candidates: its top-k is the descending order of their exact keys (unused keys
-                    // are 0 and sort last; a real key never is 0)
-                    unsigned long long key[kCmPrefixTop0];
-#pragma unroll
-                    for (uint32_t j = 0; j < kCmPrefixTop0; ++j)
-                        key[j] = j < P.n0 ? xl_exact_key(xl_transform(my_acc[j * 32], P.pp_kind, P.pp_p), j) : 0ull;
-#pragma unroll
-                    for (uint32_t a = 1; a < kCmPrefixTop0; ++a)
-#pragma unroll
-                        for (uint32_t b = a; b > 0; --b)
-                            if (key[b] > key[b - 1]) { const unsigned long long t = key[b]; key[b] = key[b - 1]; key[b - 1] = t; }
-                    // layer 1's beam slot r is the chunk of layer-0 rank r: its children's raw scores go to the next
-                    // positions of the candidate row, in column order
-                    const uint64_t o = static_cast<uint64_t>(q) * P.beam_stride;
-                    float* dst = P.cand1 + static_cast<uint64_t>(q) * P.cand1_stride;
-#pragma unroll
-                    for (uint32_t r = 0; r < kCmPrefixTop0; ++r) {
-                        if (r < P.n0) {
-                            const uint32_t j = xl_exact_key_pos(key[r]);
-                            P.beam_id[o + r] = j;
-                            P.beam_val[o + r] = xl_exact_key_value(key[r]);
-                            const ChunkHeader h = P.chunks1[j];
-                            const float* src = my_acc + (P.n0 + h.col_begin) * 32u;
-                            for (uint32_t col = 0; col < h.n_cols; ++col) dst[col] = src[col * 32];
-                            dst += h.n_cols;
-                        }
-                    }
-                    P.beam_cnt[q] = P.n0;
-                } else {
-                    float* dst = cand + static_cast<uint64_t>(q) * cand_stride_q + pos;
-                    for (uint32_t col = 0; col < n_cols; ++col) dst[col] = my_acc[col * 32];
-                }
-            }
-            trace.mark(kCmPhSlice);
+            qb = X.row_ptr[q] - X.nnz_base;
+            qn = static_cast<uint32_t>(X.row_ptr[q + 1] - X.nnz_base - qb);
         }
-        i = run_end;
+        const uint32_t qn_max = __reduce_max_sync(kFull, qn);
+        // the pairs this lane copies for: source pointers (feature fl of the pair's row) and row lengths, once per slice
+        uint32_t src_o[kIters], src_n[kIters];  // offsets fit 32 bits: a tile of queries holds < 2^32 non-zeros
+#pragma unroll
+        for (int it = 0; it < kIters; ++it) {
+            const int pi = it * kPerIter + sub;
+            src_o[it] = static_cast<uint32_t>(__shfl_sync(kFull, qb, pi)) + fl;
+            src_n[it] = __shfl_sync(kFull, qn, pi);
+        }
+        // query features travel global -> shared by cp.async through a ring of STAGES buffers: rounds r + 1 .. r + STAGES - 1
+        // are in flight while round r is processed.  Row i of a buffer = the next kCmFeat features of the slice's pair i
+        // (stride 9 words: the lane-per-row reads are bank-conflict free).  A (possibly empty) group is committed for every
+        // round slot, so "all but the newest STAGES - 1 groups are complete" always means "round r has landed".
+        auto stage_round = [&](uint32_t t0, int buf) {
+            if (t0 < qn_max) {
+                uint32_t* di = st_idx + buf * kBuf + sub * kStride + fl;
+                float* dv = st_val + buf * kBuf + sub * kStride + fl;
+#pragma unroll
+                for (int it = 0; it < kIters; ++it) {
+                    if (t0 + fl < src_n[it]) {
+                        cm_cp_async4(di + it * kPerIter * kStride, X.col_idx + src_o[it] + t0);
+                        cm_cp_async4(dv + it * kPerIter * kStride, X.val + src_o[it] + t0);
+                    }
+                }
+            }
+            cm_cp_async_commit();
+        };
+        __syncwarp();
+#pragma unroll
+        for (int st = 0; st < STAGES - 1; ++st) stage_round(static_cast<uint32_t>(st) * kCmFeat, st);
+        for (uint32_t col = 0; col < n_cols; ++col) my_acc[col * 32] = 0.0f;
+        trace.mark(kCmPhSlice);
+        uint32_t prev_f = kCmEmpty;
+        e = ee = backlog = 0;
+        x = 0.0f;
+        hp = l1_end = 0;
+        int buf = 0;
+        for (uint32_t t0 = 0; t0 < qn_max; t0 += kCmFeat, buf = (buf + 1 == kNBuf) ? 0 : buf + 1) {
+            // refills the buffer of round r - 2, whose hits the previous round's trips finished
+            stage_round(t0 + (STAGES - 1) * kCmFeat, (buf + STAGES - 1) % kNBuf);
+            cm_cp_async_wait<STAGES - 1>();
+            __syncwarp();
+            trace.mark(kCmPhStaging);
+            uint32_t* my_idx = st_idx + buf * kBuf + lane * kStride;
+            float* my_val = st_val + buf * kBuf + lane * kStride;
+            const uint32_t n_here = (qn > t0) ? min(static_cast<uint32_t>(kCmFeat), qn - t0) : 0u;
+            // phase 1: look the features up -- all loads of the round are issued before the first store (eight independent
+            // feature / lookup / value loads in flight per lane) -- then compact the hits IN PLACE as {entry range, x}
+            uint32_t fq[kCmFeat], rq[kCmFeat];
+            float xq[kCmFeat];
+#pragma unroll
+            for (int k = 0; k < kCmFeat; ++k) {
+                fq[k] = (static_cast<uint32_t>(k) < n_here) ? my_idx[k] : kCmEmpty;
+                xq[k] = my_val[k];
+            }
+#pragma unroll
+            for (int k = 0; k < kCmFeat; ++k) {
+                const uint32_t f = fq[k];
+                const bool dup = (f == prev_f);  // a repeated column index only counts once (the first occurrence)
+                if (static_cast<uint32_t>(k) < n_here) prev_f = f;
+                uint32_t range = 0;
+                if (static_cast<uint32_t>(k) < n_here && !dup && f < L.w_rows) {
+                    if (DIRECT) {
+                        range = static_cast<uint32_t>(start_s[f]) | (static_cast<uint32_t>(start_s[f + 1]) << 16);
+                    } else {
+                        const uint32_t word = look_s[f >> 5];
+                        const uint32_t bit = f & 31u;
+                        if ((word >> bit) & 1u) {
+                            const uint32_t row = static_cast<uint32_t>(pre_s[f >> 5]) + __popc(word & ((1u << bit) - 1u));
+                            range = static_cast<uint32_t>(rp_s[row]) | (static_cast<uint32_t>(rp_s[row + 1]) << 16);
+                        }
+                    }
+                }
+                rq[k] = range;
+            }
+            uint32_t cnt = 0, n_ent = 0;
+#pragma unroll
+            for (int k = 0; k < kCmFeat; ++k) {
+                const uint32_t e0 = rq[k] & 0xFFFFu, e1 = rq[k] >> 16;
+                if (e1 > e0) {
+                    my_idx[cnt] = rq[k];
+                    my_val[cnt] = xq[k];
+                    ++cnt;
+                    n_ent += e1 - e0;
+                }
+            }
+            trace.mark(kCmPhLookup);
+            // phase 2: the rest of the previous round's hit rows, then as much of this round's as the trips hold, in
+            // feature order, into this lane's accumulators
+            add_rows(static_cast<uint32_t>(buf * kBuf + lane * kStride), cnt, n_ent, false);
+            trace.mark(kCmPhAccumulate);
+            __syncwarp();
+        }
+        cm_cp_async_wait<0>();
+        {  // drain, bias row last (inference.hpp:806-811): the bias row is the last "round", staged in the buffer after the
+           // last round's (its hits are gone, and no copy is in flight any more)
+            const uint32_t o = static_cast<uint32_t>(buf * kBuf + lane * kStride);
+            const uint32_t b0 = bias_range & 0xFFFFu, b1 = bias_range >> 16;
+            const bool live = have && b1 > b0;
+            st_idx[o] = bias_range;
+            st_val[o] = L.bias;
+            add_rows(o, live ? 1u : 0u, live ? b1 - b0 : 0u, true);
+        }
+        trace.mark(kCmPhAccumulate);
+        if (have) {
+            if constexpr (PREFIX) {
+                // layer 0 keeps all n0 candidates: its top-k is the descending order of their exact keys (unused keys
+                // are 0 and sort last; a real key never is 0)
+                unsigned long long key[kCmPrefixTop0];
+#pragma unroll
+                for (uint32_t j = 0; j < kCmPrefixTop0; ++j)
+                    key[j] = j < P.n0 ? xl_exact_key(xl_transform(my_acc[j * 32], P.pp_kind, P.pp_p), j) : 0ull;
+#pragma unroll
+                for (uint32_t a = 1; a < kCmPrefixTop0; ++a)
+#pragma unroll
+                    for (uint32_t b = a; b > 0; --b)
+                        if (key[b] > key[b - 1]) { const unsigned long long t = key[b]; key[b] = key[b - 1]; key[b - 1] = t; }
+                // layer 1's beam slot r is the chunk of layer-0 rank r: its children's raw scores go to the next
+                // positions of the candidate row, in column order
+                const uint64_t o = static_cast<uint64_t>(q) * P.beam_stride;
+                float* dst = P.cand1 + static_cast<uint64_t>(q) * P.cand1_stride;
+#pragma unroll
+                for (uint32_t r = 0; r < kCmPrefixTop0; ++r) {
+                    if (r < P.n0) {
+                        const uint32_t j = xl_exact_key_pos(key[r]);
+                        P.beam_id[o + r] = j;
+                        P.beam_val[o + r] = xl_exact_key_value(key[r]);
+                        const ChunkHeader h = P.chunks1[j];
+                        const float* src = my_acc + (P.n0 + h.col_begin) * 32u;
+                        for (uint32_t col = 0; col < h.n_cols; ++col) dst[col] = src[col * 32];
+                        dst += h.n_cols;
+                    }
+                }
+                P.beam_cnt[q] = P.n0;
+            } else {
+                float* dst = cand + static_cast<uint64_t>(q) * cand_stride_q + pos;
+                for (uint32_t col = 0; col < n_cols; ++col) dst[col] = my_acc[col * 32];
+            }
+        }
+        trace.slice(s_end - s0);
+        trace.mark(kCmPhSlice);
+    };
+
+    if constexpr (PREFIX) {
+        // every pair costs the same: equal slices of the rows, and warps take 32-pair slices of the CTA's
+        const uint32_t begin = static_cast<uint32_t>(static_cast<uint64_t>(P.rows) * blockIdx.x / gridDim.x);
+        const uint32_t end = static_cast<uint32_t>(static_cast<uint64_t>(P.rows) * (blockIdx.x + 1u) / gridDim.x);
+        if (begin < end) {
+            stage_image(0);
+            for (uint32_t s0 = begin + static_cast<uint32_t>(warp) * 32u; s0 < end; s0 += static_cast<uint32_t>(nwarps) * 32u)
+                score_slice(s0, min(s0 + 32u, end));
+        }
+        trace.flush(warp, lane, P.rows);
+    } else {
+        // Claim cursors decide which pairs this CTA scores, so the output cannot depend on the schedule: a pair's result
+        // goes to the place its query and position fix.  The cursors are read back through L2 (__ldcg): the claims of
+        // other SMs are atomics there, and a stale line in this SM's L1 could show a dry chunk as unclaimed again and again.
+        const uint32_t n_vc = S.n_vc;
+        __shared__ unsigned long long s_pick_work[kCmMaxWarps];
+        __shared__ uint32_t s_pick_c[kCmMaxWarps];
+        // the better of two candidates (work, chunk): more unclaimed work first, then the lower index; n_vc = none
+        auto better = [n_vc](unsigned long long wa, uint32_t ca, unsigned long long wb, uint32_t cb) {
+            return ca != n_vc && (cb == n_vc || wa > wb || (wa == wb && ca < cb));
+        };
+        uint32_t c = cm_start_chunk(w, n_vc, blockIdx.x, gridDim.x);
+        while (c < n_vc) {
+            stage_image(c);
+            const uint32_t c_end = w.bucket_ptr[c + 1];
+            for (;;) {  // warps claim the chunk's slices until it runs dry
+                uint32_t s0 = 0;
+                if (lane == 0) s0 = atomicAdd(w.claim + c, 32u);
+                s0 = __shfl_sync(kFull, s0, 0);
+                if (s0 >= c_end) break;
+                score_slice(s0, min(s0 + 32u, c_end));
+            }
+            // every warp has left the image: the CTA moves to the chunk with the most unclaimed estimated work.  A cursor
+            // read here may already be stale; that only affects the choice, as the claims themselves are atomic.
+            __syncthreads();
+            unsigned long long bw = 0;
+            uint32_t bc = n_vc;
+            for (uint32_t v = threadIdx.x; v < n_vc; v += blockDim.x) {
+                const uint32_t v_end = w.bucket_ptr[v + 1];
+                const uint32_t cl = __ldcg(w.claim + v);
+                if (cl >= v_end) continue;
+                const uint32_t entries = reinterpret_cast<const uint32_t*>(images + static_cast<uint64_t>(v) * S.img_bytes)[3];
+                const unsigned long long work = static_cast<unsigned long long>(v_end - cl) * cm_pair_cost(L.w_rows, entries);
+                if (better(work, v, bw, bc)) { bw = work; bc = v; }
+            }
+            for (int d = 16; d > 0; d >>= 1) {
+                const unsigned long long ow = __shfl_xor_sync(kFull, bw, d);
+                const uint32_t oc = __shfl_xor_sync(kFull, bc, d);
+                if (better(ow, oc, bw, bc)) { bw = ow; bc = oc; }
+            }
+            if (lane == 0) { s_pick_work[warp] = bw; s_pick_c[warp] = bc; }
+            __syncthreads();
+            // s_pick_* are rewritten only after the next switch's first barrier, which every thread reaches after this read
+            bw = s_pick_work[0];
+            c = s_pick_c[0];
+            for (int k = 1; k < nwarps; ++k)
+                if (better(s_pick_work[k], s_pick_c[k], bw, c)) { bw = s_pick_work[k]; c = s_pick_c[k]; }
+        }
+        trace.flush(warp, lane, w.bucket_ptr[n_vc]);
     }
-    trace.flush(warp, lane);
 }

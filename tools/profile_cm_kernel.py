@@ -6,8 +6,10 @@ xl_cm_scores_kernel (the leaf layer):
   * per-CTA elapsed time from %globaltimer (max / mean / min over the CTAs, and max / mean);
   * per-warp clock64 cycles by phase: image wait, query staging wait, lookup + compaction, accumulate, slice set-up +
     output (mean over the warps, and the share of each phase);
-  * accumulate trips per warp and lane efficiency: entries added / (trips x 32 lanes x 4 slots).
-The product build never defines PB200_CM_TRACE.
+  * accumulate trips per warp and lane efficiency: entries added / (trips x 32 lanes x 4 slots);
+  * per CTA: slices claimed, images staged (chunk switches + 1) and pairs scored (mean / min / max).
+It fails if the pairs scored, summed over the CTAs, differ from the pairs bucketed for the launch: every pair must be
+claimed exactly once.  The product build never defines PB200_CM_TRACE.
 
     python tools/profile_cm_kernel.py [--queries N] [--json OUT]
 """
@@ -27,7 +29,8 @@ sys.path.insert(0, ROOT)
 PHASES = ["image_wait", "staging_wait", "lookup_compact", "accumulate", "slice_setup_output"]
 MAX_WARPS = 16  # kCmMaxWarps
 TRACE_CTAS = 1024  # kCmTraceCtas
-WARP_FIELDS = len(PHASES) + 2  # kCmTraceWarp: phase cycles, trips, useful slots
+WARP_FIELDS = len(PHASES) + 4  # kCmTraceWarp: phase cycles, trips, useful slots, slices, pairs
+HEAD, CTA_HEAD = 3, 3  # g_cm_trace: grid, warps, pairs of the launch; per CTA: start ns, end ns, images staged
 SLOTS = 4  # kCmSlots
 
 
@@ -71,17 +74,20 @@ def main():
         c.pb200_xlinear_get_kernel_ids(m.model.model_chain, kid)
         if kid[2 * (depth - 1)] != 4:
             raise RuntimeError(f"the leaf layer did not run the chunk-major kernel (score kernel id {kid[2 * (depth - 1)]})")
-        per_cta = 2 + MAX_WARPS * WARP_FIELDS
-        buf = (ctypes.c_ulonglong * (2 + TRACE_CTAS * per_cta))()
+        per_cta = CTA_HEAD + MAX_WARPS * WARP_FIELDS
+        buf = (ctypes.c_ulonglong * (HEAD + TRACE_CTAS * per_cta))()
         if c.pb200_cm_trace_fetch(buf, len(buf)) != 0:
             raise RuntimeError("pb200_cm_trace_fetch failed")
     raw = np.frombuffer(buf, dtype=np.uint64)
-    grid, warps = int(raw[0]), int(raw[1])
-    rec = raw[2: 2 + grid * per_cta].reshape(grid, per_cta)
+    grid, warps, launch_pairs = int(raw[0]), int(raw[1]), int(raw[2])
+    rec = raw[HEAD: HEAD + grid * per_cta].reshape(grid, per_cta)
     cta_us = (rec[:, 1].astype(np.float64) - rec[:, 0].astype(np.float64)) / 1e3
-    per_warp = rec[:, 2:].reshape(grid, MAX_WARPS, WARP_FIELDS)[:, :warps, :].astype(np.float64)
+    images = rec[:, 2].astype(np.int64)
+    per_warp = rec[:, CTA_HEAD:].reshape(grid, MAX_WARPS, WARP_FIELDS)[:, :warps, :].astype(np.float64)
     cyc = per_warp[:, :, : len(PHASES)]
     trips, slots = per_warp[:, :, len(PHASES)], per_warp[:, :, len(PHASES) + 1]
+    slices = per_warp[:, :, len(PHASES) + 2].sum(axis=1).astype(np.int64)
+    pairs = per_warp[:, :, len(PHASES) + 3].sum(axis=1).astype(np.int64)
     phase_mean = cyc.mean(axis=(0, 1))
     warp_total = cyc.sum(axis=2)
     out = {
@@ -93,6 +99,9 @@ def main():
                         "phases_share": {p: float(v / phase_mean.sum()) for p, v in zip(PHASES, phase_mean)}},
         "accumulate": {"trips_per_warp": float(trips.mean()), "entries_per_warp": float(slots.mean()),
                        "lane_efficiency": float(slots.sum() / max(trips.sum() * 32 * SLOTS, 1.0))},
+        "per_cta": {name: {"mean": float(v.mean()), "min": int(v.min()), "max": int(v.max())}
+                    for name, v in (("slices", slices), ("images_staged", images), ("pairs", pairs))},
+        "pairs": {"launch": launch_pairs, "scored": int(pairs.sum())},
     }
     print(f"leaf: {out['queries']} queries, {grid} CTAs x {warps} warps")
     print("CTA elapsed (us): max %.1f  mean %.1f  min %.1f  max/mean %.3f" % (
@@ -103,9 +112,14 @@ def main():
     acc = out["accumulate"]
     print("accumulate: %.0f trips and %.0f entries per warp, lane efficiency %.3f" % (
         acc["trips_per_warp"], acc["entries_per_warp"], acc["lane_efficiency"]))
+    for name, v in out["per_cta"].items():
+        print("per CTA %-14s mean %8.1f  min %6d  max %6d" % (name, v["mean"], v["min"], v["max"]))
+    print("pairs: %d bucketed, %d scored" % (launch_pairs, out["pairs"]["scored"]))
     if args.json:
         with open(args.json, "w") as f:
             json.dump(out, f, indent=1)
+    if out["pairs"]["scored"] != launch_pairs:
+        raise SystemExit(f"the CTAs scored {out['pairs']['scored']} pairs, the launch has {launch_pairs}")
 
 
 if __name__ == "__main__":
