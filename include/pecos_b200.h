@@ -300,8 +300,13 @@ void c_ann_hnsw_save_csr_l2_f32(void* model_ptr, const char* model_dir);
 void pb200_hnsw_set_foreign(int metric, void* destruct, void* searchers_create, void* searchers_destruct, void* predict, void* save);
 
 /* base-vector rows kept in flight per warp by the bulk-copy (TMA) ring: 0 = direct loads, 4 (default) or 8; returns the
- * value in effect.  Results are identical for every setting. */
+ * value in effect.  Results are identical for every setting.  A search whose per-warp shared-memory slice (query + ring
+ * rows + result heap) would exceed 200 KB at this depth runs the next shallower one that fits (8 -> 4 -> 0); dense indices
+ * with d beyond about 50,000 fit none and raise. */
 int pb200_hnsw_set_stages(void* model_ptr, int stages);
+/* the last search launch of the handle's primary engine: out[5] = {ring depth it ran, warps per CTA, CTAs, dynamic shared
+ * memory per CTA in bytes, result-heap entries allocated in global scratch (heaps of ef > 512 live there; grows only)} */
+void pb200_hnsw_launch_info(void* model_ptr, uint64_t* out);
 void pb200_hnsw_get_info(void* model_ptr, uint64_t* out);
 /* Host-only ingest check of an HNSW index folder (<model>/c_model), no GPU needed: the loader's validation of config.json
  * (hnsw_t string of the requested metric / data type, version) and of index.mmap_store (record sizes; sparse: record offsets,

@@ -474,6 +474,7 @@ class B200CoreLib(object):
                                                      POINTER(c_float)])
         fp(c.pb200_hnsw_get_counters, None, [c_void_p, POINTER(c_uint64)])
         fp(c.pb200_hnsw_set_stages, c_int, [c_void_p, c_int])
+        fp(c.pb200_hnsw_launch_info, None, [c_void_p, POINTER(c_uint64)])
         fp(c.pb200_hnsw_get_info, None, [c_void_p, POINTER(c_uint64)])
         fp(c.pb200_hnsw_host_info, c_int, [c_char_p, c_int, c_int, POINTER(c_uint64)])
         fp(c.pb200_sparse_block_distances, None, [c_int, c_int, c_void_p, c_void_p, c_void_p, c_uint32, c_void_p, c_void_p,

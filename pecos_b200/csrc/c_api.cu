@@ -1137,6 +1137,13 @@ int pb200_hnsw_set_stages(void* model_ptr, int stages) {
     PB200_API_END("pb200_hnsw_set_stages")
 }
 
+void pb200_hnsw_launch_info(void* model_ptr, uint64_t* out) {
+    PB200_API_BEGIN
+    PB200_LOCK_HNSW(model_ptr)
+    hnsw_of(model_ptr).launch_info(out);
+    PB200_API_END("pb200_hnsw_launch_info")
+}
+
 void pb200_hnsw_get_counters(void* model_ptr, uint64_t* out) {
     PB200_API_BEGIN
     PB200_LOCK_HNSW(model_ptr)

@@ -693,15 +693,15 @@ HnswEngine::~HnswEngine() {
     if (stream_) cudaStreamDestroy(stream_);
 }
 
-uint32_t HnswEngine::per_warp_smem_(uint32_t ef, uint32_t* nbmax_out) const {
+uint32_t HnswEngine::per_warp_smem_(uint32_t ef, int stages, uint32_t* nbmax_out) const {
     const HnswHostIndex& H = *host_;
     const uint32_t nbmax = ((std::max(H.l0_max_degree, H.l1_max_degree) + 31u) / 32u) * 32u;
     const bool top_in_smem = ef <= kEfSmemMax;
     if (nbmax_out) *nbmax_out = nbmax;
     if (H.sparse)  // [query indices | query values | filter | ids | distances | result heap]
         return (qcap_ * 8u + kSpFilterWords * 4u + nbmax * 8 + (top_in_smem ? (ef + 1) * 8 : 0) + 15u) & ~15u;
-    // [query | stages_ ring slots | stages_ mbarriers | ids | distances | result heap]
-    return (H.vstride() * 4 * (1u + static_cast<uint32_t>(stages_)) + static_cast<uint32_t>(stages_) * 8u + nbmax * 8 +
+    // [query | stages ring slots | stages mbarriers | ids | distances | result heap]
+    return (H.vstride() * 4 * (1u + static_cast<uint32_t>(stages)) + static_cast<uint32_t>(stages) * 8u + nbmax * 8 +
             (top_in_smem ? (ef + 1) * 8 : 0) + 15u) & ~15u;
 }
 
@@ -710,14 +710,25 @@ void HnswEngine::set_stages(int stages) {
     n_warps_ = 0;  // forces the scratch / launch geometry to be recomputed
 }
 
+// One warp's shared-memory slice must fit kWarpSmemMax.  The ring takes stages + 1 rows of 4 * vstride bytes, so wide vectors
+// run the deepest ring that fits: the configured depth, else 8 -> 4 -> 0 (direct loads: one row, dense d up to about 50,000).
+// Results do not depend on the depth.
 void HnswEngine::ensure_scratch_(uint32_t ef) {
     const HnswHostIndex& H = *host_;
     const bool top_in_smem = ef <= kEfSmemMax;
-    const uint32_t per_warp = per_warp_smem_(ef, nullptr);
+    constexpr uint32_t kWarpSmemMax = 200u * 1024u;  // the kernels' dynamic shared-memory limit (cudaFuncSetAttribute)
+    int stages = stages_;
+    uint32_t per_warp = per_warp_smem_(ef, stages, nullptr);
+    while (stages > 0 && per_warp > kWarpSmemMax) {
+        stages = stages > 4 ? 4 : 0;
+        per_warp = per_warp_smem_(ef, stages, nullptr);
+    }
+    if (per_warp > kWarpSmemMax)
+        throw std::runtime_error("pecos_b200: HNSW query dimension too large for the shared-memory staging area, even with "
+                                 "direct loads (dense indices serve d up to about 50,000)");
+    run_stages_ = H.sparse ? 0 : stages;
     uint32_t warps = 8;
     while (warps > 1 && static_cast<uint64_t>(warps) * per_warp > 96u * 1024u) warps >>= 1;
-    if (static_cast<uint64_t>(warps) * per_warp > 200u * 1024u)
-        throw std::runtime_error("pecos_b200: HNSW query dimension too large for the shared-memory staging area");
     int sms = 132;
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device_);
     const uint32_t ctas_per_sm = std::max<uint32_t>(1, std::min<uint32_t>((H.sparse ? 32u : 16u) / warps, static_cast<uint32_t>((220u * 1024u) / (static_cast<uint64_t>(warps) * per_warp))));
@@ -731,14 +742,23 @@ void HnswEngine::ensure_scratch_(uint32_t ef) {
     const uint64_t per_warp_scratch = words * 4 + static_cast<uint64_t>(vcap) * 12 + (top_in_smem ? 0 : static_cast<uint64_t>(ef + 1) * 8);
     while (n_ctas > static_cast<uint32_t>(sms) && static_cast<uint64_t>(n_ctas) * warps * per_warp_scratch > (24ull << 30)) n_ctas -= sms;
     const uint32_t n_warps = n_ctas * warps;
-    if (n_warps != n_warps_ || vcap != vcap_ || (!top_in_smem && ef > scratch_ef_) || warps != warps_per_cta_) {
+    if (n_warps != n_warps_ || vcap != vcap_ || warps != warps_per_cta_) {
         bitmap_.reserve(static_cast<uint64_t>(n_warps) * words);
         PB200_CUDA(cudaMemsetAsync(bitmap_.get(), 0, static_cast<uint64_t>(n_warps) * words * 4, stream_));
         vlist_.reserve(static_cast<uint64_t>(n_warps) * vcap);
         cand_.reserve(static_cast<uint64_t>(n_warps) * vcap);
-        if (!top_in_smem) { topk_heap_.reserve(static_cast<uint64_t>(n_warps) * (ef + 1)); scratch_ef_ = ef; }
         n_warps_ = n_warps; warps_per_cta_ = warps; n_ctas_ = n_ctas; vcap_ = vcap;
     }
+    // grows only: kept across calls, sized for this call's warps and ef whatever the calls in between used
+    if (!top_in_smem) topk_heap_.reserve(static_cast<uint64_t>(n_warps) * (ef + 1));
+}
+
+void HnswEngine::launch_info(uint64_t* out) const {
+    out[0] = static_cast<uint64_t>(run_stages_);
+    out[1] = warps_per_cta_;
+    out[2] = last_ctas_;
+    out[3] = last_smem_;
+    out[4] = topk_heap_.capacity();
 }
 
 double HnswEngine::launch_once_(const float* q_dev, uint32_t nq, uint32_t efS, uint32_t topk, int idx_fill, bool* overflow) {
@@ -748,7 +768,7 @@ double HnswEngine::launch_once_(const float* q_dev, uint32_t nq, uint32_t efS, u
     ensure_scratch_(ef);
     uint32_t nbmax = 0;
     const bool top_in_smem = ef <= kEfSmemMax;
-    const uint32_t per_warp = per_warp_smem_(ef, &nbmax);
+    const uint32_t per_warp = per_warp_smem_(ef, run_stages_, &nbmax);
     const uint32_t words = static_cast<uint32_t>((static_cast<uint64_t>(H.num_node) + 31) / 32);
     PB200_CUDA(cudaMemsetAsync(ctrl_.get(), 0, 8 * sizeof(unsigned long long), stream_));
     PB200_CUDA(cudaMemsetAsync(out_idx_.get(), idx_fill, static_cast<uint64_t>(nq) * topk * 4, stream_));
@@ -764,10 +784,12 @@ double HnswEngine::launch_once_(const float* q_dev, uint32_t nq, uint32_t efS, u
     };
     const bool ip = H.metric == HNSW_IP;
     if (H.sparse) { if (ip) launch(hnsw_search_kernel<HNSW_IP, 0, true>); else launch(hnsw_search_kernel<HNSW_L2, 0, true>); }
-    else if (stages_ == 0) { if (ip) launch(hnsw_search_kernel<HNSW_IP, 0, false>); else launch(hnsw_search_kernel<HNSW_L2, 0, false>); }
-    else if (stages_ == 4) { if (ip) launch(hnsw_search_kernel<HNSW_IP, 4, false>); else launch(hnsw_search_kernel<HNSW_L2, 4, false>); }
+    else if (run_stages_ == 0) { if (ip) launch(hnsw_search_kernel<HNSW_IP, 0, false>); else launch(hnsw_search_kernel<HNSW_L2, 0, false>); }
+    else if (run_stages_ == 4) { if (ip) launch(hnsw_search_kernel<HNSW_IP, 4, false>); else launch(hnsw_search_kernel<HNSW_L2, 4, false>); }
     else { if (ip) launch(hnsw_search_kernel<HNSW_IP, 8, false>); else launch(hnsw_search_kernel<HNSW_L2, 8, false>); }
     PB200_CUDA(cudaGetLastError());
+    last_ctas_ = ctas;
+    last_smem_ = static_cast<uint32_t>(smem);
     PB200_CUDA(cudaEventRecord(ev_[1], stream_));
     ++launches_;
     PB200_CUDA(cudaEventSynchronize(ev_[1]));

@@ -82,13 +82,17 @@ public:
     uint32_t vcap_retries() const { return vcap_retries_; }  // batches re-run after a candidate-queue overflow
     uint64_t index_bytes() const { return index_bytes_; }
     double last_kernel_ms() const { return last_ms_; }
-    // rows kept in flight per warp by the bulk-copy ring: 0 (direct loads), 4 or 8
+    // rows kept in flight per warp by the bulk-copy ring: 0 (direct loads), 4 or 8, used wherever the ring fits (see
+    // ensure_scratch_)
     void set_stages(int stages);
     int stages() const { return stages_; }
+    // the last search launch: {ring depth it ran, warps per CTA, CTAs, dynamic shared memory per CTA (bytes),
+    // result-heap entries held in global scratch (0 while every heap fitted in shared memory)}
+    void launch_info(uint64_t* out) const;
 
 private:
     void ensure_scratch_(uint32_t ef);
-    uint32_t per_warp_smem_(uint32_t ef, uint32_t* nbmax_out) const;
+    uint32_t per_warp_smem_(uint32_t ef, int stages, uint32_t* nbmax_out) const;
     // idx_fill: byte value out_idx_ is filled with before the search (0: the reference's zeros; 0xFF: empty slots read
     // 0xFFFFFFFF, which no node id can be, for the shard pack kernel)
     double launch_(const float* q_dev, uint32_t nq, uint32_t efS, uint32_t topk, int idx_fill = 0);
@@ -107,7 +111,9 @@ private:
 
     // per-warp scratch
     uint32_t n_warps_ = 0, warps_per_cta_ = 0, n_ctas_ = 0;
-    uint32_t vcap_ = 0, scratch_ef_ = 0;
+    int run_stages_ = 0;  // ring depth of the current launch geometry: stages_, or shallower where stages_ does not fit
+    uint32_t last_ctas_ = 0, last_smem_ = 0;
+    uint32_t vcap_ = 0;
     uint32_t vcap_floor_ = 0;    // minimum candidate-queue capacity (doubled after an overflow)
     uint32_t vcap_retries_ = 0;
     DeviceBuffer<uint32_t> bitmap_;

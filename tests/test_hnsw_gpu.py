@@ -12,6 +12,8 @@ import os
 import numpy as np
 import pytest
 
+from .util import save_hnsw_index
+
 pytestmark = pytest.mark.gpu
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "hnsw_toy")
@@ -107,33 +109,10 @@ def test_mid_size_goldens_all_ring_depths(gpu_clib):
             assert np.array_equal(dist.view(np.uint32), E[f"{name}|200|10|dist"].view(np.uint32)), (name, stages)
 
 
-BUILD_SEED = 3
-
-
-def _save_index(tmp, X, M, efC, metric, have_ref, threads=8):
-    """Index trained by the reference library where oracle/_ref is built (returned, to search the saved file with), else built
-    by this library's own index builder (pecos_b200/hnsw_build.py, same on-disk format; returns None).  The restatement the
-    kernel is compared with bit for bit is pinned to the reference by tests/test_oracle_hnsw_cpu.py."""
-    if not have_ref:
-        from pecos_b200.hnsw_build import build_hnsw_index
-
-        build_hnsw_index(X, tmp, M=M, efC=efC, metric=metric, seed=BUILD_SEED)
-        return None
-    from oracle import ref
-
-    r = ref.RefHNSW.train(X, M=M, efC=efC, metric=metric, threads=threads)
-    os.makedirs(tmp, exist_ok=True)
-    r.save(os.path.join(tmp, "c_model"))
-    json.dump({"model": "HNSW", "data_type": "drm", "metric_type": metric, "num_item": int(X.shape[0]),
-               "feat_dim": int(X.shape[1]), "pred_kwargs": {"efS": 50, "topk": 10, "threads": 1}},
-              open(os.path.join(tmp, "param.json"), "w"))
-    return r
-
-
 @pytest.mark.parametrize("N,d,M,metric", [(4000, 64, 8, "ip"), (3000, 70, 12, "l2"), (2500, 128, 16, "ip"),
                                           (1200, 3, 4, "l2"), (6000, 768, 16, "ip"), (2000, 100, 6, "l2")])
 def test_random_indices_match_reference_library(tmp_path, gpu_clib, have_ref, N, d, M, metric):
-    """Random indices (_save_index); the same saved index searched by the reference (where built), the restatement and us."""
+    """Random indices (util.save_hnsw_index); the same saved index searched by the reference (where built), the restatement and us."""
     from oracle import restatement
 
     rng = np.random.default_rng(N + d)
@@ -142,7 +121,7 @@ def test_random_indices_match_reference_library(tmp_path, gpu_clib, have_ref, N,
     Q = rng.standard_normal((257, d)).astype(np.float32)
     Q /= np.linalg.norm(Q, axis=1, keepdims=True)
     folder = str(tmp_path / "idx")
-    r = _save_index(folder, X, M, 60, metric, have_ref)
+    r = save_hnsw_index(folder, X, M, 60, metric, have_ref)
     m = _load(folder)
     o = restatement.OracleHNSW(folder, isa=0)  # avx512f order == what the kernel restates
     isa = restatement.host_isa()
@@ -170,7 +149,7 @@ def test_duplicate_points_and_ties(tmp_path, gpu_clib, have_ref):
     X = np.concatenate([base] * 6, axis=0)  # every point six times
     Q = base[:64] + 0.0
     folder = str(tmp_path / "idx")
-    r = _save_index(folder, X, 8, 50, "l2", have_ref, threads=1)
+    r = save_hnsw_index(folder, X, 8, 50, "l2", have_ref, threads=1)
     m = _load(folder)
     for efS, topk in [(30, 12), (100, 20)]:
         idx, dist = m.predict(Q, pred_params=_pp(efS, topk), ret_csr=False)
@@ -188,7 +167,7 @@ def test_bulk_copy_ring_depths_give_identical_results(tmp_path, gpu_clib, have_r
     X /= np.linalg.norm(X, axis=1, keepdims=True)
     Q = rng.standard_normal((300, 200)).astype(np.float32)
     folder = str(tmp_path / "idx")
-    _save_index(folder, X, 12, 60, "ip", have_ref)
+    save_hnsw_index(folder, X, 12, 60, "ip", have_ref)
     m = _load(folder)
     c = gpu_clib.clib_float32
     ref_out = None

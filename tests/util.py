@@ -64,6 +64,32 @@ def csr_with_empty_rows(X, rows):
     return X
 
 
+HNSW_BUILD_SEED = 3
+
+
+def save_hnsw_index(tmp, X, M, efC, metric, have_ref, threads=8):
+    """Index of the rows X (dense float32, or scipy csr) trained by the reference library where oracle/_ref is built (returned,
+    to search the saved file with), else built by this library's own index builder (pecos_b200/hnsw_build.py, same on-disk
+    format; returns None).  The restatement the kernel is compared with bit for bit is pinned to the reference by
+    tests/test_oracle_hnsw_cpu.py."""
+    import json
+
+    if not have_ref:
+        from pecos_b200.hnsw_build import build_hnsw_index
+
+        build_hnsw_index(X, tmp, M=M, efC=efC, metric=metric, seed=HNSW_BUILD_SEED)
+        return None
+    from oracle import ref
+
+    r = ref.RefHNSW.train(X, M=M, efC=efC, metric=metric, threads=threads)
+    os.makedirs(tmp, exist_ok=True)
+    r.save(os.path.join(tmp, "c_model"))
+    json.dump({"model": "HNSW", "data_type": r.data_type, "metric_type": metric, "num_item": int(X.shape[0]),
+               "feat_dim": int(X.shape[1]), "pred_kwargs": {"efS": 50, "topk": 10, "threads": 1}},
+              open(os.path.join(tmp, "param.json"), "w"))
+    return r
+
+
 def merge_shards_numpy(g_keys, g_ids, g_vals, g_cnt, k):
     """Reference semantics of the index-sharding merge (test-only): per query keep the k largest 64-bit keys
     among the valid entries of all ranks.  g_* have shape [world, rows, stride], g_cnt [world, rows]."""
