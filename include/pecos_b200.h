@@ -249,6 +249,10 @@ void pb200_xlinear_get_profile(void* ptr, double* out);
  * lookup (xl_chunk_scores_kernel), 2 dense, 3 xl_query_warp_scores_kernel, 4 xl_cm_scores_kernel.  Top-k: 0 xl_topk_kernel,
  * 1 xl_topk_warp_kernel, 2 xl_topk_filter_kernel. */
 void pb200_xlinear_get_kernel_ids(void* ptr, int* out);
+/* The chunk-major image geometry chosen at load time for `layer` (-1: the merged prefix image of layers 0 and 1):
+ * out[6] = {images built, direct feature table, column cap (wider chunks are cut into ranges of at most this many columns),
+ * virtual chunks, bytes per image, warps that fit next to one image}.  Returns 1 (out untouched) for a layer out of range. */
+int pb200_xlinear_cm_info(void* ptr, int layer, uint64_t* out);
 void pb200_xlinear_get_stats(void* ptr, uint64_t* out);
 uint64_t pb200_xlinear_launches(void* ptr);
 uint64_t pb200_xlinear_model_bytes(void* ptr);
@@ -352,6 +356,17 @@ uint32_t pb200_xlinear_host_depth(void* hptr);
 void pb200_xlinear_host_layer_dims(void* hptr, uint32_t layer, uint64_t* out);
 void pb200_xlinear_host_layer_export(void* hptr, uint32_t layer, void* chunks32, uint32_t* meta, void* entries8,
                                      uint32_t* label_of_col);
+/* Beam limit of XR-Linear prediction.  The beam entering a layer (1 at the root, then min(k, candidates) of the layer above,
+ * k = beam_size or the stored only_topk) may hold at most 15,701 nodes: the block top-k keeps 2048 sort keys and three words
+ * per beam slot in 200 KB of shared memory.  c_xlinear_predict_* (and the resident / index-sharded calls) with a wider beam
+ * is a fatal error, so callers check first: returns 1 when the (beam_size, only_topk) call fits, else 0, and
+ * out[4] = {first layer whose entering beam is too wide, that beam's width, the limit, widest beam_size that fits
+ * (0xFFFFFFFF: all)}.  Host-only: hptr is a pb200_xlinear_host_* handle, ptr a loaded model (c_xlinear_load_*). */
+int pb200_xlinear_host_plan_fits(void* hptr, uint32_t beam_size, uint32_t only_topk, uint32_t* out);
+int pb200_xlinear_plan_fits(void* ptr, uint32_t beam_size, uint32_t only_topk, uint32_t* out);
+/* The limit itself: 15,701 when the layer selects a top-k (topk != 0), else 32,768.  One layer of the python chain
+ * (c_xlinear_single_layer_predict_*) enters with a beam of max(row nnz of csr_codes) nodes, or C.cols without codes. */
+uint32_t pb200_xlinear_beam_limit(int topk);
 
 #ifdef __cplusplus
 }

@@ -487,6 +487,33 @@ class B200CoreLib(object):
         fp(c.pb200_xlinear_host_depth, c_uint32, [c_void_p])
         fp(c.pb200_xlinear_host_layer_dims, None, [c_void_p, c_uint32, POINTER(c_uint64)])
         fp(c.pb200_xlinear_host_layer_export, None, [c_void_p, c_uint32, c_void_p, c_void_p, c_void_p, c_void_p])
+        fp(c.pb200_xlinear_host_plan_fits, c_int, [c_void_p, c_uint32, c_uint32, POINTER(c_uint32)])
+        fp(c.pb200_xlinear_plan_fits, c_int, [c_void_p, c_uint32, c_uint32, POINTER(c_uint32)])
+        fp(c.pb200_xlinear_beam_limit, c_uint32, [c_int])
+        fp(c.pb200_xlinear_cm_info, c_int, [c_void_p, c_int, POINTER(c_uint64)])
+
+    def xlinear_check_layer_beam(self, b_prev):
+        """Raises ValueError unless one layer of the python chain (c_xlinear_single_layer_predict_*) may enter with a beam of
+        b_prev nodes: max(row nnz of csr_codes), or C.shape[1] without codes.  Host-only."""
+        limit = int(self.clib_float32.pb200_xlinear_beam_limit(1))
+        if b_prev > limit:
+            raise ValueError(f"pecos_b200: the beam entering this layer would hold {b_prev} nodes, more than the supported "
+                             f"maximum of {limit}")
+
+    def xlinear_check_plan(self, c_model, beam_size, only_topk, host=False):
+        """Raises ValueError unless a predict call on `c_model` (a loaded model; host=True: a pb200_xlinear_host_* handle)
+        with this beam_size / only_topk (0 or None: the stored values) fits the beam limit; returns the widest beam_size that
+        fits (None: any).  Host-only, so it runs before any GPU work of the call."""
+        c = self.clib_float32
+        out = (c_uint32 * 4)()
+        f = c.pb200_xlinear_host_plan_fits if host else c.pb200_xlinear_plan_fits
+        fits = f(c_model, int(beam_size or 0), int(only_topk or 0), out)
+        layer, width, limit, widest = [int(v) for v in out]
+        if not fits:
+            raise ValueError(
+                f"pecos_b200: the beam entering layer {layer} would hold {width} nodes, more than the supported maximum of "
+                f"{limit}" + (f"; the widest beam_size that fits this model is {widest}" if widest else ""))
+        return None if widest == 0xFFFFFFFF else widest
 
     def device_count(self):
         return int(self.clib_float32.pb200_device_count())

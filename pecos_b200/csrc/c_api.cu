@@ -99,6 +99,14 @@ pb200::XLinearEngine& engine_of(void* ptr) {
     return *static_cast<XLinearHandle*>(ptr)->engines.at(0);
 }
 
+// pb200_xlinear_{host_,}plan_fits: 1 if a predict call with (beam_size, only_topk) fits the beam limits, else 0;
+// out[4] = {first layer whose entering beam is too wide, that beam's width, the limit, widest beam_size that fits}
+int plan_fits(const pb200::XLinearHostModel& m, uint32_t beam_size, uint32_t only_topk, uint32_t* out) {
+    const pb200::XLinearBeamCheck r = pb200::xlinear_check_beam(m, beam_size, only_topk);
+    if (out) { out[0] = r.layer; out[1] = r.b_prev; out[2] = r.limit; out[3] = r.widest; }
+    return r.fits ? 1 : 0;
+}
+
 void emit_results(const std::vector<pb200::XLinearEngine::Result>& parts, py_sparse_allocator_t pred_alloc) {
     // create_pycsr contract (pecos/core/utils/matrix.hpp:300-316): one allocator call, then fill the three arrays.
     uint64_t nnz = 0, rows = 0;
@@ -778,6 +786,19 @@ void pb200_xlinear_get_kernel_ids(void* ptr, int* out) {
     PB200_API_END("pb200_xlinear_get_kernel_ids")
 }
 
+int pb200_xlinear_cm_info(void* ptr, int layer, uint64_t* out) {
+    PB200_API_BEGIN
+    PB200_LOCK_XL(ptr)
+    const pb200::CmShape* s = engine_of(ptr).cm_shape_of(layer);
+    if (!s) return 1;
+    out[0] = s->ok ? 1 : 0; out[1] = s->direct ? 1 : 0; out[2] = s->col_cap; out[3] = s->n_vc; out[4] = s->img_bytes;
+    out[5] = s->warps_fit;
+    return 0;
+    PB200_API_END("pb200_xlinear_cm_info")
+}
+
+uint32_t pb200_xlinear_beam_limit(int topk) { return topk ? pb200::kXlBeamMaxTopk : pb200::kXlBeamMax; }
+
 void pb200_xlinear_get_stats(void* ptr, uint64_t* out) {
     PB200_API_BEGIN
     PB200_LOCK_XL(ptr)
@@ -839,6 +860,19 @@ void* pb200_xlinear_host_prefix_layer(void* hptr) {
 }
 
 void pb200_xlinear_host_free(void* hptr) { delete static_cast<pb200::XLinearHostModel*>(hptr); }
+
+int pb200_xlinear_host_plan_fits(void* hptr, uint32_t beam_size, uint32_t only_topk, uint32_t* out) {
+    PB200_API_BEGIN
+    if (!hptr) throw std::runtime_error("null host model");
+    return plan_fits(*static_cast<pb200::XLinearHostModel*>(hptr), beam_size, only_topk, out);
+    PB200_API_END("pb200_xlinear_host_plan_fits")
+}
+
+int pb200_xlinear_plan_fits(void* ptr, uint32_t beam_size, uint32_t only_topk, uint32_t* out) {
+    PB200_API_BEGIN
+    return plan_fits(engine_of(ptr).host(), beam_size, only_topk, out);  // host model only: callable while the device is busy
+    PB200_API_END("pb200_xlinear_plan_fits")
+}
 
 uint32_t pb200_xlinear_host_depth(void* hptr) { return static_cast<pb200::XLinearHostModel*>(hptr)->depth(); }
 

@@ -872,8 +872,50 @@ size_t chunk_kernel_smem(int warps, bool lookup, uint32_t q_cap, uint32_t sb_cap
            static_cast<size_t>(warps) * (lookup ? sizeof(WarpScratch<kMCapLookup>) : sizeof(WarpScratch<kMCap>));
 }
 size_t topk_kernel_smem(uint32_t b_prev) { return static_cast<size_t>(kSortCap) * 8 + (static_cast<size_t>(b_prev) * 3 + 1) * 4; }
+static_assert(kSortCap * 8 + (kXlBeamMaxTopk * 3 + 1) * 4 <= 200 * 1024 && kSortCap * 8 + ((kXlBeamMaxTopk + 1) * 3 + 1) * 4 > 200 * 1024,
+              "kXlBeamMaxTopk is the widest beam whose block top-k fits 200 KB of shared memory");
+
+// Widths of the beams entering each layer (the b_prev / k_cap chain of make_plan_); false at the first one over `limit`.
+bool beam_chain_fits(const XLinearHostModel& m, uint32_t beam_size, uint32_t only_topk, const std::vector<uint32_t>& b_in,
+                     uint32_t limit, uint32_t* layer, uint32_t* width) {
+    const size_t depth = m.layers.size();
+    uint32_t b_prev = 1;
+    for (size_t d = 0; d < depth; ++d) {
+        const auto& L = m.layers[d];
+        if (d < b_in.size() && b_in[d] > 0) b_prev = b_in[d];
+        if (b_prev > limit) {
+            if (layer) *layer = static_cast<uint32_t>(d);
+            if (width) *width = b_prev;
+            return false;
+        }
+        const uint32_t local = (d + 1 == depth) ? only_topk : beam_size;
+        const uint32_t k = local > 0 ? local : static_cast<uint32_t>(L.only_topk);
+        const uint64_t cand_max = static_cast<uint64_t>(b_prev) * std::max<uint32_t>(L.c_max, 1u);
+        b_prev = static_cast<uint32_t>(std::max<uint64_t>(1, std::min<uint64_t>(k, cand_max)));
+    }
+    return true;
+}
 
 }  // namespace
+
+XLinearBeamCheck xlinear_check_beam(const XLinearHostModel& m, uint32_t beam_size, uint32_t only_topk,
+                                    const std::vector<uint32_t>& b_in, bool topk) {
+    XLinearBeamCheck r;
+    r.limit = topk ? kXlBeamMaxTopk : kXlBeamMax;
+    r.fits = beam_chain_fits(m, beam_size, only_topk, b_in, r.limit, &r.layer, &r.b_prev);
+    // a wider beam_size never narrows a beam, so the plans that fit are the beam sizes up to some bound
+    if (beam_chain_fits(m, 0xFFFFFFFFu, only_topk, b_in, r.limit, nullptr, nullptr)) {
+        r.widest = 0xFFFFFFFFu;
+    } else {
+        uint32_t lo = 0, hi = 0xFFFFFFFFu;  // fits(lo) (or lo == 0), !fits(hi)
+        while (hi - lo > 1) {
+            const uint32_t mid = lo + (hi - lo) / 2;
+            if (beam_chain_fits(m, mid, only_topk, b_in, r.limit, nullptr, nullptr)) lo = mid; else hi = mid;
+        }
+        r.widest = lo;
+    }
+    return r;
+}
 
 // ------------------------------------------------------------------------------------------------------------------
 // engine
@@ -1106,6 +1148,10 @@ void XLinearEngine::reset_profile() {
 
 std::vector<XLinearEngine::LayerPlan> XLinearEngine::make_plan_(uint32_t beam_size, const char* post_processor, uint32_t only_topk,
                                                                  const std::vector<uint32_t>& b_in, bool topk) const {
+    const XLinearBeamCheck fit = xlinear_check_beam(*host_, beam_size, only_topk, b_in, topk);
+    if (!fit.fits)
+        throw std::runtime_error("pecos_b200: beam of " + std::to_string(fit.b_prev) + " nodes entering layer " +
+                                 std::to_string(fit.layer) + " exceeds the supported maximum of " + std::to_string(fit.limit));
     const size_t depth = layers_.size();
     std::vector<LayerPlan> plan(depth);
     uint32_t b_prev = 1;
@@ -1120,8 +1166,6 @@ std::vector<XLinearEngine::LayerPlan> XLinearEngine::make_plan_(uint32_t beam_si
         plan[d].b_prev = b_prev;
         const uint64_t cand_max = static_cast<uint64_t>(b_prev) * std::max<uint32_t>(L.c_max, 1u);
         plan[d].k_cap = static_cast<uint32_t>(std::max<uint64_t>(1, std::min<uint64_t>(k, cand_max)));
-        if (b_prev > 32768u || (topk && topk_kernel_smem(b_prev) > 200u * 1024u))
-            throw std::runtime_error("pecos_b200: beam of " + std::to_string(b_prev) + " nodes exceeds the supported maximum");
         b_prev = plan[d].k_cap;
     }
     return plan;

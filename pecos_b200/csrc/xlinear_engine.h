@@ -90,6 +90,22 @@ struct XLinearLayerProfile {
     int topk_kernel = 0;     // last launch: 0 block-wide sort, 1 warp arg-max, 2 estimate filter
 };
 
+// Beam limits of a prediction, from the host model alone (no CUDA calls).  The beam entering a layer that selects a top-k
+// may hold at most kXlBeamMaxTopk nodes: the block top-k keeps 2048 sort keys and three words per beam slot in <= 200 KB
+// of shared memory, (200 KB - 16 KB - 4) / 12 = 15,701.  Without a top-k (selected outputs) the limit is kXlBeamMax.
+// b_in, topk: as for XLinearEngine::make_plan_.
+constexpr uint32_t kXlBeamMaxTopk = 15701;
+constexpr uint32_t kXlBeamMax = 32768;
+struct XLinearBeamCheck {
+    bool fits = true;
+    uint32_t layer = 0;   // first layer whose entering beam is too wide (when !fits)
+    uint32_t b_prev = 0;  // that beam's width
+    uint32_t limit = 0;   // the limit it exceeds
+    uint32_t widest = 0;  // widest beam_size whose plan fits (0: none; 0xFFFFFFFF: every beam_size fits)
+};
+XLinearBeamCheck xlinear_check_beam(const XLinearHostModel& m, uint32_t beam_size, uint32_t only_topk,
+                                    const std::vector<uint32_t>& b_in = {}, bool topk = true);
+
 class XLinearEngine {
 public:
     XLinearEngine(std::unique_ptr<XLinearHostModel> host, int device);
@@ -147,6 +163,11 @@ public:
     // kernel selection for A/B runs and cross-checks: modes 0 - 7, listed at the definition; any other value behaves as 1
     void set_kernel_mode(int mode);
     bool has_feature_maps() const;
+    // chunk-major image geometry chosen at load time for layer d (d < 0: the prefix image); ok == false: no images
+    const CmShape* cm_shape_of(int d) const {
+        if (d < 0) return &prefix_.cm_shape;
+        return static_cast<size_t>(d) < layers_.size() ? &layers_[d].cm_shape : nullptr;
+    }
     const std::vector<XLinearLayerProfile>& layer_profile() const { return layer_profile_; }
     void reset_profile();
     const std::vector<XLinearStats>& layer_stats() const { return layer_stats_; }

@@ -107,6 +107,7 @@ class ShardedXLinearModel(object):
         import torch
 
         assert X.dtype == np.float32 and X.has_sorted_indices
+        self._clib.xlinear_check_plan(self.model_chain, beam_size, only_topk)
         c = self._clib.clib_float32
         k = int(only_topk or self.pred_params[-1]["only_topk"])
         rows = X.shape[0]

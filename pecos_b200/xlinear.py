@@ -125,6 +125,12 @@ class MLModel(object):
             pred_params.post_processor = kwargs["post_processor"]
         if isinstance(X, smat.csr_matrix) and not X.has_sorted_indices:
             raise ValueError("Query matrix does not have sorted indices!")
+        # the beam entering this layer: the widest row of the previous layer's prediction, or every parent
+        if csr_codes is not None:
+            b_prev = max(1, int(np.diff(smat.csr_matrix(csr_codes).indptr).max(initial=0)))
+        else:
+            b_prev = max(1, self.nr_codes)
+        self._clib.xlinear_check_layer_beam(b_prev)
         pred_alloc = ScipyCompressedSparseAllocator()
         self._clib.xlinear_single_layer_predict(
             X,
@@ -310,6 +316,8 @@ class HierarchicalMLModel(object):
         else:
             raise NotImplementedError("when is_predict_only=True, beam_size is not supported for overriding")
 
+        # a beam too wide for the top-k kernels is a ValueError here, not a fatal error inside the predict call
+        self._clib.xlinear_check_plan(self.model_chain, overridden_beam_size, new_chain[-1].only_topk)
         pred_alloc = ScipyCompressedSparseAllocator()
         self._clib.xlinear_predict(
             self.model_chain,
