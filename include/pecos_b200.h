@@ -303,6 +303,45 @@ void c_ann_hnsw_save_csr_ip_f32(void* model_ptr, const char* model_dir);
 void c_ann_hnsw_save_csr_l2_f32(void* model_ptr, const char* model_dir);
 void pb200_hnsw_set_foreign(int metric, void* destruct, void* searchers_create, void* searchers_destruct, void* predict, void* save);
 
+/* ================================================== PairwiseANN ================================================== */
+/* libpecos.cpp:567-659, pecos/core/ann/pairwise.hpp.  Two types, as in the reference: drm (dense X_trn, FeatVecDenseIPSimd) and
+ * csr (X_trn rows with strictly ascending indices, FeatVecSparseIPSimd); inner-product distance only.
+ * train deep-copies X_trn and Y_csc (X.rows must equal Y.rows); load reads <model>/c_model (config.json + index.mmap_store) and
+ * save writes the same two files.  Neither touches the GPU: a model's arrays move to the device on its first search.
+ * searchers_create: num_searcher is accepted and ignored; a token owns a stream and scratch, calls on one token are
+ * serialised, tokens of one model may run concurrently.
+ * predict: pair b uses query row (is_same_input ? 0 : b) and column label_keys[b]; slot k < min(only_topk, column length)
+ * of row b of ret_* (batch_size x only_topk) receives {row id, distance, Y value, 1} in the reference's order, ties
+ * included; every other slot is left as the caller had it.  A label key >= the model's number of labels is a fatal error
+ * before any GPU work. */
+void* c_pairwise_ann_train_drm_ip_f32(const ScipyDrmF32* pX, const ScipyCscF32* pY);
+void* c_pairwise_ann_train_csr_ip_f32(const ScipyCsrF32* pX, const ScipyCscF32* pY);
+void* c_pairwise_ann_load_drm_ip_f32(const char* model_dir, const bool lazy_load);
+void* c_pairwise_ann_load_csr_ip_f32(const char* model_dir, const bool lazy_load);
+void c_pairwise_ann_save_drm_ip_f32(void* model_ptr, const char* model_dir);
+void c_pairwise_ann_save_csr_ip_f32(void* model_ptr, const char* model_dir);
+void c_pairwise_ann_destruct_drm_ip_f32(void* model_ptr);
+void c_pairwise_ann_destruct_csr_ip_f32(void* model_ptr);
+void* c_pairwise_ann_searchers_create_drm_ip_f32(void* model_ptr, uint32_t num_searcher);
+void* c_pairwise_ann_searchers_create_csr_ip_f32(void* model_ptr, uint32_t num_searcher);
+void c_pairwise_ann_searchers_destruct_drm_ip_f32(void* searchers_ptr);
+void c_pairwise_ann_searchers_destruct_csr_ip_f32(void* searchers_ptr);
+void c_pairwise_ann_predict_drm_ip_f32(void* searchers_ptr, uint32_t batch_size, uint32_t only_topk, const ScipyDrmF32* pQ,
+                                       uint32_t* label_keys, uint32_t* ret_Imat, uint32_t* ret_Mmat, float* ret_Dmat,
+                                       float* ret_Vmat, const bool is_same_input);
+void c_pairwise_ann_predict_csr_ip_f32(void* searchers_ptr, uint32_t batch_size, uint32_t only_topk, const ScipyCsrF32* pQ,
+                                       uint32_t* label_keys, uint32_t* ret_Imat, uint32_t* ret_Mmat, float* ret_Dmat,
+                                       float* ret_Vmat, const bool is_same_input);
+/* the token's last predict call: out[4] = {pairs, distances evaluated (sum of column lengths), stored entries of the sparse
+ * rows read, pairs whose selection replayed the reference's heap sequence (ties at the top-k boundary or within it)} */
+void pb200_pairwise_ann_get_counters(void* searchers_ptr, uint64_t* out);
+/* device time (CUDA events) of the distance and select kernels of the token's last predict call, in ms */
+double pb200_pairwise_ann_kernel_ms(void* searchers_ptr);
+/* Host-only ingest check of a PairwiseANN folder (<model>/c_model), no GPU needed: pairwise_ann_t of the data type (sparse 0 =
+ * drm, 1 = csr), version, block sizes, offsets, row ids of Y within X.  Returns 0 and out[6] = {num_input_keys, num_label_keys,
+ * feat_dim, nnz of Y, nnz of X, longest column}, or 1 (reason on stderr). */
+int pb200_pairwise_ann_host_info(const char* model_dir, int sparse, uint64_t* out);
+
 /* base-vector rows kept in flight per warp by the bulk-copy (TMA) ring: 0 = direct loads, 4 (default) or 8; returns the
  * value in effect.  Results are identical for every setting.  A search whose per-warp shared-memory slice (query + ring
  * rows + result heap) would exceed 200 KB at this depth runs the next shallower one that fits (8 -> 4 -> 0); dense indices

@@ -6,6 +6,7 @@ Mirrors, for the two hot paths only, the reference's Python-side FFI layer:
 * result allocator ``ScipyCompressedSparseAllocator`` .. pecos/core/base.py:407-478
 * ``corelib.xlinear_*`` helpers ......................... pecos/core/base.py:990-1095
 * ``corelib.link_ann_hnsw_methods`` / fn_dict ........... pecos/core/base.py:1865-1964
+* ``corelib.link_pairwise_ann_methods`` / fn_dict ....... pecos/core/base.py:1966-2066
 
 There is no CPU fallback: if the CUDA library is missing, or no GPU is visible when a model is loaded,
 a ``RuntimeError`` is raised.
@@ -182,6 +183,7 @@ class B200CoreLib(object):
         self.clib_float32 = ctypes.CDLL(path)
         self.link_xlinear_methods()
         self.link_ann_hnsw_methods()
+        self.link_pairwise_ann_methods()
         self.link_b200_methods()
 
     @staticmethod
@@ -430,6 +432,51 @@ class B200CoreLib(object):
             raise NotImplementedError("data_type={}, metric_type={} is not implemented".format(data_type, metric_type))
         return self.ann_hnsw_fn_dict[key]
 
+    def link_pairwise_ann_methods(self):
+        """pairwise_ann_fn_dict[(data_type, "ip")]: the seven c_pairwise_ann_* functions with the reference's prototypes."""
+        c = self.clib_float32
+        fp = B200CoreLib.fillprototype
+        self.pairwise_ann_fn_dict = {}
+        for data_type, mat_t in (("drm", ScipyDrmF32), ("csr", ScipyCsrF32)):
+            sfx = "{}_ip_f32".format(data_type)
+            d = {"data_type": data_type, "metric_type": "ip"}
+            d["train"] = getattr(c, "c_pairwise_ann_train_" + sfx)
+            fp(d["train"], c_void_p, [POINTER(mat_t), POINTER(ScipyCscF32)])
+            d["load"] = getattr(c, "c_pairwise_ann_load_" + sfx)
+            fp(d["load"], c_void_p, [c_char_p, c_bool])
+            d["save"] = getattr(c, "c_pairwise_ann_save_" + sfx)
+            fp(d["save"], None, [c_void_p, c_char_p])
+            d["destruct"] = getattr(c, "c_pairwise_ann_destruct_" + sfx)
+            fp(d["destruct"], None, [c_void_p])
+            d["searchers_create"] = getattr(c, "c_pairwise_ann_searchers_create_" + sfx)
+            fp(d["searchers_create"], c_void_p, [c_void_p, c_uint32])
+            d["searchers_destruct"] = getattr(c, "c_pairwise_ann_searchers_destruct_" + sfx)
+            fp(d["searchers_destruct"], None, [c_void_p])
+            d["predict"] = getattr(c, "c_pairwise_ann_predict_" + sfx)
+            fp(d["predict"], None, [c_void_p, c_uint32, c_uint32, POINTER(mat_t), POINTER(c_uint32), POINTER(c_uint32),
+                                    POINTER(c_uint32), POINTER(c_float), POINTER(c_float), c_bool])
+            self.pairwise_ann_fn_dict[(data_type, "ip")] = d
+
+    def pairwise_ann_init(self, data_type, metric_type):
+        key = (data_type, metric_type)
+        if key not in self.pairwise_ann_fn_dict:
+            raise NotImplementedError("data_type={} and metric_type={} is not implemented".format(data_type, metric_type))
+        return self.pairwise_ann_fn_dict[key]
+
+    def pairwise_ann_counters(self, searchers_ptr):
+        """{pairs, distances, sparse_entries, replays} of the searcher token's last predict call."""
+        out = (c_uint64 * 4)()
+        self.clib_float32.pb200_pairwise_ann_get_counters(searchers_ptr, out)
+        return dict(zip(("pairs", "distances", "sparse_entries", "replays"), [int(v) for v in out]))
+
+    def pairwise_ann_host_info(self, c_model_dir, data_type):
+        """Host-only ingest check of a <model>/c_model folder; returns its sizes, raises ValueError if it does not load."""
+        out = (c_uint64 * 6)()
+        if self.clib_float32.pb200_pairwise_ann_host_info(c_model_dir.encode("utf-8"), 1 if data_type == "csr" else 0, out) != 0:
+            raise ValueError("pecos_b200: {} is not a loadable PairwiseANN {} folder".format(c_model_dir, data_type))
+        keys = ("num_input_keys", "num_label_keys", "feat_dim", "nnz_of_Y", "nnz_of_X", "longest_column")
+        return dict(zip(keys, [int(v) for v in out]))
+
     # ---------------------------------------------------------------- pb200_* additions
     def link_b200_methods(self):
         c = self.clib_float32
@@ -477,6 +524,9 @@ class B200CoreLib(object):
         fp(c.pb200_hnsw_launch_info, None, [c_void_p, POINTER(c_uint64)])
         fp(c.pb200_hnsw_get_info, None, [c_void_p, POINTER(c_uint64)])
         fp(c.pb200_hnsw_host_info, c_int, [c_char_p, c_int, c_int, POINTER(c_uint64)])
+        fp(c.pb200_pairwise_ann_get_counters, None, [c_void_p, POINTER(c_uint64)])
+        fp(c.pb200_pairwise_ann_kernel_ms, c_double, [c_void_p])
+        fp(c.pb200_pairwise_ann_host_info, c_int, [c_char_p, c_int, POINTER(c_uint64)])
         fp(c.pb200_sparse_block_distances, None, [c_int, c_int, c_void_p, c_void_p, c_void_p, c_uint32, c_void_p, c_void_p,
                                                   c_uint32, c_uint32, c_void_p, c_void_p, c_void_p])
         fp(c.pb200_sparse_candidate_distances, None, [c_int, c_int, c_void_p, c_void_p, c_void_p, c_uint32, c_uint32, c_void_p,

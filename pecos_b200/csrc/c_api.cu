@@ -17,6 +17,7 @@
 
 #include "hnsw_build_sparse.h"
 #include "hnsw_engine.h"
+#include "pairwise_engine.h"
 #include "xlinear_engine.h"
 
 namespace {
@@ -1241,6 +1242,148 @@ void pb200_hnsw_get_info(void* model_ptr, uint64_t* out) {
     out[0] = h.num_node; out[1] = h.feat_dim; out[2] = h.maxM; out[3] = h.maxM0; out[4] = h.max_level; out[5] = h.init_node;
     out[6] = e.index_bytes(); out[7] = e.launches();
     PB200_API_END("pb200_hnsw_get_info")
+}
+
+}  // extern "C"
+
+// ------------------------------------------------ PairwiseANN ---------------------------------------------------
+// Every handle and searcher token comes from this library: train (a deep copy, pairwise.hpp:245-263) is served here too.
+
+namespace {
+
+struct PairwiseHandle {
+    std::unique_ptr<pb200::PairwiseModel> model;
+};
+
+struct PairwiseSearchers {  // the reference's vector<Searcher>: here one stream + scratch, calls serialised on the token
+    std::unique_ptr<pb200::PairwiseSearcher> searcher;
+    std::mutex mu;
+};
+
+pb200::PairwiseModel& pairwise_of(void* ptr) {
+    if (!ptr) throw std::runtime_error("null PairwiseANN handle");
+    return *static_cast<PairwiseHandle*>(ptr)->model;
+}
+
+PairwiseSearchers& pairwise_searchers_of(void* ptr) {
+    if (!ptr) throw std::runtime_error("null PairwiseANN searchers token");
+    return *static_cast<PairwiseSearchers*>(ptr);
+}
+
+void* pairwise_wrap(std::unique_ptr<pb200::PairwiseHostModel> host) {
+    auto h = std::make_unique<PairwiseHandle>();
+    h->model = std::make_unique<pb200::PairwiseModel>(std::move(host));
+    return h.release();
+}
+
+void pairwise_check_type(void* model_ptr, bool sparse) {
+    if (pairwise_of(model_ptr).host().sparse != sparse) throw std::runtime_error("PairwiseANN handle of the other data type");
+}
+
+}  // namespace
+
+extern "C" {
+
+#define PB200_PAIRWISE_API(SUFFIX, MAT_T, SPARSE)                                                                          \
+    void* c_pairwise_ann_load##SUFFIX(const char* model_dir, const bool lazy_load) {                                      \
+        PB200_API_BEGIN                                                                                                   \
+        return pairwise_wrap(pb200::load_pairwise_model(model_dir, SPARSE, lazy_load));                                   \
+        PB200_API_END("c_pairwise_ann_load" #SUFFIX)                                                                      \
+    }                                                                                                                     \
+    void c_pairwise_ann_save##SUFFIX(void* model_ptr, const char* model_dir) {                                            \
+        PB200_API_BEGIN                                                                                                   \
+        pairwise_check_type(model_ptr, SPARSE);                                                                           \
+        pb200::save_pairwise_model(pairwise_of(model_ptr).host(), model_dir);                                             \
+        PB200_API_END("c_pairwise_ann_save" #SUFFIX)                                                                      \
+    }                                                                                                                     \
+    void c_pairwise_ann_destruct##SUFFIX(void* model_ptr) {                                                               \
+        PB200_API_BEGIN                                                                                                   \
+        delete static_cast<PairwiseHandle*>(model_ptr);                                                                   \
+        PB200_API_END("c_pairwise_ann_destruct" #SUFFIX)                                                                  \
+    }                                                                                                                     \
+    void* c_pairwise_ann_searchers_create##SUFFIX(void* model_ptr, uint32_t num_searcher) {                               \
+        PB200_API_BEGIN                                                                                                   \
+        (void)num_searcher; /* one token serves any number of pairs: the GPU kernels balance them */                      \
+        pairwise_check_type(model_ptr, SPARSE);                                                                           \
+        auto t = std::make_unique<PairwiseSearchers>();                                                                   \
+        t->searcher = std::make_unique<pb200::PairwiseSearcher>(&pairwise_of(model_ptr), g_device.load());                \
+        return t.release();                                                                                               \
+        PB200_API_END("c_pairwise_ann_searchers_create" #SUFFIX)                                                          \
+    }                                                                                                                     \
+    void c_pairwise_ann_searchers_destruct##SUFFIX(void* searchers_ptr) {                                                 \
+        PB200_API_BEGIN                                                                                                   \
+        delete static_cast<PairwiseSearchers*>(searchers_ptr);                                                            \
+        PB200_API_END("c_pairwise_ann_searchers_destruct" #SUFFIX)                                                        \
+    }
+
+PB200_PAIRWISE_API(_drm_ip_f32, ScipyDrmF32, false)
+PB200_PAIRWISE_API(_csr_ip_f32, ScipyCsrF32, true)
+
+void* c_pairwise_ann_train_drm_ip_f32(const ScipyDrmF32* pX, const ScipyCscF32* pY) {
+    PB200_API_BEGIN
+    return pairwise_wrap(pb200::pairwise_train(false, pX->rows, pX->cols, nullptr, nullptr, pX->val, pY->rows, pY->cols, pY->col_ptr,
+                                               pY->row_idx, pY->val));
+    PB200_API_END("c_pairwise_ann_train_drm_ip_f32")
+}
+
+void* c_pairwise_ann_train_csr_ip_f32(const ScipyCsrF32* pX, const ScipyCscF32* pY) {
+    PB200_API_BEGIN
+    return pairwise_wrap(pb200::pairwise_train(true, pX->rows, pX->cols, pX->row_ptr, pX->col_idx, pX->val, pY->rows, pY->cols,
+                                               pY->col_ptr, pY->row_idx, pY->val));
+    PB200_API_END("c_pairwise_ann_train_csr_ip_f32")
+}
+
+void c_pairwise_ann_predict_drm_ip_f32(void* searchers_ptr, uint32_t batch_size, uint32_t only_topk, const ScipyDrmF32* pQ,
+                                       uint32_t* label_keys, uint32_t* ret_Imat, uint32_t* ret_Mmat, float* ret_Dmat,
+                                       float* ret_Vmat, const bool is_same_input) {
+    PB200_API_BEGIN
+    auto& t = pairwise_searchers_of(searchers_ptr);
+    std::lock_guard<std::mutex> lock(t.mu);
+    t.searcher->predict(batch_size, only_topk, pQ->val, nullptr, nullptr, nullptr, pQ->rows, pQ->cols, label_keys, ret_Imat, ret_Mmat,
+                        ret_Dmat, ret_Vmat, is_same_input);
+    PB200_API_END("c_pairwise_ann_predict_drm_ip_f32")
+}
+
+void c_pairwise_ann_predict_csr_ip_f32(void* searchers_ptr, uint32_t batch_size, uint32_t only_topk, const ScipyCsrF32* pQ,
+                                       uint32_t* label_keys, uint32_t* ret_Imat, uint32_t* ret_Mmat, float* ret_Dmat,
+                                       float* ret_Vmat, const bool is_same_input) {
+    PB200_API_BEGIN
+    auto& t = pairwise_searchers_of(searchers_ptr);
+    std::lock_guard<std::mutex> lock(t.mu);
+    t.searcher->predict(batch_size, only_topk, nullptr, pQ->row_ptr, pQ->col_idx, pQ->val, pQ->rows, pQ->cols, label_keys, ret_Imat,
+                        ret_Mmat, ret_Dmat, ret_Vmat, is_same_input);
+    PB200_API_END("c_pairwise_ann_predict_csr_ip_f32")
+}
+
+void pb200_pairwise_ann_get_counters(void* searchers_ptr, uint64_t* out) {
+    PB200_API_BEGIN
+    auto& t = pairwise_searchers_of(searchers_ptr);
+    std::lock_guard<std::mutex> lock(t.mu);
+    const auto c = t.searcher->counters();
+    out[0] = c.pairs; out[1] = c.n_dist; out[2] = c.n_entries; out[3] = c.replays;
+    PB200_API_END("pb200_pairwise_ann_get_counters")
+}
+
+double pb200_pairwise_ann_kernel_ms(void* searchers_ptr) {
+    PB200_API_BEGIN
+    auto& t = pairwise_searchers_of(searchers_ptr);
+    std::lock_guard<std::mutex> lock(t.mu);
+    return t.searcher->last_kernel_ms();
+    PB200_API_END("pb200_pairwise_ann_kernel_ms")
+}
+
+int pb200_pairwise_ann_host_info(const char* model_dir, int sparse, uint64_t* out) {
+    try {
+        auto m = pb200::load_pairwise_model(model_dir, sparse != 0, false);
+        uint64_t longest = 0;
+        for (uint32_t l = 0; l < m->num_label_keys; ++l) longest = std::max<uint64_t>(longest, m->col_len(l));
+        out[0] = m->num_input_keys; out[1] = m->num_label_keys; out[2] = m->feat_dim; out[3] = m->nnz_y; out[4] = m->nnz_x;
+        out[5] = longest;
+        return 0;
+    } catch (const std::exception& e) {
+        std::fprintf(stderr, "pb200_pairwise_ann_host_info: %s\n", e.what());
+        return 1;
+    }
 }
 
 }  // extern "C"

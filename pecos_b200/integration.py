@@ -1,8 +1,8 @@
 """Overlay the GPU hot-path symbols onto a live ``pecos.core.clib`` (see INTEGRATION.md section 2).
 
 ``overlay(clib)`` re-points the XR-Linear predict-only and HNSW (dense and sparse) search function pointers of the reference's
-``corelib`` instance (pecos/core/base.py:481-539, :1951-1964) at ``libpecos_b200_float32.so``; every other symbol keeps
-using the reference CPU library.  The reference package itself is not imported here: pass its ``clib`` object in.
+``corelib`` instance (pecos/core/base.py:481-539, :1951-1964), and all seven PairwiseANN slots (base.py:1966-2051), at
+``libpecos_b200_float32.so``; every other symbol keeps using the reference CPU library.  The reference package itself is not imported here: pass its ``clib`` object in.
 """
 import ctypes
 
@@ -37,6 +37,8 @@ XLINEAR_SYMBOLS = (
     "c_mlmodel_predict_on_selected_outputs_drm_f32",
 )
 HNSW_SLOTS = ("load", "destruct", "searchers_create", "searchers_destruct", "predict", "save")
+# PairwiseANN handles all come from one library (train is a deep copy and is served here), so every slot is swapped together
+PAIRWISE_SLOTS = ("train", "load", "save", "destruct", "searchers_create", "searchers_destruct", "predict")
 
 
 def overlay(clib, lib_path=LIB_PATH, require_gpu=True):
@@ -72,6 +74,19 @@ def overlay(clib, lib_path=LIB_PATH, require_gpu=True):
             fn.restype, fn.argtypes = ref.restype, ref.argtypes
             fn_dict[key][slot] = fn
             setattr(clib.clib_float32, name, fn)  # direct attribute users see the same function as fn_dict users
+            swapped.append(name)
+    pw_dict = getattr(clib, "pairwise_ann_fn_dict", {})
+    for data_type in ("drm", "csr"):
+        key = (data_type, "ip")
+        if key not in pw_dict:
+            continue
+        for slot in PAIRWISE_SLOTS:
+            name = "c_pairwise_ann_{}_{}_ip_f32".format(slot, data_type)
+            ref = pw_dict[key][slot]
+            fn = getattr(b200, name)
+            fn.restype, fn.argtypes = ref.restype, ref.argtypes
+            pw_dict[key][slot] = fn
+            setattr(clib.clib_float32, name, fn)
             swapped.append(name)
     clib.clib_b200 = b200
     return swapped
