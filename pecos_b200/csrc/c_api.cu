@@ -183,12 +183,20 @@ std::vector<uint32_t> split_rows_by_nnz(const uint64_t* row_ptr, uint32_t rows, 
     return cut;
 }
 
-// the C-ABI matrix arguments as the engine sees them (an absent matrix: empty)
+// rows [0, rows) cut into n contiguous blocks of (nearly) equal row counts
+std::vector<uint32_t> split_rows_evenly(uint32_t rows, size_t n) {
+    std::vector<uint32_t> cut(n + 1);
+    for (size_t i = 0; i <= n; ++i) cut[i] = static_cast<uint32_t>(static_cast<uint64_t>(rows) * i / n);
+    return cut;
+}
+
+// the C-ABI matrix arguments as the engines see them (an absent matrix: empty)
 pb200::HostMatrix host_matrix(const ScipyCsrF32* Xs, const ScipyDrmF32* Xd = nullptr) {
     if (Xs) return pb200::HostMatrix{Xs->row_ptr, Xs->col_idx, Xs->val, nullptr, Xs->rows, Xs->cols};
     if (Xd) return pb200::HostMatrix{nullptr, nullptr, nullptr, Xd->val, Xd->rows, Xd->cols};
     return pb200::HostMatrix{};
 }
+pb200::HostMatrix host_matrix(const ScipyDrmF32* Xd) { return host_matrix(nullptr, Xd); }
 
 constexpr uint32_t kFanOutMinRows = 256;  // below this many rows per device a single engine serves the call
 
@@ -270,7 +278,7 @@ void c_xlinear_predict_csr_f32(void* ptr, const ScipyCsrF32* X, const uint32_t o
     const auto cut = split_rows_by_nnz(X->row_ptr, X->rows, n);
     std::vector<pb200::XLinearEngine::Result> parts(n);
     fan_out(n, [&](size_t i) {
-        const pb200::HostMatrix x{X->row_ptr + cut[i], X->col_idx, X->val, nullptr, cut[i + 1] - cut[i], X->cols};
+        const pb200::HostMatrix x = host_matrix(X).row_block(cut[i], cut[i + 1]);
         parts[i] = H.engines[i]->predict(x, overridden_beam_size, overridden_post_processor_str, overridden_only_topk);
     });
     emit_results(parts, pred_alloc);
@@ -287,11 +295,10 @@ void c_xlinear_predict_drm_f32(void* ptr, const ScipyDrmF32* X, const uint32_t o
     if (X->cols != engine_of(ptr).host().nr_features()) throw std::runtime_error("dense query width != nr_features");
     size_t n = H.engines.size();
     if (static_cast<uint64_t>(X->rows) < static_cast<uint64_t>(kFanOutMinRows) * n) n = 1;
+    const auto cut = split_rows_evenly(X->rows, n);
     std::vector<pb200::XLinearEngine::Result> parts(n);
     fan_out(n, [&](size_t i) {
-        const uint32_t r0 = static_cast<uint32_t>(static_cast<uint64_t>(X->rows) * i / n);
-        const uint32_t r1 = static_cast<uint32_t>(static_cast<uint64_t>(X->rows) * (i + 1) / n);
-        const pb200::HostMatrix x{nullptr, nullptr, nullptr, X->val + static_cast<uint64_t>(r0) * X->cols, r1 - r0, X->cols};
+        const pb200::HostMatrix x = host_matrix(X).row_block(cut[i], cut[i + 1]);
         parts[i] = H.engines[i]->predict(x, overridden_beam_size, overridden_post_processor_str, overridden_only_topk);
     });
     emit_results(parts, pred_alloc);
@@ -938,34 +945,18 @@ void* hnsw_load(const char* model_dir, bool lazy_load, int metric, bool sparse) 
     return h.release();
 }
 
-void hnsw_predict(void* model_ptr, const ScipyDrmF32* pX, uint32_t* ret_idx, float* ret_val, uint32_t efS, uint32_t topk,
-                  int metric) {
-    PB200_LOCK_HNSW(model_ptr)
-    auto& H = *static_cast<HnswHandle*>(model_ptr);
-    if (hnsw_of(model_ptr).metric() != metric) throw std::runtime_error("HNSW handle was loaded with a different metric");
-    size_t n = H.engines.size();  // replicas: contiguous row blocks, each engine writes its slice of the caller's arrays
-    if (static_cast<uint64_t>(pX->rows) < static_cast<uint64_t>(kFanOutMinRows) * n) n = 1;
-    fan_out(n, [&](size_t i) {
-        const uint32_t r0 = static_cast<uint32_t>(static_cast<uint64_t>(pX->rows) * i / n);
-        const uint32_t r1 = static_cast<uint32_t>(static_cast<uint64_t>(pX->rows) * (i + 1) / n);
-        H.engines[i]->predict(pX->val + static_cast<uint64_t>(r0) * pX->cols, r1 - r0, pX->cols, efS, topk,
-                              ret_idx + static_cast<uint64_t>(r0) * topk, ret_val + static_cast<uint64_t>(r0) * topk);
-    });
-}
-
-// sparse index, csr queries: the same row fan-out; every engine gets its rows of the caller's csr arrays
-void hnsw_predict(void* model_ptr, const ScipyCsrF32* pX, uint32_t* ret_idx, float* ret_val, uint32_t efS, uint32_t topk,
+// replicas: contiguous row blocks, each engine writes its slice of the caller's arrays
+void hnsw_predict(void* model_ptr, const pb200::HostMatrix& x, uint32_t* ret_idx, float* ret_val, uint32_t efS, uint32_t topk,
                   int metric) {
     PB200_LOCK_HNSW(model_ptr)
     auto& H = *static_cast<HnswHandle*>(model_ptr);
     if (hnsw_of(model_ptr).metric() != metric) throw std::runtime_error("HNSW handle was loaded with a different metric");
     size_t n = H.engines.size();
-    if (static_cast<uint64_t>(pX->rows) < static_cast<uint64_t>(kFanOutMinRows) * n) n = 1;
+    if (static_cast<uint64_t>(x.rows) < static_cast<uint64_t>(kFanOutMinRows) * n) n = 1;
+    const auto cut = split_rows_evenly(x.rows, n);
     fan_out(n, [&](size_t i) {
-        const uint32_t r0 = static_cast<uint32_t>(static_cast<uint64_t>(pX->rows) * i / n);
-        const uint32_t r1 = static_cast<uint32_t>(static_cast<uint64_t>(pX->rows) * (i + 1) / n);
-        H.engines[i]->predict_csr(pX->row_ptr + r0, pX->col_idx, pX->val, r1 - r0, pX->cols, efS, topk,
-                                  ret_idx + static_cast<uint64_t>(r0) * topk, ret_val + static_cast<uint64_t>(r0) * topk);
+        const uint64_t o = static_cast<uint64_t>(cut[i]) * topk;
+        H.engines[i]->predict(x.row_block(cut[i], cut[i + 1]), efS, topk, ret_idx + o, ret_val + o);
     });
 }
 
@@ -1091,7 +1082,7 @@ void pb200_hnsw_set_foreign(int metric, void* destruct, void* searchers_create, 
             g_hnsw_foreign[METRIC + 2 * SPARSE].predict(model_ptr, pX, ret_idx, ret_val, efS, topk, threads, searchers_ptr);         \
             return;                                                                                                     \
         }                                                                                                               \
-        hnsw_predict(model_ptr, pX, ret_idx, ret_val, efS, topk, METRIC);                                               \
+        hnsw_predict(model_ptr, host_matrix(pX), ret_idx, ret_val, efS, topk, METRIC);                                  \
         PB200_API_END("c_ann_hnsw_predict" #SUFFIX)                                                                     \
     }                                                                                                                   \
     void c_ann_hnsw_save##SUFFIX(void* model_ptr, const char* model_dir) {                                              \
@@ -1113,14 +1104,14 @@ PB200_HNSW_API(_csr_l2_f32, pb200::HNSW_L2, ScipyCsrF32, 1)
 void pb200_hnsw_resident_upload_csr(void* model_ptr, const ScipyCsrF32* pX) {
     PB200_API_BEGIN
     PB200_LOCK_HNSW(model_ptr)
-    hnsw_of(model_ptr).resident_upload_csr(pX->row_ptr, pX->col_idx, pX->val, pX->rows, pX->cols);
+    hnsw_of(model_ptr).resident_upload(host_matrix(pX));
     PB200_API_END("pb200_hnsw_resident_upload_csr")
 }
 
 void pb200_hnsw_resident_upload(void* model_ptr, const ScipyDrmF32* pX) {
     PB200_API_BEGIN
     PB200_LOCK_HNSW(model_ptr)
-    hnsw_of(model_ptr).resident_upload(pX->val, pX->rows, pX->cols);
+    hnsw_of(model_ptr).resident_upload(host_matrix(pX));
     PB200_API_END("pb200_hnsw_resident_upload")
 }
 
@@ -1143,7 +1134,7 @@ void pb200_hnsw_sharded_local_packed_drm(void* model_ptr, const ScipyDrmF32* pX,
                                          uint32_t id_offset, void* rec_dev) {
     PB200_API_BEGIN
     PB200_LOCK_HNSW(model_ptr)
-    hnsw_of(model_ptr).sharded_local_packed(pX->val, pX->rows, pX->cols, efS, topk, rank, id_offset, rec_dev);
+    hnsw_of(model_ptr).sharded_local_packed(host_matrix(pX), efS, topk, rank, id_offset, rec_dev);
     PB200_API_END("pb200_hnsw_sharded_local_packed_drm")
 }
 
@@ -1151,8 +1142,7 @@ void pb200_hnsw_sharded_local_packed_csr(void* model_ptr, const ScipyCsrF32* pX,
                                          uint32_t id_offset, void* rec_dev) {
     PB200_API_BEGIN
     PB200_LOCK_HNSW(model_ptr)
-    hnsw_of(model_ptr).sharded_local_packed_csr(pX->row_ptr, pX->col_idx, pX->val, pX->rows, pX->cols, efS, topk, rank, id_offset,
-                                                rec_dev);
+    hnsw_of(model_ptr).sharded_local_packed(host_matrix(pX), efS, topk, rank, id_offset, rec_dev);
     PB200_API_END("pb200_hnsw_sharded_local_packed_csr")
 }
 
@@ -1314,46 +1304,26 @@ extern "C" {
         PB200_API_BEGIN                                                                                                   \
         delete static_cast<PairwiseSearchers*>(searchers_ptr);                                                            \
         PB200_API_END("c_pairwise_ann_searchers_destruct" #SUFFIX)                                                        \
+    }                                                                                                                     \
+    void* c_pairwise_ann_train##SUFFIX(const MAT_T* pX, const ScipyCscF32* pY) {                                          \
+        PB200_API_BEGIN                                                                                                   \
+        return pairwise_wrap(                                                                                             \
+            pb200::pairwise_train(host_matrix(pX), pY->rows, pY->cols, pY->col_ptr, pY->row_idx, pY->val));               \
+        PB200_API_END("c_pairwise_ann_train" #SUFFIX)                                                                     \
+    }                                                                                                                     \
+    void c_pairwise_ann_predict##SUFFIX(void* searchers_ptr, uint32_t batch_size, uint32_t only_topk, const MAT_T* pQ,    \
+                                        uint32_t* label_keys, uint32_t* ret_Imat, uint32_t* ret_Mmat, float* ret_Dmat,    \
+                                        float* ret_Vmat, const bool is_same_input) {                                      \
+        PB200_API_BEGIN                                                                                                   \
+        auto& t = pairwise_searchers_of(searchers_ptr);                                                                   \
+        std::lock_guard<std::mutex> lock(t.mu);                                                                           \
+        t.searcher->predict(batch_size, only_topk, host_matrix(pQ), label_keys, ret_Imat, ret_Mmat, ret_Dmat, ret_Vmat,   \
+                            is_same_input);                                                                               \
+        PB200_API_END("c_pairwise_ann_predict" #SUFFIX)                                                                   \
     }
 
 PB200_PAIRWISE_API(_drm_ip_f32, ScipyDrmF32, false)
 PB200_PAIRWISE_API(_csr_ip_f32, ScipyCsrF32, true)
-
-void* c_pairwise_ann_train_drm_ip_f32(const ScipyDrmF32* pX, const ScipyCscF32* pY) {
-    PB200_API_BEGIN
-    return pairwise_wrap(pb200::pairwise_train(false, pX->rows, pX->cols, nullptr, nullptr, pX->val, pY->rows, pY->cols, pY->col_ptr,
-                                               pY->row_idx, pY->val));
-    PB200_API_END("c_pairwise_ann_train_drm_ip_f32")
-}
-
-void* c_pairwise_ann_train_csr_ip_f32(const ScipyCsrF32* pX, const ScipyCscF32* pY) {
-    PB200_API_BEGIN
-    return pairwise_wrap(pb200::pairwise_train(true, pX->rows, pX->cols, pX->row_ptr, pX->col_idx, pX->val, pY->rows, pY->cols,
-                                               pY->col_ptr, pY->row_idx, pY->val));
-    PB200_API_END("c_pairwise_ann_train_csr_ip_f32")
-}
-
-void c_pairwise_ann_predict_drm_ip_f32(void* searchers_ptr, uint32_t batch_size, uint32_t only_topk, const ScipyDrmF32* pQ,
-                                       uint32_t* label_keys, uint32_t* ret_Imat, uint32_t* ret_Mmat, float* ret_Dmat,
-                                       float* ret_Vmat, const bool is_same_input) {
-    PB200_API_BEGIN
-    auto& t = pairwise_searchers_of(searchers_ptr);
-    std::lock_guard<std::mutex> lock(t.mu);
-    t.searcher->predict(batch_size, only_topk, pQ->val, nullptr, nullptr, nullptr, pQ->rows, pQ->cols, label_keys, ret_Imat, ret_Mmat,
-                        ret_Dmat, ret_Vmat, is_same_input);
-    PB200_API_END("c_pairwise_ann_predict_drm_ip_f32")
-}
-
-void c_pairwise_ann_predict_csr_ip_f32(void* searchers_ptr, uint32_t batch_size, uint32_t only_topk, const ScipyCsrF32* pQ,
-                                       uint32_t* label_keys, uint32_t* ret_Imat, uint32_t* ret_Mmat, float* ret_Dmat,
-                                       float* ret_Vmat, const bool is_same_input) {
-    PB200_API_BEGIN
-    auto& t = pairwise_searchers_of(searchers_ptr);
-    std::lock_guard<std::mutex> lock(t.mu);
-    t.searcher->predict(batch_size, only_topk, nullptr, pQ->row_ptr, pQ->col_idx, pQ->val, pQ->rows, pQ->cols, label_keys, ret_Imat,
-                        ret_Mmat, ret_Dmat, ret_Vmat, is_same_input);
-    PB200_API_END("c_pairwise_ann_predict_csr_ip_f32")
-}
 
 void pb200_pairwise_ann_get_counters(void* searchers_ptr, uint64_t* out) {
     PB200_API_BEGIN

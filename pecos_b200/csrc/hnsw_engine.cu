@@ -272,108 +272,152 @@ __global__ void hnsw_shard_pack_kernel(const uint32_t* __restrict__ idx, const f
     rec[i] = out;
 }
 
+constexpr uint64_t kStageBytes = 32ull << 20;  // pinned staging of base rows and neighbour lists, per chunk
+
+// Copies rows [0, n) to dst through pinned staging memory: row r takes elements [off(r), off(r + 1)) of dst, and fill(r, out)
+// writes all of them, padding included, to `out`.  Chunks of whole rows of at most kStageBytes (a longer row: alone).
+template <typename T, typename Off, typename Fill>
+void stage_rows(T* dst, uint64_t n, const Off& off, const Fill& fill, cudaStream_t stream) {
+    PinnedBuffer<T> buf;  // sized once: chunks vary in size, and re-pinning costs more than the copy (grows only for a longer row)
+    buf.reserve(std::max<uint64_t>(1, std::min<uint64_t>(off(n) - off(0), kStageBytes / sizeof(T))));
+    for (uint64_t c0 = 0; c0 < n;) {
+        uint64_t c1 = c0 + 1, hi = n;  // the most rows from c0 on that fit, at least one
+        while (c1 < hi) {
+            const uint64_t mid = (c1 + hi + 1) / 2;
+            if ((off(mid) - off(c0)) * sizeof(T) <= kStageBytes) c1 = mid; else hi = mid - 1;
+        }
+        const uint64_t e0 = off(c0), en = off(c1) - e0;
+        buf.reserve(std::max<uint64_t>(en, 1));
+        parallel_for_chunks(c1 - c0, [&](uint64_t r) { fill(c0 + r, buf.get() + (off(c0 + r) - e0)); });
+        if (en) PB200_CUDA(cudaMemcpyAsync(dst + e0, buf.get(), en * sizeof(T), cudaMemcpyHostToDevice, stream));
+        PB200_CUDA(cudaStreamSynchronize(stream));
+        c0 = c1;
+    }
+}
+
+void check_shard_slots(uint32_t rank, uint32_t topk) {
+    if ((static_cast<uint64_t>(rank) + 1) * topk > static_cast<uint64_t>(kSelKeys))
+        throw std::runtime_error("pecos_b200: (rank + 1) * topk exceeds the shard merge capacity of 1024 records per query");
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------------------------
+uint32_t warp_smem_bytes(bool sparse, uint32_t vstride, int stages, uint32_t qcap, uint32_t tail) {
+    const uint32_t query = sparse ? qcap * 8u + kSpFilterWords * 4u
+                                  : vstride * 4u * (1u + static_cast<uint32_t>(stages)) + static_cast<uint32_t>(stages) * 8u;
+    return (query + tail + 15u) & ~15u;
+}
+
+CtaShape cta_shape(int device, uint32_t per_warp, uint32_t max_warps_per_sm) {
+    uint32_t warps = 8;
+    while (warps > 1 && static_cast<uint64_t>(warps) * per_warp > 96u * 1024u) warps >>= 1;
+    int sms = 132;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device);
+    const uint32_t by_smem = static_cast<uint32_t>((220u * 1024u) / (static_cast<uint64_t>(warps) * per_warp));
+    return CtaShape{warps, std::max<uint32_t>(1, std::min<uint32_t>(max_warps_per_sm / warps, by_smem)), static_cast<uint32_t>(sms)};
+}
+
+void DeviceQueries::upload(const HostMatrix& x, uint32_t rows, cudaStream_t stream) {
+    std::vector<unsigned long long> ptr;
+    if (!x.row_ptr) {
+        val_.upload(x.dense, static_cast<uint64_t>(rows) * x.cols, stream);
+        qcap_ = 0;
+    } else {
+        const uint64_t e0 = x.row_ptr[0], nnz = x.row_ptr[rows] - e0;
+        ptr.resize(static_cast<size_t>(rows) + 1);
+        uint64_t longest = 0;
+        for (uint32_t i = 0; i <= rows; ++i) {
+            ptr[i] = x.row_ptr[i] - e0;
+            if (i) longest = std::max<uint64_t>(longest, x.row_ptr[i] - x.row_ptr[i - 1]);
+        }
+        ptr_.upload(ptr.data(), ptr.size(), stream);
+        idx_.reserve(std::max<uint64_t>(nnz, 1));
+        val_.reserve(std::max<uint64_t>(nnz, 1));
+        if (nnz) {
+            PB200_CUDA(cudaMemcpyAsync(idx_.get(), x.col_idx + e0, nnz * 4, cudaMemcpyHostToDevice, stream));
+            PB200_CUDA(cudaMemcpyAsync(val_.get(), x.val + e0, nnz * 4, cudaMemcpyHostToDevice, stream));
+        }
+        qcap_ = static_cast<uint32_t>(std::min<uint64_t>(kSpQcapMax, (std::max<uint64_t>(longest, 1) + 31) / 32 * 32));
+    }
+    PB200_CUDA(cudaStreamSynchronize(stream));  // `ptr` is a local, and the caller may release x on return
+}
+
+uint64_t DeviceRows::upload(uint64_t n, uint32_t feat_dim, bool sparse, const RowFn& row, cudaStream_t stream, HnswDev* view) {
+    if (sparse) {
+        std::vector<unsigned long long> ptr(n + 1, 0ull);
+        for (uint64_t r = 0; r < n; ++r) {
+            const float* v; const uint32_t* c;
+            ptr[r + 1] = ptr[r] + row(r, &v, &c);
+        }
+        const uint64_t nnz = ptr[n];
+        sp_ptr_.upload(ptr.data(), n + 1, stream);
+        sp_ent_.reserve(std::max<uint64_t>(nnz, 1));
+        stage_rows(sp_ent_.get(), n, [&](uint64_t r) { return ptr[r]; }, [&](uint64_t r, uint2* dst) {
+            const float* v; const uint32_t* c;
+            const uint32_t len = row(r, &v, &c);
+            for (uint32_t j = 0; j < len; ++j) {
+                uint32_t bits;
+                std::memcpy(&bits, v + j, 4);
+                dst[j] = make_uint2(c[j], bits);
+            }
+        }, stream);
+        PB200_CUDA(cudaStreamSynchronize(stream));  // `ptr` is a local
+        view->sp_ptr = sp_ptr_.get();
+        view->sp_ent = sp_ent_.get();
+        return (n + 1) * 8 + nnz * 8;
+    }
+    const uint32_t vs = dense_vstride(feat_dim);
+    std::vector<uint32_t> pos(feat_dim);
+    for (uint32_t i = 0; i < feat_dim; ++i) pos[i] = dense_permuted_pos(feat_dim, i);
+    vec_.reserve(std::max<uint64_t>(n * vs, 1));
+    stage_rows(vec_.get(), n, [vs](uint64_t r) { return r * vs; }, [&](uint64_t r, float* dst) {
+        const float* v; const uint32_t* c;
+        row(r, &v, &c);
+        std::fill(dst, dst + vs, 0.0f);
+        for (uint32_t i = 0; i < feat_dim; ++i) dst[pos[i]] = v[i];
+    }, stream);
+    view->vec = vec_.get();
+    view->vstride = vs;
+    view->main_pad = dense_main_pad(feat_dim);
+    view->tail_len = dense_tail_len(feat_dim);
+    return n * vs * 4;
+}
+
 HnswEngine::HnswEngine(std::unique_ptr<HnswHostIndex> host, int device) : host_(std::move(host)), device_(device) {
     PB200_CUDA(cudaSetDevice(device_));
     PB200_CUDA(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
     for (auto& e : ev_) PB200_CUDA(cudaEventCreate(&e));
     const HnswHostIndex& H = *host_;
     const uint64_t N = H.num_node;
-    const uint32_t vs = H.sparse ? 0u : H.vstride(), n0 = H.n0stride(), d = H.feat_dim;
-    uint64_t sparse_bytes = 0;
-    if (H.sparse) {
-        // entry offsets + interleaved {index, value} entries + neighbour lists, re-laid-out on the host
-        std::vector<unsigned long long> ptr(N + 1, 0ull);
-        for (uint64_t i = 0; i < N; ++i) {
-            const float* v; const uint32_t* c;
-            ptr[i + 1] = ptr[i] + H.l0_sparse_row(static_cast<uint32_t>(i), &v, &c);
-        }
-        const uint64_t nnz = ptr[N];
-        sp_ptr_.upload(ptr.data(), N + 1, stream_);
-        sp_ent_.reserve(std::max<uint64_t>(nnz, 1));
-        nbr0_.reserve(N * n0);
-        const uint64_t chunk = std::max<uint64_t>(1, std::min<uint64_t>(N, 1u << 16));
-        PinnedBuffer<uint2> se;
-        PinnedBuffer<uint32_t> sn;
-        sn.reserve(chunk * n0);
-        for (uint64_t c0 = 0; c0 < N; c0 += chunk) {
-            const uint64_t cn = std::min(chunk, N - c0);
-            const uint64_t e0 = ptr[c0], en = ptr[c0 + cn] - e0;
-            se.reserve(std::max<uint64_t>(en, 1));
-            std::memset(sn.get(), 0, cn * n0 * 4);
-            parallel_for_chunks(cn, [&](uint64_t r) {
-                const uint32_t node = static_cast<uint32_t>(c0 + r);
-                const float* v; const uint32_t* c;
-                const uint32_t len = H.l0_sparse_row(node, &v, &c);
-                uint2* dst = se.get() + (ptr[node] - e0);
-                for (uint32_t j = 0; j < len; ++j) {
-                    uint32_t bits;
-                    std::memcpy(&bits, v + j, 4);
-                    dst[j] = make_uint2(c[j], bits);
-                }
-                const uint32_t* nb = H.l0_neighborhood(node);
-                uint32_t* nd = sn.get() + r * n0;
-                const uint32_t deg = std::min(nb[0], H.l0_max_degree);
-                nd[0] = deg;
-                for (uint32_t j = 0; j < deg; ++j) nd[1 + j] = nb[1 + j];
-            });
-            if (en) PB200_CUDA(cudaMemcpyAsync(sp_ent_.get() + e0, se.get(), en * sizeof(uint2), cudaMemcpyHostToDevice, stream_));
-            PB200_CUDA(cudaMemcpyAsync(nbr0_.get() + c0 * n0, sn.get(), cn * n0 * 4, cudaMemcpyHostToDevice, stream_));
-            PB200_CUDA(cudaStreamSynchronize(stream_));
-        }
-        sparse_bytes = (N + 1) * 8 + nnz * 8;
-    } else {
-    vec_.reserve(N * vs);
+    const uint32_t n0 = H.n0stride();
+    index_bytes_ = rows_.upload(N, H.feat_dim, H.sparse, [&H](uint64_t r, const float** v, const uint32_t** c) {
+        const uint32_t node = static_cast<uint32_t>(r);
+        if (H.sparse) return H.l0_sparse_row(node, v, c);
+        *v = H.l0_vector(node);
+        return H.feat_dim;
+    }, stream_, &view_);
     nbr0_.reserve(N * n0);
-    // re-layout in chunks through a pinned staging buffer
-    const uint64_t chunk = std::max<uint64_t>(1, std::min<uint64_t>(N, (256ull << 20) / (static_cast<uint64_t>(vs) * 4 + n0 * 4)));
-    PinnedBuffer<float> sv;
-    PinnedBuffer<uint32_t> sn;
-    sv.reserve(chunk * vs);
-    sn.reserve(chunk * n0);
-    std::vector<uint32_t> pos(d);
-    for (uint32_t i = 0; i < d; ++i) pos[i] = H.permuted_pos(i);
-    for (uint64_t c0 = 0; c0 < N; c0 += chunk) {
-        const uint64_t cn = std::min(chunk, N - c0);
-        std::memset(sv.get(), 0, cn * vs * 4);
-        std::memset(sn.get(), 0, cn * n0 * 4);
-        parallel_for_chunks(cn, [&](uint64_t r) {
-            const uint32_t node = static_cast<uint32_t>(c0 + r);
-            const float* src = H.l0_vector(node);
-            float* dst = sv.get() + r * vs;
-            for (uint32_t i = 0; i < d; ++i) dst[pos[i]] = src[i];
-            const uint32_t* nb = H.l0_neighborhood(node);
-            uint32_t* nd = sn.get() + r * n0;
-            const uint32_t deg = std::min(nb[0], H.l0_max_degree);
-            nd[0] = deg;
-            for (uint32_t j = 0; j < deg; ++j) nd[1 + j] = nb[1 + j];
-        });
-        PB200_CUDA(cudaMemcpyAsync(vec_.get() + c0 * vs, sv.get(), cn * vs * 4, cudaMemcpyHostToDevice, stream_));
-        PB200_CUDA(cudaMemcpyAsync(nbr0_.get() + c0 * n0, sn.get(), cn * n0 * 4, cudaMemcpyHostToDevice, stream_));
-        PB200_CUDA(cudaStreamSynchronize(stream_));
-    }
-    }
+    stage_rows(nbr0_.get(), N, [n0](uint64_t r) { return r * n0; }, [&H, n0](uint64_t r, uint32_t* nd) {
+        const uint32_t* nb = H.l0_neighborhood(static_cast<uint32_t>(r));
+        const uint32_t deg = std::min(nb[0], H.l0_max_degree);
+        std::fill(nd, nd + n0, 0u);
+        nd[0] = deg;
+        for (uint32_t j = 0; j < deg; ++j) nd[1 + j] = nb[1 + j];
+    }, stream_);
     uint64_t l1_len = 0;
     if (H.max_level > 0) {
         l1_len = static_cast<uint64_t>(N) * H.l1_node_mem_size;
         l1_.upload(H.l1_buffer, l1_len, stream_);
         PB200_CUDA(cudaStreamSynchronize(stream_));
     }
-    index_bytes_ = N * vs * 4 + N * n0 * 4 + l1_len * 4 + sparse_bytes;
-    view_.sp_ptr = sp_ptr_.get();
-    view_.sp_ent = sp_ent_.get();
-    view_.vec = vec_.get();
+    index_bytes_ += N * n0 * 4 + l1_len * 4;
     view_.nbr0 = nbr0_.get();
     view_.l1 = l1_.get();
     view_.num_node = H.num_node;
     view_.max_level = H.max_level;
     view_.init_node = H.init_node;
-    view_.feat_dim = d;
-    view_.vstride = vs;
-    view_.main_pad = H.sparse ? 0u : H.main_pad();
-    view_.tail_len = H.sparse ? 0u : H.tail_len();
+    view_.feat_dim = H.feat_dim;
     view_.n0stride = n0;
     view_.l0_max_degree = H.l0_max_degree;
     view_.l1_node_mem = H.l1_node_mem_size;
@@ -383,7 +427,7 @@ HnswEngine::HnswEngine(std::unique_ptr<HnswHostIndex> host, int device) : host_(
     ctrl_.reserve(8);
     PB200_CUDA(cudaMemsetAsync(ctrl_.get(), 0, 8 * sizeof(unsigned long long), stream_));
     PB200_CUDA(cudaStreamSynchronize(stream_));
-    const int max_smem = 200 * 1024;
+    const int max_smem = static_cast<int>(kWarpSmemMax);
     PB200_CUDA(cudaFuncSetAttribute(hnsw_search_kernel<HNSW_IP, 0, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
     PB200_CUDA(cudaFuncSetAttribute(hnsw_search_kernel<HNSW_L2, 0, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
     PB200_CUDA(cudaFuncSetAttribute(hnsw_search_kernel<HNSW_IP, 4, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, max_smem));
@@ -414,13 +458,9 @@ HnswEngine::~HnswEngine() {
 uint32_t HnswEngine::per_warp_smem_(uint32_t ef, int stages, uint32_t* nbmax_out) const {
     const HnswHostIndex& H = *host_;
     const uint32_t nbmax = ((std::max(H.l0_max_degree, H.l1_max_degree) + 31u) / 32u) * 32u;
-    const bool top_in_smem = ef <= kEfSmemMax;
     if (nbmax_out) *nbmax_out = nbmax;
-    if (H.sparse)  // [query indices | query values | filter | ids | distances | result heap]
-        return (qcap_ * 8u + kSpFilterWords * 4u + nbmax * 8 + (top_in_smem ? (ef + 1) * 8 : 0) + 15u) & ~15u;
-    // [query | stages ring slots | stages mbarriers | ids | distances | result heap]
-    return (H.vstride() * 4 * (1u + static_cast<uint32_t>(stages)) + static_cast<uint32_t>(stages) * 8u + nbmax * 8 +
-            (top_in_smem ? (ef + 1) * 8 : 0) + 15u) & ~15u;
+    // [staged query | ids | distances | result heap]
+    return warp_smem_bytes(H.sparse, view_.vstride, stages, queries_.qcap(), nbmax * 8 + (ef <= kEfSmemMax ? (ef + 1) * 8 : 0));
 }
 
 void HnswEngine::set_stages(int stages) {
@@ -434,7 +474,6 @@ void HnswEngine::set_stages(int stages) {
 void HnswEngine::ensure_scratch_(uint32_t ef) {
     const HnswHostIndex& H = *host_;
     const bool top_in_smem = ef <= kEfSmemMax;
-    constexpr uint32_t kWarpSmemMax = 200u * 1024u;  // the kernels' dynamic shared-memory limit (cudaFuncSetAttribute)
     int stages = stages_;
     uint32_t per_warp = per_warp_smem_(ef, stages, nullptr);
     while (stages > 0 && per_warp > kWarpSmemMax) {
@@ -445,12 +484,9 @@ void HnswEngine::ensure_scratch_(uint32_t ef) {
         throw std::runtime_error("pecos_b200: HNSW query dimension too large for the shared-memory staging area, even with "
                                  "direct loads (dense indices serve d up to about 50,000)");
     run_stages_ = H.sparse ? 0 : stages;
-    uint32_t warps = 8;
-    while (warps > 1 && static_cast<uint64_t>(warps) * per_warp > 96u * 1024u) warps >>= 1;
-    int sms = 132;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device_);
-    const uint32_t ctas_per_sm = std::max<uint32_t>(1, std::min<uint32_t>((H.sparse ? 32u : 16u) / warps, static_cast<uint32_t>((220u * 1024u) / (static_cast<uint64_t>(warps) * per_warp))));
-    uint32_t n_ctas = static_cast<uint32_t>(sms) * ctas_per_sm;
+    const CtaShape shape = cta_shape(device_, per_warp, H.sparse ? 32u : 16u);
+    const uint32_t warps = shape.warps, sms = shape.sms;
+    uint32_t n_ctas = sms * shape.ctas_per_sm;
     // bound the scratch footprint (bitmap N/8 bytes per warp)
     const uint64_t words = (static_cast<uint64_t>(H.num_node) + 31) / 32;
     uint32_t vcap = 32768;
@@ -458,7 +494,7 @@ void HnswEngine::ensure_scratch_(uint32_t ef) {
     vcap = std::max(vcap, vcap_floor_);  // raised by launch_ after a candidate-queue overflow
     vcap = static_cast<uint32_t>(std::min<uint64_t>(vcap, static_cast<uint64_t>(H.num_node) + 1));
     const uint64_t per_warp_scratch = words * 4 + static_cast<uint64_t>(vcap) * 12 + (top_in_smem ? 0 : static_cast<uint64_t>(ef + 1) * 8);
-    while (n_ctas > static_cast<uint32_t>(sms) && static_cast<uint64_t>(n_ctas) * warps * per_warp_scratch > (24ull << 30)) n_ctas -= sms;
+    while (n_ctas > sms && static_cast<uint64_t>(n_ctas) * warps * per_warp_scratch > (24ull << 30)) n_ctas -= sms;
     const uint32_t n_warps = n_ctas * warps;
     if (n_warps != n_warps_ || vcap != vcap_ || warps != warps_per_cta_) {
         bitmap_.reserve(static_cast<uint64_t>(n_warps) * words);
@@ -479,7 +515,7 @@ void HnswEngine::launch_info(uint64_t* out) const {
     out[4] = topk_heap_.capacity();
 }
 
-double HnswEngine::launch_once_(const float* q_dev, uint32_t nq, uint32_t efS, uint32_t topk, int idx_fill, bool* overflow) {
+double HnswEngine::launch_once_(uint32_t nq, uint32_t efS, uint32_t topk, int idx_fill, bool* overflow) {
     const HnswHostIndex& H = *host_;
     const uint32_t ef = std::max(efS, topk);
     if (ef == 0) throw std::runtime_error("pecos_b200: efS and topk are both zero");
@@ -493,7 +529,8 @@ double HnswEngine::launch_once_(const float* q_dev, uint32_t nq, uint32_t efS, u
     PB200_CUDA(cudaMemsetAsync(out_val_.get(), 0, static_cast<uint64_t>(nq) * topk * 4, stream_));
     const uint32_t ctas = std::max<uint32_t>(1, std::min<uint32_t>(n_ctas_, (nq + warps_per_cta_ - 1) / warps_per_cta_));
     const size_t smem = static_cast<size_t>(warps_per_cta_) * per_warp;
-    const HnswSparseQueries sq{q_ptr_.get(), q_idx_.get(), q_dev, qcap_};  // csr batch (sparse indices; q_dev = its values)
+    const float* q_dev = queries_.dense();
+    const HnswSparseQueries sq = queries_.sparse();
     PB200_CUDA(cudaEventRecord(ev_[0], stream_));
     auto launch = [&](auto kernel) {
         kernel<<<ctas, warps_per_cta_ * 32, smem, stream_>>>(view_, q_dev, sq, nq, efS, topk, ef, out_idx_.get(), out_val_.get(),
@@ -523,10 +560,10 @@ double HnswEngine::launch_once_(const float* q_dev, uint32_t nq, uint32_t efS, u
 // A query whose candidate queue outgrows the per-warp scratch (vcap entries) flags an overflow; the batch is then re-run with
 // twice the capacity (at most num_node + 1 entries, which can never overflow: a node enters the queue at most once), instead
 // of aborting the host process.
-double HnswEngine::launch_(const float* q_dev, uint32_t nq, uint32_t efS, uint32_t topk, int idx_fill) {
+double HnswEngine::launch_(uint32_t nq, uint32_t efS, uint32_t topk, int idx_fill) {
     for (;;) {
         bool overflow = false;
-        const double ms = launch_once_(q_dev, nq, efS, topk, idx_fill, &overflow);
+        const double ms = launch_once_(nq, efS, topk, idx_fill, &overflow);
         if (!overflow) return ms;
         const uint64_t cap_max = static_cast<uint64_t>(host_->num_node) + 1;
         if (vcap_ >= cap_max) throw std::runtime_error("pecos_b200: HNSW candidate queue overflow at full capacity (internal error)");
@@ -536,74 +573,33 @@ double HnswEngine::launch_(const float* q_dev, uint32_t nq, uint32_t efS, uint32
 }
 
 
-void HnswEngine::predict(const float* X, uint32_t nq, uint32_t d, uint32_t efS, uint32_t topk, uint32_t* ret_idx, float* ret_val) {
+bool HnswEngine::upload_(const HostMatrix& x, uint32_t topk) {
     PB200_CUDA(cudaSetDevice(device_));
-    if (host_->sparse) throw std::runtime_error("pecos_b200: dense queries against a sparse (csr) HNSW index");
-    if (d != host_->feat_dim) throw std::runtime_error("pecos_b200: query dimension != index dimension");
-    if (nq == 0 || topk == 0) return;
-    q_dev_.upload(X, static_cast<uint64_t>(nq) * d, stream_);
-    out_idx_.reserve(static_cast<uint64_t>(nq) * topk);
-    out_val_.reserve(static_cast<uint64_t>(nq) * topk);
-    launch_(q_dev_.get(), nq, efS, topk);
+    if (host_->sparse && !x.row_ptr) throw std::runtime_error("pecos_b200: dense queries against a sparse (csr) HNSW index");
+    if (!host_->sparse && x.row_ptr) throw std::runtime_error("pecos_b200: csr queries against a dense HNSW index");
+    if (x.cols != host_->feat_dim) throw std::runtime_error("pecos_b200: query dimension != index dimension");
+    if (x.rows == 0 || topk == 0) return false;
+    const uint32_t qcap = queries_.qcap();
+    queries_.upload(x, x.rows, stream_);
+    if (queries_.qcap() != qcap) n_warps_ = 0;  // launch geometry depends on the staging capacity
+    return true;
+}
+
+void HnswEngine::predict(const HostMatrix& x, uint32_t efS, uint32_t topk, uint32_t* ret_idx, float* ret_val) {
+    if (!upload_(x, topk)) return;
+    const uint64_t n = static_cast<uint64_t>(x.rows) * topk;
+    out_idx_.reserve(n);
+    out_val_.reserve(n);
+    launch_(x.rows, efS, topk);
     // rows with fewer than topk results keep the caller's zeros (libpecos.cpp:554-558): our buffers were zeroed too
-    PB200_CUDA(cudaMemcpyAsync(ret_idx, out_idx_.get(), static_cast<uint64_t>(nq) * topk * 4, cudaMemcpyDeviceToHost, stream_));
-    PB200_CUDA(cudaMemcpyAsync(ret_val, out_val_.get(), static_cast<uint64_t>(nq) * topk * 4, cudaMemcpyDeviceToHost, stream_));
+    PB200_CUDA(cudaMemcpyAsync(ret_idx, out_idx_.get(), n * 4, cudaMemcpyDeviceToHost, stream_));
+    PB200_CUDA(cudaMemcpyAsync(ret_val, out_val_.get(), n * 4, cudaMemcpyDeviceToHost, stream_));
     PB200_CUDA(cudaStreamSynchronize(stream_));
 }
 
-// csr query batch -> device (row offsets rebased to the batch), and the per-warp staging capacity for its longest row
-void HnswEngine::upload_csr_(const uint64_t* row_ptr, const uint32_t* col_idx, const float* val, uint32_t nq) {
-    const uint64_t e0 = row_ptr[0], nnz = row_ptr[nq] - e0;
-    std::vector<unsigned long long> ptr(static_cast<size_t>(nq) + 1);
-    uint64_t longest = 0;
-    for (uint32_t i = 0; i <= nq; ++i) {
-        ptr[i] = row_ptr[i] - e0;
-        if (i) longest = std::max<uint64_t>(longest, row_ptr[i] - row_ptr[i - 1]);
-    }
-    q_ptr_.upload(ptr.data(), static_cast<uint64_t>(nq) + 1, stream_);
-    q_idx_.reserve(std::max<uint64_t>(nnz, 1));
-    q_dev_.reserve(std::max<uint64_t>(nnz, 1));
-    if (nnz) {
-        PB200_CUDA(cudaMemcpyAsync(q_idx_.get(), col_idx + e0, nnz * 4, cudaMemcpyHostToDevice, stream_));
-        PB200_CUDA(cudaMemcpyAsync(q_dev_.get(), val + e0, nnz * 4, cudaMemcpyHostToDevice, stream_));
-    }
-    PB200_CUDA(cudaStreamSynchronize(stream_));  // `ptr` is a local
-    const uint32_t qcap = static_cast<uint32_t>(std::min<uint64_t>(kSpQcapMax, (std::max<uint64_t>(longest, 1) + 31) / 32 * 32));
-    if (qcap != qcap_) { qcap_ = qcap; n_warps_ = 0; }  // launch geometry depends on the staging capacity
-}
-
-void HnswEngine::predict_csr(const uint64_t* row_ptr, const uint32_t* col_idx, const float* val, uint32_t nq, uint32_t cols,
-                             uint32_t efS, uint32_t topk, uint32_t* ret_idx, float* ret_val) {
-    PB200_CUDA(cudaSetDevice(device_));
-    if (!host_->sparse) throw std::runtime_error("pecos_b200: csr queries against a dense HNSW index");
-    if (cols != host_->feat_dim) throw std::runtime_error("pecos_b200: query dimension != index dimension");
-    if (nq == 0 || topk == 0) return;
-    upload_csr_(row_ptr, col_idx, val, nq);
-    out_idx_.reserve(static_cast<uint64_t>(nq) * topk);
-    out_val_.reserve(static_cast<uint64_t>(nq) * topk);
-    launch_(q_dev_.get(), nq, efS, topk);
-    PB200_CUDA(cudaMemcpyAsync(ret_idx, out_idx_.get(), static_cast<uint64_t>(nq) * topk * 4, cudaMemcpyDeviceToHost, stream_));
-    PB200_CUDA(cudaMemcpyAsync(ret_val, out_val_.get(), static_cast<uint64_t>(nq) * topk * 4, cudaMemcpyDeviceToHost, stream_));
-    PB200_CUDA(cudaStreamSynchronize(stream_));
-}
-
-void HnswEngine::resident_upload_csr(const uint64_t* row_ptr, const uint32_t* col_idx, const float* val, uint32_t nq, uint32_t cols) {
-    PB200_CUDA(cudaSetDevice(device_));
-    if (!host_->sparse) throw std::runtime_error("pecos_b200: csr queries against a dense HNSW index");
-    if (cols != host_->feat_dim) throw std::runtime_error("pecos_b200: query dimension != index dimension");
-    upload_csr_(row_ptr, col_idx, val, nq);
-    res_nq_ = nq;
-    res_d_ = cols;
-}
-
-void HnswEngine::resident_upload(const float* X, uint32_t nq, uint32_t d) {
-    PB200_CUDA(cudaSetDevice(device_));
-    if (host_->sparse) throw std::runtime_error("pecos_b200: dense queries against a sparse (csr) HNSW index");
-    if (d != host_->feat_dim) throw std::runtime_error("pecos_b200: query dimension != index dimension");
-    q_dev_.upload(X, static_cast<uint64_t>(nq) * d, stream_);
-    PB200_CUDA(cudaStreamSynchronize(stream_));
-    res_nq_ = nq;
-    res_d_ = d;
+void HnswEngine::resident_upload(const HostMatrix& x) {
+    upload_(x, 1);  // searched later with resident_predict's topk
+    res_nq_ = x.rows;
 }
 
 double HnswEngine::resident_predict(uint32_t efS, uint32_t topk) {
@@ -612,7 +608,7 @@ double HnswEngine::resident_predict(uint32_t efS, uint32_t topk) {
     out_idx_.reserve(static_cast<uint64_t>(res_nq_) * topk);
     out_val_.reserve(static_cast<uint64_t>(res_nq_) * topk);
     res_topk_ = topk;
-    return launch_(q_dev_.get(), res_nq_, efS, topk);
+    return launch_(res_nq_, efS, topk);
 }
 
 void HnswEngine::resident_fetch(uint32_t* ret_idx, float* ret_val) {
@@ -622,44 +618,19 @@ void HnswEngine::resident_fetch(uint32_t* ret_idx, float* ret_val) {
 }
 
 // search into out_idx_ / out_val_ (empty slots 0xFFFFFFFF), then pack the records into the caller's device buffer
-void HnswEngine::shard_pack_(uint32_t nq, uint32_t efS, uint32_t topk, uint32_t rank, uint32_t id_offset, void* rec_dev) {
-    const uint64_t n = static_cast<uint64_t>(nq) * topk;
+void HnswEngine::sharded_local_packed(const HostMatrix& x, uint32_t efS, uint32_t topk, uint32_t rank, uint32_t id_offset,
+                                      void* rec_dev) {
+    check_shard_slots(rank, topk);
+    if (!upload_(x, topk)) return;
+    const uint64_t n = static_cast<uint64_t>(x.rows) * topk;
     out_idx_.reserve(n);
     out_val_.reserve(n);
-    launch_(q_dev_.get(), nq, efS, topk, 0xFF);
+    launch_(x.rows, efS, topk, 0xFF);
     hnsw_shard_pack_kernel<<<static_cast<uint32_t>((n + 255) / 256), 256, 0, stream_>>>(out_idx_.get(), out_val_.get(), n, topk, rank,
                                                                                       id_offset, static_cast<ShardRecord*>(rec_dev));
     PB200_CUDA(cudaGetLastError());
     ++launches_;
     PB200_CUDA(cudaStreamSynchronize(stream_));
-}
-
-static void check_shard_slots(uint32_t rank, uint32_t topk) {
-    if ((static_cast<uint64_t>(rank) + 1) * topk > static_cast<uint64_t>(kSelKeys))
-        throw std::runtime_error("pecos_b200: (rank + 1) * topk exceeds the shard merge capacity of 1024 records per query");
-}
-
-void HnswEngine::sharded_local_packed(const float* X, uint32_t nq, uint32_t d, uint32_t efS, uint32_t topk, uint32_t rank,
-                                      uint32_t id_offset, void* rec_dev) {
-    PB200_CUDA(cudaSetDevice(device_));
-    if (host_->sparse) throw std::runtime_error("pecos_b200: dense queries against a sparse (csr) HNSW index");
-    if (d != host_->feat_dim) throw std::runtime_error("pecos_b200: query dimension != index dimension");
-    check_shard_slots(rank, topk);
-    if (nq == 0 || topk == 0) return;
-    q_dev_.upload(X, static_cast<uint64_t>(nq) * d, stream_);
-    shard_pack_(nq, efS, topk, rank, id_offset, rec_dev);
-}
-
-void HnswEngine::sharded_local_packed_csr(const uint64_t* row_ptr, const uint32_t* col_idx, const float* val, uint32_t nq,
-                                          uint32_t cols, uint32_t efS, uint32_t topk, uint32_t rank, uint32_t id_offset,
-                                          void* rec_dev) {
-    PB200_CUDA(cudaSetDevice(device_));
-    if (!host_->sparse) throw std::runtime_error("pecos_b200: csr queries against a dense HNSW index");
-    if (cols != host_->feat_dim) throw std::runtime_error("pecos_b200: query dimension != index dimension");
-    check_shard_slots(rank, topk);
-    if (nq == 0 || topk == 0) return;
-    upload_csr_(row_ptr, col_idx, val, nq);
-    shard_pack_(nq, efS, topk, rank, id_offset, rec_dev);
 }
 
 void HnswEngine::sharded_merge_packed(uint32_t world, uint32_t rows, uint32_t topk, const void* g_rec, uint32_t* ret_idx,

@@ -8,6 +8,7 @@
 //   FeatVecDense{IP,L2}Simd::distance  pecos/core/ann/feat_vectors.hpp:134-162 + distance_impl/x86.hpp:121-157, :256-296
 #pragma once
 
+#include <functional>
 #include <memory>
 #include <vector>
 
@@ -44,6 +45,53 @@ struct HnswCounters {  // algorithmic-byte counters of SURVEY.md 8(d), totals ov
     unsigned long long n_entries = 0;  // sparse indices: stored entries of the evaluated base rows (8 bytes each)
 };
 
+// One warp's shared-memory slice may take at most this much; also the search kernels' dynamic shared-memory limit.
+constexpr uint32_t kWarpSmemMax = 200u * 1024u;
+
+// Bytes of one warp's shared-memory slice (a multiple of 16): the staged query -- dense, the query row plus `stages` bulk-copy
+// ring rows and their mbarriers; sparse, qcap indices and values plus the index filter -- followed by `tail` bytes of the
+// caller's own.
+uint32_t warp_smem_bytes(bool sparse, uint32_t vstride, int stages, uint32_t qcap, uint32_t tail);
+
+// CTA shape of a search launch with `per_warp` bytes of shared memory per warp: 8 warps per CTA, halved while a CTA would
+// take more than 96 KB; as many CTAs per SM (at least one) as max_warps_per_sm warps and 220 KB of shared memory allow.
+struct CtaShape {
+    uint32_t warps, ctas_per_sm, sms;
+};
+CtaShape cta_shape(int device, uint32_t per_warp, uint32_t max_warps_per_sm);
+
+// A query batch in HBM, as the search kernels take it: dense rows, or csr rows with offsets rebased to the batch.
+class DeviceQueries {
+public:
+    // the first `rows` rows of x, on `stream`; returns once x is no longer read
+    void upload(const HostMatrix& x, uint32_t rows, cudaStream_t stream);
+    const float* dense() const { return val_.get(); }  // dense rows (csr: the values)
+    HnswSparseQueries sparse() const { return HnswSparseQueries{ptr_.get(), idx_.get(), val_.get(), qcap_}; }
+    uint32_t qcap() const { return qcap_; }  // csr: entries staged per warp (the longest row, rounded up to 32, at most kSpQcapMax)
+
+private:
+    DeviceBuffer<float> val_;
+    DeviceBuffer<unsigned long long> ptr_;
+    DeviceBuffer<uint32_t> idx_;
+    uint32_t qcap_ = 0;
+};
+
+// The base rows in HBM as the search kernels read them (layouts in hnsw_host.h): dense rows in the permuted layout, or
+// sparse rows as sp_ptr offsets and interleaved {index, value bits} entries.
+class DeviceRows {
+public:
+    // row(r, &val, &idx): the values of row r and, sparse, its ascending indices; returns its stored entries (dense: feat_dim)
+    using RowFn = std::function<uint32_t(uint64_t r, const float** val, const uint32_t** idx)>;
+    // uploads rows [0, n) on `stream`, sets the row fields of *view (vec, vstride, main_pad, tail_len, sp_ptr, sp_ent) and
+    // returns the bytes placed in HBM
+    uint64_t upload(uint64_t n, uint32_t feat_dim, bool sparse, const RowFn& row, cudaStream_t stream, HnswDev* view);
+
+private:
+    DeviceBuffer<float> vec_;
+    DeviceBuffer<unsigned long long> sp_ptr_;
+    DeviceBuffer<uint2> sp_ent_;
+};
+
 class HnswEngine {
 public:
     HnswEngine(std::unique_ptr<HnswHostIndex> host, int device);
@@ -51,30 +99,24 @@ public:
 
     const HnswHostIndex& host() const { return *host_; }
     int metric() const { return host_->metric; }
-
-    // Host-buffer entry point: X row-major nq x d; ret arrays nq x topk (caller-zeroed, like the reference).
-    void predict(const float* X, uint32_t nq, uint32_t d, uint32_t efS, uint32_t topk, uint32_t* ret_idx, float* ret_val);
-
-    // Sparse index, csr queries (column indices ascending within a row): the same walk, distances by ordered sparse intersection.
-    void predict_csr(const uint64_t* row_ptr, const uint32_t* col_idx, const float* val, uint32_t nq, uint32_t cols, uint32_t efS,
-                     uint32_t topk, uint32_t* ret_idx, float* ret_val);
-    void resident_upload_csr(const uint64_t* row_ptr, const uint32_t* col_idx, const float* val, uint32_t nq, uint32_t cols);
     bool sparse() const { return host_->sparse; }
 
+    // Host-buffer entry point: x holds nq queries, dense rows for a dense index or csr rows (column indices ascending within a
+    // row) for a sparse one, whose distances are ordered sparse intersections; ret arrays nq x topk (caller-zeroed, like the
+    // reference).
+    void predict(const HostMatrix& x, uint32_t efS, uint32_t topk, uint32_t* ret_idx, float* ret_val);
+
     // Device-resident queries (bench "value" leg).
-    void resident_upload(const float* X, uint32_t nq, uint32_t d);
+    void resident_upload(const HostMatrix& x);
     double resident_predict(uint32_t efS, uint32_t topk);  // returns device ms of the search kernel
     void resident_fetch(uint32_t* ret_idx, float* ret_val);
 
-    // Index sharding (one graph per shard, one engine per rank).  sharded_local_packed{,_csr} search this shard and write
+    // Index sharding (one graph per shard, one engine per rank).  sharded_local_packed searches this shard and writes
     // [nq][topk] 16-byte ShardRecords (shard_merge.cuh) to the caller-owned device buffer rec_dev:
     //   key = (~orderable(dist) << 32) | ~(rank * topk + slot), id = id_offset + local id, val = dist; key 0 = empty slot.
     // sharded_merge_packed merges the all-gathered [world][rows][topk] records into ret arrays rows x topk; rows with fewer
     // than topk results keep zeros, as in predict.
-    void sharded_local_packed(const float* X, uint32_t nq, uint32_t d, uint32_t efS, uint32_t topk, uint32_t rank,
-                              uint32_t id_offset, void* rec_dev);
-    void sharded_local_packed_csr(const uint64_t* row_ptr, const uint32_t* col_idx, const float* val, uint32_t nq, uint32_t cols,
-                                  uint32_t efS, uint32_t topk, uint32_t rank, uint32_t id_offset, void* rec_dev);
+    void sharded_local_packed(const HostMatrix& x, uint32_t efS, uint32_t topk, uint32_t rank, uint32_t id_offset, void* rec_dev);
     void sharded_merge_packed(uint32_t world, uint32_t rows, uint32_t topk, const void* g_rec, uint32_t* ret_idx, float* ret_val);
 
     HnswCounters counters();
@@ -91,19 +133,21 @@ public:
     void launch_info(uint64_t* out) const;
 
 private:
+    // selects the device, checks x against the index and uploads it, unless there is nothing to search (no rows or topk 0):
+    // returns whether it did
+    bool upload_(const HostMatrix& x, uint32_t topk);
     void ensure_scratch_(uint32_t ef);
     uint32_t per_warp_smem_(uint32_t ef, int stages, uint32_t* nbmax_out) const;
     // idx_fill: byte value out_idx_ is filled with before the search (0: the reference's zeros; 0xFF: empty slots read
     // 0xFFFFFFFF, which no node id can be, for the shard pack kernel)
-    double launch_(const float* q_dev, uint32_t nq, uint32_t efS, uint32_t topk, int idx_fill = 0);
-    double launch_once_(const float* q_dev, uint32_t nq, uint32_t efS, uint32_t topk, int idx_fill, bool* overflow);
-    void shard_pack_(uint32_t nq, uint32_t efS, uint32_t topk, uint32_t rank, uint32_t id_offset, void* rec_dev);
+    double launch_(uint32_t nq, uint32_t efS, uint32_t topk, int idx_fill = 0);
+    double launch_once_(uint32_t nq, uint32_t efS, uint32_t topk, int idx_fill, bool* overflow);
 
     std::unique_ptr<HnswHostIndex> host_;
     int device_ = 0;
     cudaStream_t stream_ = nullptr;
     cudaEvent_t ev_[2] = {nullptr, nullptr};
-    DeviceBuffer<float> vec_;
+    DeviceRows rows_;
     DeviceBuffer<uint32_t> nbr0_;
     DeviceBuffer<uint32_t> l1_;
     HnswDev view_{};
@@ -122,19 +166,11 @@ private:
     DeviceBuffer<uint2> topk_heap_;
     DeviceBuffer<unsigned long long> ctrl_;  // [0] query counter, [1] error flag, [2..5] counters
 
-    DeviceBuffer<unsigned long long> sp_ptr_;
-    DeviceBuffer<uint2> sp_ent_;
-    DeviceBuffer<unsigned long long> q_ptr_;  // csr query batch
-    DeviceBuffer<uint32_t> q_idx_;
-    uint32_t qcap_ = 0;
-    void upload_csr_(const uint64_t* row_ptr, const uint32_t* col_idx, const float* val, uint32_t nq);
-    DeviceBuffer<float> q_dev_;
+    DeviceQueries queries_;
     DeviceBuffer<uint32_t> out_idx_;
     DeviceBuffer<float> out_val_;
     DeviceBuffer<uint32_t> merge_cnt_;  // per-query result counts of the shard merge
-    uint32_t res_nq_ = 0, res_d_ = 0, res_topk_ = 0;
-    PinnedBuffer<uint32_t> stage_idx_;
-    PinnedBuffer<float> stage_val_;
+    uint32_t res_nq_ = 0, res_topk_ = 0;
 
     uint64_t launches_ = 0;
     double last_ms_ = 0.0;

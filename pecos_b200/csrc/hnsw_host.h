@@ -30,6 +30,22 @@ namespace pb200 {
 
 enum HnswMetric { HNSW_IP = 0, HNSW_L2 = 1 };
 
+// The dense device row layout above, for rows of d components: the permuted main part, its padded length, the natural-order
+// tail and the row stride (floats)
+inline uint32_t dense_len16(uint32_t d) { return d / 16u; }
+inline uint32_t dense_main_pad(uint32_t d) { return 64u * ((dense_len16(d) + 3u) / 4u); }
+inline uint32_t dense_tail_len(uint32_t d) { return d - 16u * dense_len16(d); }
+inline uint32_t dense_vstride(uint32_t d) { return dense_main_pad(d) + (dense_tail_len(d) ? 16u : 0u); }
+// component i of a d-component vector -> position inside its dense_vstride(d)-long device row
+inline uint32_t dense_permuted_pos(uint32_t d, uint32_t i) {
+    const uint32_t m = 16u * dense_len16(d);
+    if (i < m) {
+        const uint32_t k = i / 16u, j = i % 16u;
+        return 64u * (k / 4u) + 4u * j + (k % 4u);
+    }
+    return dense_main_pad(d) + (i - m);
+}
+
 struct HnswHostIndex {
     uint32_t num_node = 0, maxM = 0, maxM0 = 0, efC = 0, max_level = 0, init_node = 0;
     uint32_t feat_dim = 0;
@@ -45,11 +61,6 @@ struct HnswHostIndex {
     uint64_t l1_buffer_len = 0;
     uint32_t l1_max_level = 0, l1_max_degree = 0, l1_node_mem_size = 0, l1_level_mem_size = 0;
 
-    // derived device layout parameters
-    uint32_t len16() const { return feat_dim / 16; }
-    uint32_t main_pad() const { return 64u * ((len16() + 3u) / 4u); }
-    uint32_t tail_len() const { return feat_dim - 16u * len16(); }
-    uint32_t vstride() const { return main_pad() + (tail_len() ? 16u : 0u); }
     uint32_t n0stride() const { return (1u + l0_max_degree + 3u) & ~3u; }
 
     const uint32_t* l0_neighborhood(uint32_t node) const {
@@ -66,15 +77,6 @@ struct HnswHostIndex {
     const float* l0_vector(uint32_t node) const {
         return reinterpret_cast<const float*>(l0_buffer + static_cast<uint64_t>(node) * l0_node_mem_size +
                                               static_cast<uint64_t>(1 + l0_max_degree) * 4 + 4);
-    }
-    // component i of a vector -> position inside a vstride()-long device row
-    uint32_t permuted_pos(uint32_t i) const {
-        const uint32_t m = 16u * len16();
-        if (i < m) {
-            const uint32_t k = i / 16u, j = i % 16u;
-            return 64u * (k / 4u) + 4u * j + (k % 4u);
-        }
-        return main_pad() + (i - m);
     }
 };
 

@@ -32,6 +32,26 @@
 
 namespace pb200 {
 
+// Host view of a caller's matrix (queries, codes or a selected-outputs pattern): CSR (row_ptr/col_idx/val, absolute
+// offsets) or row-major dense (dense).  An empty HostMatrix stands for "not given".
+struct HostMatrix {
+    const uint64_t* row_ptr = nullptr;
+    const uint32_t* col_idx = nullptr;
+    const float* val = nullptr;
+    const float* dense = nullptr;
+    uint32_t rows = 0;
+    uint32_t cols = 0;
+
+    // rows [r0, r1) (CSR: the offsets stay absolute into col_idx / val)
+    HostMatrix row_block(uint32_t r0, uint32_t r1) const {
+        HostMatrix b = *this;
+        if (row_ptr) b.row_ptr = row_ptr + r0;
+        else b.dense = dense + static_cast<uint64_t>(r0) * cols;
+        b.rows = r1 - r0;
+        return b;
+    }
+};
+
 // ----------------------------------------------------------------------------------------------
 // Read-only memory mapped file
 // ----------------------------------------------------------------------------------------------

@@ -258,63 +258,21 @@ const HnswDev& PairwiseModel::device_view(int device) {
     }
     PB200_CUDA(cudaSetDevice(device));
     const PairwiseHostModel& H = *host_;
-    const uint64_t N = H.num_input_keys;
     cudaStream_t st = nullptr;
     PB200_CUDA(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
     HnswDev v{};
     v.feat_dim = H.feat_dim;
     v.metric = HNSW_IP;
     v.num_node = H.num_input_keys;
-    if (H.sparse) {
-        std::vector<unsigned long long> ptr(H.x_ptr, H.x_ptr + N + 1);
-        sp_ptr_.upload(ptr.data(), N + 1, st);
-        sp_ent_.reserve(std::max<uint64_t>(H.nnz_x, 1));
-        const uint64_t chunk = 1ull << 22;
-        PinnedBuffer<uint2> se;
-        se.reserve(std::min<uint64_t>(chunk, std::max<uint64_t>(H.nnz_x, 1)));
-        for (uint64_t e0 = 0; e0 < H.nnz_x; e0 += chunk) {
-            const uint64_t en = std::min(chunk, H.nnz_x - e0);
-            parallel_for_chunks((en + 4095) / 4096, [&](uint64_t b) {
-                for (uint64_t j = b * 4096; j < std::min(en, (b + 1) * 4096); ++j) {
-                    uint32_t bits;
-                    std::memcpy(&bits, H.x_val + e0 + j, 4);
-                    se.get()[j] = make_uint2(H.x_idx[e0 + j], bits);
-                }
-            });
-            PB200_CUDA(cudaMemcpyAsync(sp_ent_.get() + e0, se.get(), en * sizeof(uint2), cudaMemcpyHostToDevice, st));
-            PB200_CUDA(cudaStreamSynchronize(st));
+    rows_.upload(H.num_input_keys, H.feat_dim, H.sparse, [&H](uint64_t r, const float** val, const uint32_t** idx) {
+        if (!H.sparse) {
+            *val = H.x_val + r * H.feat_dim;
+            return H.feat_dim;
         }
-        PB200_CUDA(cudaStreamSynchronize(st));
-        v.sp_ptr = sp_ptr_.get();
-        v.sp_ent = sp_ent_.get();
-    } else {
-        HnswHostIndex geo;  // the HNSW permuted row layout, so that the HNSW distance code reads the rows unchanged
-        geo.feat_dim = H.feat_dim;
-        const uint32_t vs = geo.vstride(), d = H.feat_dim;
-        vec_.reserve(std::max<uint64_t>(N * vs, 1));
-        if (N * vs) {
-            std::vector<uint32_t> pos(d);
-            for (uint32_t i = 0; i < d; ++i) pos[i] = geo.permuted_pos(i);
-            const uint64_t chunk = std::max<uint64_t>(1, (256ull << 20) / (static_cast<uint64_t>(vs) * 4));
-            PinnedBuffer<float> sv;
-            sv.reserve(std::min(chunk, N) * vs);
-            for (uint64_t c0 = 0; c0 < N; c0 += chunk) {
-                const uint64_t cn = std::min(chunk, N - c0);
-                std::memset(sv.get(), 0, cn * vs * 4);
-                parallel_for_chunks(cn, [&](uint64_t r) {
-                    const float* src = H.x_val + (c0 + r) * d;
-                    float* dst = sv.get() + r * vs;
-                    for (uint32_t i = 0; i < d; ++i) dst[pos[i]] = src[i];
-                });
-                PB200_CUDA(cudaMemcpyAsync(vec_.get() + c0 * vs, sv.get(), cn * vs * 4, cudaMemcpyHostToDevice, st));
-                PB200_CUDA(cudaStreamSynchronize(st));
-            }
-        }
-        v.vec = vec_.get();
-        v.vstride = vs;
-        v.main_pad = geo.main_pad();
-        v.tail_len = geo.tail_len();
-    }
+        *val = H.x_val + H.x_ptr[r];
+        *idx = H.x_idx + H.x_ptr[r];
+        return static_cast<uint32_t>(H.x_ptr[r + 1] - H.x_ptr[r]);
+    }, st, &v);
     std::vector<unsigned long long> cp(H.col_ptr, H.col_ptr + static_cast<uint64_t>(H.num_label_keys) + 1);
     col_ptr_.upload(cp.data(), cp.size(), st);
     row_idx_.reserve(std::max<uint64_t>(H.nnz_y, 1));
@@ -347,8 +305,7 @@ PairwiseSearcher::~PairwiseSearcher() {
     if (stream_) cudaStreamDestroy(stream_);
 }
 
-void PairwiseSearcher::predict(uint32_t batch, uint32_t topk, const float* q_dense, const uint64_t* q_ptr, const uint32_t* q_idx,
-                               const float* q_val, uint32_t rows, uint32_t cols, const uint32_t* label_keys, uint32_t* ret_I,
+void PairwiseSearcher::predict(uint32_t batch, uint32_t topk, const HostMatrix& q, const uint32_t* label_keys, uint32_t* ret_I,
                                uint32_t* ret_M, float* ret_D, float* ret_V, bool is_same_input) {
     const PairwiseHostModel& H = model_->host();
     counters_ = PairwiseCounters{};
@@ -360,36 +317,15 @@ void PairwiseSearcher::predict(uint32_t batch, uint32_t topk, const float* q_den
             throw std::runtime_error("pecos_b200: label_keys[" + std::to_string(b) + "] = " + std::to_string(label_keys[b]) +
                                      " is out of range (num_label_keys = " + std::to_string(H.num_label_keys) + ")");
     const uint32_t need_rows = is_same_input ? 1u : batch;
-    if (rows < need_rows) throw std::runtime_error("pecos_b200: PairwiseANN query matrix has fewer rows than the batch needs");
-    if (cols != H.feat_dim) throw std::runtime_error("pecos_b200: PairwiseANN query dimension != feat_dim");
-    if ((q_ptr != nullptr) != H.sparse) throw std::runtime_error("pecos_b200: PairwiseANN query type differs from the model's");
+    if (q.rows < need_rows) throw std::runtime_error("pecos_b200: PairwiseANN query matrix has fewer rows than the batch needs");
+    if (q.cols != H.feat_dim) throw std::runtime_error("pecos_b200: PairwiseANN query dimension != feat_dim");
+    if ((q.row_ptr != nullptr) != H.sparse) throw std::runtime_error("pecos_b200: PairwiseANN query type differs from the model's");
 
     PB200_CUDA(cudaSetDevice(device_));
     const HnswDev ix = model_->device_view(device_);
 
-    // queries: the rows the batch uses
-    HnswSparseQueries sq{nullptr, nullptr, nullptr, 0u};
-    if (H.sparse) {
-        const uint64_t e0 = q_ptr[0], nnz = q_ptr[need_rows] - e0;
-        std::vector<unsigned long long> ptr(static_cast<size_t>(need_rows) + 1);
-        uint64_t longest = 0;
-        for (uint32_t i = 0; i <= need_rows; ++i) {
-            ptr[i] = q_ptr[i] - e0;
-            if (i) longest = std::max<uint64_t>(longest, q_ptr[i] - q_ptr[i - 1]);
-        }
-        q_ptr_.upload(ptr.data(), ptr.size(), stream_);
-        q_idx_.reserve(std::max<uint64_t>(nnz, 1));
-        q_val_.reserve(std::max<uint64_t>(nnz, 1));
-        if (nnz) {
-            PB200_CUDA(cudaMemcpyAsync(q_idx_.get(), q_idx + e0, nnz * 4, cudaMemcpyHostToDevice, stream_));
-            PB200_CUDA(cudaMemcpyAsync(q_val_.get(), q_val + e0, nnz * 4, cudaMemcpyHostToDevice, stream_));
-        }
-        PB200_CUDA(cudaStreamSynchronize(stream_));  // `ptr` is a local
-        sq = HnswSparseQueries{q_ptr_.get(), q_idx_.get(), q_val_.get(),
-                               static_cast<uint32_t>(std::min<uint64_t>(kSpQcapMax, (std::max<uint64_t>(longest, 1) + 31) / 32 * 32))};
-    } else {
-        q_dense_.upload(q_dense, static_cast<uint64_t>(need_rows) * cols, stream_);
-    }
+    queries_.upload(q, need_rows, stream_);  // the rows the batch uses
+    const HnswSparseQueries sq = queries_.sparse();
     // the caller's result slots travel both ways: slots the reference leaves untouched stay as the caller had them
     const uint64_t n_out = static_cast<uint64_t>(batch) * topk;
     out_I_.upload(ret_I, n_out, stream_);
@@ -398,27 +334,16 @@ void PairwiseSearcher::predict(uint32_t batch, uint32_t topk, const float* q_den
     out_V_.upload(ret_V, n_out, stream_);
     PB200_CUDA(cudaMemsetAsync(ctrl_.get(), 0, 4 * sizeof(unsigned long long), stream_));
 
-    // launch geometry of the distance kernel
-    int sms = 132;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device_);
-    constexpr uint32_t kWarpSmemMax = 200u * 1024u;
-    auto dense_bytes = [&](int stages) {
-        return (ix.vstride * 4u * (1u + static_cast<uint32_t>(stages)) + static_cast<uint32_t>(stages) * 8u + kSlice * 4u + 15u) & ~15u;
-    };
-    int stages = 0;
-    uint32_t per_warp;
-    if (H.sparse) {
-        per_warp = (sq.qcap * 8u + kSpFilterWords * 4u + kSlice * 4u + 15u) & ~15u;
-    } else {
-        stages = (ix.vstride > 0 && dense_bytes(4) <= kWarpSmemMax) ? 4 : 0;
-        per_warp = dense_bytes(stages);
-        if (per_warp > kWarpSmemMax)
-            throw std::runtime_error("pecos_b200: PairwiseANN feat_dim too large for the shared-memory staging area (about 50,000 at most)");
-    }
-    uint32_t warps = 8;
-    while (warps > 1 && warps * per_warp > 96u * 1024u) warps >>= 1;
+    // launch geometry of the distance kernel: [staged query | distances of a slice] per warp; dense rows through a ring of 4
+    // where it fits, else direct loads
+    auto per_warp_bytes = [&](int stages) { return warp_smem_bytes(H.sparse, ix.vstride, stages, sq.qcap, kSlice * 4u); };
+    const int stages = (!H.sparse && ix.vstride > 0 && per_warp_bytes(4) <= kWarpSmemMax) ? 4 : 0;
+    const uint32_t per_warp = per_warp_bytes(stages);
+    if (per_warp > kWarpSmemMax)
+        throw std::runtime_error("pecos_b200: PairwiseANN feat_dim too large for the shared-memory staging area (about 50,000 at most)");
+    const CtaShape shape = cta_shape(device_, per_warp, 64u);
+    const uint32_t warps = shape.warps, sms = shape.sms, ctas_per_sm = shape.ctas_per_sm;
     const uint32_t cta_smem = warps * per_warp;
-    const uint32_t ctas_per_sm = std::max<uint32_t>(1, std::min<uint32_t>(64u / warps, (220u * 1024u) / cta_smem));
     auto dist_kernel = H.sparse ? pw_distance_kernel<0, true> : (stages ? pw_distance_kernel<4, false> : pw_distance_kernel<0, false>);
     PB200_CUDA(cudaFuncSetAttribute(dist_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(cta_smem)));
 
@@ -451,10 +376,10 @@ void PairwiseSearcher::predict(uint32_t batch, uint32_t topk, const float* q_den
             scratch_.reserve(total);
             PB200_CUDA(cudaMemsetAsync(ctrl_.get(), 0, sizeof(unsigned long long), stream_));
             const uint32_t n_items = static_cast<uint32_t>(items.size());
-            const uint32_t ctas = std::max<uint32_t>(1, std::min<uint32_t>(static_cast<uint32_t>(sms) * ctas_per_sm, (n_items + warps - 1) / warps));
-            const uint32_t sel_ctas = std::max<uint32_t>(1, std::min<uint32_t>(static_cast<uint32_t>(sms) * 16u, (np + kSelectWarps - 1) / kSelectWarps));
+            const uint32_t ctas = std::max<uint32_t>(1, std::min<uint32_t>(sms * ctas_per_sm, (n_items + warps - 1) / warps));
+            const uint32_t sel_ctas = std::max<uint32_t>(1, std::min<uint32_t>(sms * 16u, (np + kSelectWarps - 1) / kSelectWarps));
             PB200_CUDA(cudaEventRecord(ev_[0], stream_));
-            dist_kernel<<<ctas, warps * 32, cta_smem, stream_>>>(ix, q_dense_.get(), sq, pairs_.get(), pair_off_.get(), items_.get(), n_items,
+            dist_kernel<<<ctas, warps * 32, cta_smem, stream_>>>(ix, queries_.dense(), sq, pairs_.get(), pair_off_.get(), items_.get(), n_items,
                                                                 model_->row_idx(), scratch_.get(), per_warp, ctrl_.get());
             PB200_CUDA(cudaGetLastError());
             pw_select_kernel<<<sel_ctas, kSelectWarps * 32, 0, stream_>>>(pairs_.get(), pair_off_.get(), np, topk, scratch_.get(),

@@ -37,9 +37,7 @@ private:
     bool uploaded_ = false;
     int device_ = 0;
     HnswDev view_{};
-    DeviceBuffer<float> vec_;                 // dense: [N][vstride] in the HNSW permuted row layout
-    DeviceBuffer<unsigned long long> sp_ptr_;  // sparse: row offsets
-    DeviceBuffer<uint2> sp_ent_;               // sparse: {index, value bits} entries
+    DeviceRows rows_;  // X_trn, as the HNSW distance code reads it
     DeviceBuffer<unsigned long long> col_ptr_;
     DeviceBuffer<uint32_t> row_idx_;
     DeviceBuffer<float> y_val_;
@@ -57,10 +55,9 @@ class PairwiseSearcher {
 public:
     PairwiseSearcher(PairwiseModel* model, int device);
     ~PairwiseSearcher();
-    // Host buffers in and out.  Q: dense rows (q_dense, d columns) or csr (q_ptr / q_idx / q_val); `rows` query rows given.
+    // Host buffers in and out.  q: dense or csr query rows, of the model's kind.
     // ret_* hold batch x topk slots; only slot k < min(topk, column length) of each pair is written.
-    void predict(uint32_t batch, uint32_t topk, const float* q_dense, const uint64_t* q_ptr, const uint32_t* q_idx,
-                 const float* q_val, uint32_t rows, uint32_t cols, const uint32_t* label_keys, uint32_t* ret_I, uint32_t* ret_M,
+    void predict(uint32_t batch, uint32_t topk, const HostMatrix& q, const uint32_t* label_keys, uint32_t* ret_I, uint32_t* ret_M,
                  float* ret_D, float* ret_V, bool is_same_input);
     PairwiseCounters counters() const { return counters_; }
     double last_kernel_ms() const { return last_ms_; }
@@ -70,10 +67,7 @@ private:
     int device_ = 0;
     cudaStream_t stream_ = nullptr;
     cudaEvent_t ev_[2] = {nullptr, nullptr};
-    DeviceBuffer<float> q_dense_;
-    DeviceBuffer<unsigned long long> q_ptr_;
-    DeviceBuffer<uint32_t> q_idx_;
-    DeviceBuffer<float> q_val_;
+    DeviceQueries queries_;
     DeviceBuffer<uint4> pairs_;    // per pair: {query row, column length, column start (u64 as 2 words)}
     DeviceBuffer<unsigned long long> pair_off_;  // per pair: offset of its scratch
     DeviceBuffer<uint2> items_;    // distance work items {pair, first position}

@@ -68,16 +68,16 @@ struct PairwiseHostModel {
     }
 };
 
-// c_pairwise_ann_train_*: deep copies (X rows = Y rows is required, as in the reference)
-inline std::unique_ptr<PairwiseHostModel> pairwise_train(bool sparse, uint32_t x_rows, uint32_t x_cols, const uint64_t* x_ptr,
-                                                         const uint32_t* x_idx, const float* x_val, uint32_t y_rows, uint32_t y_cols,
-                                                         const uint64_t* y_ptr, const uint32_t* y_idx, const float* y_val) {
-    if (x_rows != y_rows) throw std::runtime_error("X_trn.rows != Y_csc.rows");
+// c_pairwise_ann_train_*: deep copies of X (dense or csr) and Y_csc (X rows = Y rows is required, as in the reference)
+inline std::unique_ptr<PairwiseHostModel> pairwise_train(const HostMatrix& x, uint32_t y_rows, uint32_t y_cols, const uint64_t* y_ptr,
+                                                         const uint32_t* y_idx, const float* y_val) {
+    if (x.rows != y_rows) throw std::runtime_error("X_trn.rows != Y_csc.rows");
+    const bool sparse = x.row_ptr != nullptr;
     auto m = std::make_unique<PairwiseHostModel>();
     m->sparse = sparse;
     m->num_input_keys = y_rows;
     m->num_label_keys = y_cols;
-    m->feat_dim = x_cols;
+    m->feat_dim = x.cols;
     const uint64_t y0 = y_ptr[0];
     m->nnz_y = y_ptr[y_cols] - y0;
     m->own_col_ptr.resize(static_cast<size_t>(y_cols) + 1);
@@ -85,15 +85,15 @@ inline std::unique_ptr<PairwiseHostModel> pairwise_train(bool sparse, uint32_t x
     m->own_row_idx.assign(y_idx + y0, y_idx + y0 + m->nnz_y);
     m->own_y_val.assign(y_val + y0, y_val + y0 + m->nnz_y);
     if (sparse) {
-        const uint64_t x0 = x_ptr[0];
-        m->nnz_x = x_ptr[x_rows] - x0;
-        m->own_x_ptr.resize(static_cast<size_t>(x_rows) + 1);
-        for (uint32_t r = 0; r <= x_rows; ++r) m->own_x_ptr[r] = x_ptr[r] - x0;
-        m->own_x_idx.assign(x_idx + x0, x_idx + x0 + m->nnz_x);
-        m->own_x_val.assign(x_val + x0, x_val + x0 + m->nnz_x);
+        const uint64_t x0 = x.row_ptr[0];
+        m->nnz_x = x.row_ptr[x.rows] - x0;
+        m->own_x_ptr.resize(static_cast<size_t>(x.rows) + 1);
+        for (uint32_t r = 0; r <= x.rows; ++r) m->own_x_ptr[r] = x.row_ptr[r] - x0;
+        m->own_x_idx.assign(x.col_idx + x0, x.col_idx + x0 + m->nnz_x);
+        m->own_x_val.assign(x.val + x0, x.val + x0 + m->nnz_x);
     } else {
-        m->nnz_x = static_cast<uint64_t>(x_rows) * x_cols;
-        m->own_x_val.assign(x_val, x_val + m->nnz_x);
+        m->nnz_x = static_cast<uint64_t>(x.rows) * x.cols;
+        m->own_x_val.assign(x.dense, x.dense + m->nnz_x);
     }
     m->col_ptr = m->own_col_ptr.data();
     m->row_idx = m->own_row_idx.data();

@@ -61,17 +61,6 @@ struct QueryDev {
     uint32_t max_row_nnz;     // longest row of the batch (sizes the shared-memory staging of the query)
 };
 
-// Host view of a caller's matrix (queries, codes or a selected-outputs pattern): CSR (row_ptr/col_idx/val, absolute
-// offsets) or row-major dense (dense).  An empty HostMatrix stands for "not given".
-struct HostMatrix {
-    const uint64_t* row_ptr = nullptr;
-    const uint32_t* col_idx = nullptr;
-    const float* val = nullptr;
-    const float* dense = nullptr;
-    uint32_t rows = 0;
-    uint32_t cols = 0;
-};
-
 struct XLinearStats {  // algorithmic-byte counters of SURVEY.md section 8(d), accumulated by the STATS kernel variant
     unsigned long long chunks;      // (query, chunk) products evaluated
     unsigned long long chunk_rows;  // sum R_p
