@@ -17,8 +17,8 @@
 //     begins (a pair's cost grows with its chunk's entry count: cm_pair_cost), stages that chunk's image by ONE bulk
 //     asynchronous copy (cp.async.bulk + mbarrier, the TMA engine's non-tensor form), and its warps CLAIM 32-pair slices of
 //     the chunk from a per-chunk cursor (one atomicAdd per slice) until the chunk runs dry; then the CTA moves to the chunk
-//     with the most unclaimed estimated work.  Work moves between SMs at run time, so the launch ends when the last slice
-//     does, not when the CTA with the most expensive static share does;
+//     with the most unclaimed estimated work per CTA on it (a per-chunk count of the CTAs there).  Work moves between SMs at
+//     run time, so the launch ends when the last slice does, not when the CTA with the most expensive static share does;
 //   * a lane walks its pair's query features in ascending order (staged global -> shared by cp.async, rounds of 8 in
 //     flight), compacts the hits of a round in place as {entry range, x}, then streams the hit rows' entries as one flat
 //     stream, kCmSlots entries per trip across row boundaries AND across rounds: after round r's lookup the warp runs only
@@ -26,7 +26,8 @@
 //     largest backlog of a lane rather than each round's busiest lane; one drain (with the bias row) ends the pair.  The
 //     entries go into the lane's PRIVATE accumulators acc[column][lane].  That is the reference's marching loop
 //     (inference.hpp:788-811): ascending feature order, separate multiply and add, bias row last; a column is only ever
-//     touched by the lane that owns the pair: no compaction across lanes, no conflict resolution.
+//     touched by the lane that owns the pair: no compaction across lanes, no conflict resolution.  The scores leave through
+//     a shared-memory tile, 8 consecutive columns of 4 pairs per store instruction.
 //
 // Bit-identical to the query-major kernels (tests/test_chunk_major_gpu.py).  Eligibility: shape (cm_shape, at load: width
 // <= 256, rows / entries per chunk < 65535, image + 4 warps fit in shared memory, images within PB200_CMIMG_MB) and call
@@ -52,6 +53,7 @@ struct CmWork {
     uint32_t* pair_q;       // [pairs] query of a pair, grouped by chunk
     uint32_t* pair_pos;     // [pairs] candidate position of the pair's first column inside the query's row
     uint32_t* claim;        // [n_chunks] first unclaimed pair of a chunk's bucket (at or past bucket_ptr[c + 1]: none left)
+    uint32_t* active;       // [n_chunks] CTAs of the score kernel currently on the chunk
 };
 
 struct CmPlan {  // per call
@@ -326,7 +328,8 @@ __device__ __forceinline__ uint64_t warp_incl_scan64(uint64_t v, int lane) {
 }
 
 // single CTA: exclusive scans of the pair counts (bucket offsets) and of the chunks' estimated work (cost_ptr); count[]
-// becomes the scatter cursor and claim[] the score kernel's claim cursor.  A chunk's entry count is read from its image header.
+// becomes the scatter cursor and claim[] the score kernel's claim cursor; active[] starts at 0.  A chunk's entry count is
+// read from its image header.
 __global__ void __launch_bounds__(1024)
 xl_cm_scan_kernel(const uint32_t n_chunks, CmWork w, const unsigned char* __restrict__ images, const uint32_t img_bytes,
                   const uint32_t w_rows) {
@@ -362,6 +365,7 @@ xl_cm_scan_kernel(const uint32_t n_chunks, CmWork w, const unsigned char* __rest
             w.cost_ptr[c] = ex_c;
             w.count[c] = ex_p;  // cursor
             w.claim[c] = ex_p;
+            w.active[c] = 0;
         }
         __syncthreads();
         if (threadIdx.x == 1023) { carry_pairs = ex_p + n; carry_cost = ex_c + cost; }
@@ -414,9 +418,9 @@ __device__ inline uint32_t cm_start_chunk(const CmWork& w, uint32_t n_vc, uint32
 // slots (entries added; a trip offers 32 x kCmSlots), and the slices and pairs it scored, in g_cm_trace:
 //   [0] grid, [1] warps per CTA, [2] pairs of the launch, then per CTA: start ns, end ns, images staged,
 //   kCmMaxWarps x (kCmPhases cycles, trips, useful slots, slices, pairs).
-// The image phase covers a chunk switch: the barrier, the choice of the next chunk and the bulk copy.
+// A chunk switch is two phases: the barrier with the choice of the next chunk, and the wait for the bulk copy.
 // Without the define CmTrace is empty and the kernel is unchanged.
-enum { kCmPhImage, kCmPhStaging, kCmPhLookup, kCmPhAccumulate, kCmPhSlice, kCmPhases };
+enum { kCmPhSwitch, kCmPhCopy, kCmPhStaging, kCmPhLookup, kCmPhAccumulate, kCmPhSlice, kCmPhases };
 #ifdef PB200_CM_TRACE
 constexpr uint32_t kCmTraceCtas = 1024;
 constexpr uint32_t kCmTraceWarp = kCmPhases + 4;
@@ -606,7 +610,7 @@ xl_cm_scores_kernel(const LayerDev L, const QueryDev X, const CmWork w, const Cm
         cm_mbar_wait(mbar, parity);
         parity ^= 1u;
         trace.staged();
-        trace.mark(kCmPhImage);
+        trace.mark(kCmPhCopy);
         bias_range = hdr_s[0];
         n_cols = hdr_s[1];
     };
@@ -761,9 +765,32 @@ xl_cm_scores_kernel(const LayerDev L, const QueryDev X, const CmWork w, const Cm
                     }
                 }
                 P.beam_cnt[q] = P.n0;
-            } else {
-                float* dst = cand + static_cast<uint64_t>(q) * cand_stride_q + pos;
-                for (uint32_t col = 0; col < n_cols; ++col) dst[col] = my_acc[col * 32];
+            }
+        }
+        if constexpr (!PREFIX) {
+            // write-out, kCmFeat columns at a time through a [32][kStride] tile in the last round's buffer (free once the
+            // drain is done; the next slice's first stage_round comes after a __syncwarp): lane i puts its pair's columns
+            // into row i, then every store instruction writes kCmFeat consecutive columns of each of kPerIter pairs (the
+            // staging geometry: this lane serves column fl of the pairs sub, sub + kPerIter, ...) where a store per column
+            // touched 32 scattered candidate rows
+            float* tile = st_val + ((buf + kNBuf - 1) % kNBuf) * kBuf;
+            const uint32_t n_pairs = s_end - s0;
+            const uint64_t o_mine = have ? static_cast<uint64_t>(q) * cand_stride_q + pos : 0u;
+            float* dst[kIters];
+#pragma unroll
+            for (int it = 0; it < kIters; ++it) dst[it] = cand + __shfl_sync(kFull, o_mine, it * kPerIter + sub) + fl;
+            for (uint32_t c0 = 0; c0 < n_cols; c0 += kCmFeat) {
+                const uint32_t nc = min(static_cast<uint32_t>(kCmFeat), n_cols - c0);
+                __syncwarp();
+#pragma unroll
+                for (int k = 0; k < kCmFeat; ++k)
+                    if (static_cast<uint32_t>(k) < nc) tile[lane * kStride + k] = my_acc[(c0 + k) * 32];
+                __syncwarp();
+                if (static_cast<uint32_t>(fl) < nc) {
+#pragma unroll
+                    for (int it = 0; it < kIters; ++it)
+                        if (static_cast<uint32_t>(it * kPerIter + sub) < n_pairs) dst[it][c0] = tile[(it * kPerIter + sub) * kStride + fl];
+                }
             }
         }
         trace.slice(s_end - s0);
@@ -782,17 +809,27 @@ xl_cm_scores_kernel(const LayerDev L, const QueryDev X, const CmWork w, const Cm
         trace.flush(warp, lane, P.rows);
     } else {
         // Claim cursors decide which pairs this CTA scores, so the output cannot depend on the schedule: a pair's result
-        // goes to the place its query and position fix.  The cursors are read back through L2 (__ldcg): the claims of
-        // other SMs are atomics there, and a stale line in this SM's L1 could show a dry chunk as unclaimed again and again.
+        // goes to the place its query and position fix.  The cursors and CTA counts are read back through L2 (__ldcg): the
+        // claims of other SMs are atomics there, and a stale line in this SM's L1 could show a dry chunk as unclaimed
+        // again and again.
         const uint32_t n_vc = S.n_vc;
         __shared__ unsigned long long s_pick_work[kCmMaxWarps];
+        __shared__ uint32_t s_pick_act[kCmMaxWarps];
         __shared__ uint32_t s_pick_c[kCmMaxWarps];
-        // the better of two candidates (work, chunk): more unclaimed work first, then the lower index; n_vc = none
-        auto better = [n_vc](unsigned long long wa, uint32_t ca, unsigned long long wb, uint32_t cb) {
-            return ca != n_vc && (cb == n_vc || wa > wb || (wa == wb && ca < cb));
+        // the better of two candidates (unclaimed work, CTAs on the chunk, chunk): more work per CTA once this one joins,
+        // work / (active + 1), compared crosswise (work < 2^32 pairs x 2^17, active <= grid: the products fit 64 bits),
+        // then the lower index; n_vc = none.  CTAs that become free together spread over the chunks instead of all
+        // draining the one with the most work and switching again.
+        auto better = [n_vc](unsigned long long wa, uint32_t aa, uint32_t ca, unsigned long long wb, uint32_t ab, uint32_t cb) {
+            if (ca == n_vc) return false;
+            if (cb == n_vc) return true;
+            const unsigned long long la = wa * (ab + 1u), lb = wb * (aa + 1u);
+            return la > lb || (la == lb && ca < cb);
         };
         uint32_t c = cm_start_chunk(w, n_vc, blockIdx.x, gridDim.x);
+        trace.mark(kCmPhSwitch);
         while (c < n_vc) {
+            if (threadIdx.x == 0) atomicAdd(w.active + c, 1u);
             stage_image(c);
             const uint32_t c_end = w.bucket_ptr[c + 1];
             for (;;) {  // warps claim the chunk's slices until it runs dry
@@ -802,31 +839,37 @@ xl_cm_scores_kernel(const LayerDev L, const QueryDev X, const CmWork w, const Cm
                 if (s0 >= c_end) break;
                 score_slice(s0, min(s0 + 32u, c_end));
             }
-            // every warp has left the image: the CTA moves to the chunk with the most unclaimed estimated work.  A cursor
-            // read here may already be stale; that only affects the choice, as the claims themselves are atomic.
+            // every warp has left the image: the CTA leaves the chunk and moves to the one with the most unclaimed
+            // estimated work per CTA.  A cursor or count read here may already be stale; that only affects the choice, as
+            // the claims themselves are atomic.
             __syncthreads();
+            if (threadIdx.x == 0) atomicSub(w.active + c, 1u);
             unsigned long long bw = 0;
-            uint32_t bc = n_vc;
+            uint32_t ba = 0, bc = n_vc;
             for (uint32_t v = threadIdx.x; v < n_vc; v += blockDim.x) {
                 const uint32_t v_end = w.bucket_ptr[v + 1];
                 const uint32_t cl = __ldcg(w.claim + v);
                 if (cl >= v_end) continue;
                 const uint32_t entries = reinterpret_cast<const uint32_t*>(images + static_cast<uint64_t>(v) * S.img_bytes)[3];
                 const unsigned long long work = static_cast<unsigned long long>(v_end - cl) * cm_pair_cost(L.w_rows, entries);
-                if (better(work, v, bw, bc)) { bw = work; bc = v; }
+                const uint32_t act = __ldcg(w.active + v);
+                if (better(work, act, v, bw, ba, bc)) { bw = work; ba = act; bc = v; }
             }
             for (int d = 16; d > 0; d >>= 1) {
                 const unsigned long long ow = __shfl_xor_sync(kFull, bw, d);
+                const uint32_t oa = __shfl_xor_sync(kFull, ba, d);
                 const uint32_t oc = __shfl_xor_sync(kFull, bc, d);
-                if (better(ow, oc, bw, bc)) { bw = ow; bc = oc; }
+                if (better(ow, oa, oc, bw, ba, bc)) { bw = ow; ba = oa; bc = oc; }
             }
-            if (lane == 0) { s_pick_work[warp] = bw; s_pick_c[warp] = bc; }
+            if (lane == 0) { s_pick_work[warp] = bw; s_pick_act[warp] = ba; s_pick_c[warp] = bc; }
             __syncthreads();
             // s_pick_* are rewritten only after the next switch's first barrier, which every thread reaches after this read
             bw = s_pick_work[0];
+            ba = s_pick_act[0];
             c = s_pick_c[0];
             for (int k = 1; k < nwarps; ++k)
-                if (better(s_pick_work[k], s_pick_c[k], bw, c)) { bw = s_pick_work[k]; c = s_pick_c[k]; }
+                if (better(s_pick_work[k], s_pick_act[k], s_pick_c[k], bw, ba, c)) { bw = s_pick_work[k]; ba = s_pick_act[k]; c = s_pick_c[k]; }
+            trace.mark(kCmPhSwitch);
         }
         trace.flush(warp, lane, w.bucket_ptr[n_vc]);
     }

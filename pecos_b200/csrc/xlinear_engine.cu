@@ -1203,6 +1203,7 @@ uint32_t XLinearEngine::ensure_workspace_(const std::vector<LayerPlan>& plan, ui
         cm_pair_pos_.reserve(tile * pairs);
         cm_count_.reserve(chunks_max * 4 + 1);
         cm_claim_.reserve(chunks_max * 4 + 1);
+        cm_active_.reserve(chunks_max * 4 + 1);
         cm_bucket_ptr_.reserve(chunks_max * 4 + 1);
         cm_cost_ptr_.reserve(chunks_max * 4 + 1);
     }
@@ -1257,7 +1258,7 @@ int XLinearEngine::score_layer_(size_t d, const QueryDev& q, uint32_t b_prev, in
         const CmShape& shape = layers_[d].cm_shape;
         const uint32_t n_vc = shape.n_vc;
         CmWork w{cm_slot_pos_.get(), cm_count_.get(), cm_bucket_ptr_.get(), cm_cost_ptr_.get(), cm_pair_q_.get(), cm_pair_pos_.get(),
-                 cm_claim_.get()};
+                 cm_claim_.get(), cm_active_.get()};
         PB200_CUDA(cudaMemsetAsync(w.count, 0, (static_cast<uint64_t>(n_vc) + 1) * 4, stream_));
         const uint32_t warp_grid = (rows * 32u + 127u) / 128u;
         xl_cm_count_kernel<<<warp_grid, 128, 0, stream_>>>(L, q, bid, bcnt, beam_stride_, rows, w, shape.vc_ptr);

@@ -291,7 +291,7 @@ private:
     // Layer 0's beam into beam_*_[1] and layer 1's raw scores into its candidate rows, for rows [ws_row, ws_row + q.rows).
     void launch_prefix_(const QueryDev& q, const std::vector<LayerPlan>& plan, uint32_t ws_row);
     uint32_t n_sm_ = 132;
-    DeviceBuffer<uint32_t> cm_slot_pos_, cm_count_, cm_claim_, cm_bucket_ptr_, cm_pair_q_, cm_pair_pos_;
+    DeviceBuffer<uint32_t> cm_slot_pos_, cm_count_, cm_claim_, cm_active_, cm_bucket_ptr_, cm_pair_q_, cm_pair_pos_;
     DeviceBuffer<uint64_t> cm_cost_ptr_;
     bool force_block_topk_ = false;  // A/B switch: first-generation kernels (row-list streaming + block-wide sort)
     std::vector<XLinearLayerProfile> layer_profile_;

@@ -4,8 +4,8 @@ Builds a side copy of the library with -DPB200_CM_TRACE into a temporary directo
 the eurlex-4k workload of bench.py (same model and query seeds) through it, and prints, for the last launch of
 xl_cm_scores_kernel (the leaf layer):
   * per-CTA elapsed time from %globaltimer (max / mean / min over the CTAs, and max / mean);
-  * per-warp clock64 cycles by phase: image wait, query staging wait, lookup + compaction, accumulate, slice set-up +
-    output (mean over the warps, and the share of each phase);
+  * per-warp clock64 cycles by phase: chunk switch (barrier + choice of the next chunk), bulk-copy wait, query staging
+    wait, lookup + compaction, accumulate, slice set-up + output (mean over the warps, and the share of each phase);
   * accumulate trips per warp and lane efficiency: entries added / (trips x 32 lanes x 4 slots);
   * per CTA: slices claimed, images staged (chunk switches + 1) and pairs scored (mean / min / max).
 It fails if the pairs scored, summed over the CTAs, differ from the pairs bucketed for the launch: every pair must be
@@ -26,7 +26,7 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-PHASES = ["image_wait", "staging_wait", "lookup_compact", "accumulate", "slice_setup_output"]
+PHASES = ["switch_choice", "copy_wait", "staging_wait", "lookup_compact", "accumulate", "slice_setup_output"]
 MAX_WARPS = 16  # kCmMaxWarps
 TRACE_CTAS = 1024  # kCmTraceCtas
 WARP_FIELDS = len(PHASES) + 4  # kCmTraceWarp: phase cycles, trips, useful slots, slices, pairs
