@@ -202,43 +202,30 @@ class B200CoreLib(object):
         fp(c.c_xlinear_destruct_model, None, [c_void_p])
         fp(c.c_xlinear_get_int_attr, c_uint32, [c_void_p, c_char_p])
         fp(c.c_xlinear_get_layer_type, c_int, [c_void_p, c_int])
-        pred_args = [c_uint32, c_char_p, c_uint32, c_int, ScipyCompressedSparseAllocator.CFUNCTYPE]
-        fp(c.c_xlinear_predict_csr_f32, None, [c_void_p, POINTER(ScipyCsrF32)] + pred_args)
-        fp(c.c_xlinear_predict_drm_f32, None, [c_void_p, POINTER(ScipyDrmF32)] + pred_args)
-
-        sel_args = [POINTER(ScipyCsrF32), c_char_p, c_int, ScipyCompressedSparseAllocator.CFUNCTYPE]  # pecos/core/base.py:846-876
-        fp(c.c_xlinear_predict_on_selected_outputs_csr_f32, None, [c_void_p, POINTER(ScipyCsrF32)] + sel_args)
-        fp(c.c_xlinear_predict_on_selected_outputs_drm_f32, None, [c_void_p, POINTER(ScipyDrmF32)] + sel_args)
-
         # single-layer mmap handles (pecos/core/base.py:541-606)
         fp(c.c_mlmodel_load_mmap_model, c_void_p, [c_char_p, c_bool])
         fp(c.c_mlmodel_destruct_model, None, [c_void_p])
         fp(c.c_mlmodel_get_int_attr, c_uint32, [c_void_p, c_char_p])
         fp(c.c_mlmodel_compile_mmap_model, None, [c_char_p, c_char_p])
-        ml_args = [POINTER(ScipyCsrF32), c_char_p, c_uint32, c_int, ScipyCompressedSparseAllocator.CFUNCTYPE]
-        fp(c.c_mlmodel_predict_csr_f32, None, [c_void_p, POINTER(ScipyCsrF32)] + ml_args)
-        fp(c.c_mlmodel_predict_drm_f32, None, [c_void_p, POINTER(ScipyDrmF32)] + ml_args)
-        ml_sel = [POINTER(ScipyCsrF32), POINTER(ScipyCsrF32), c_char_p, c_int, ScipyCompressedSparseAllocator.CFUNCTYPE]
-        fp(c.c_mlmodel_predict_on_selected_outputs_csr_f32, None, [c_void_p, POINTER(ScipyCsrF32)] + ml_sel)
-        fp(c.c_mlmodel_predict_on_selected_outputs_drm_f32, None, [c_void_p, POINTER(ScipyDrmF32)] + ml_sel)
-
-        single = [POINTER(ScipyCsrF32), POINTER(ScipyCscF32), POINTER(ScipyCscF32), c_char_p, c_uint32, c_int, c_float,
-                  ScipyCompressedSparseAllocator.CFUNCTYPE]  # pecos/core/base.py:880-933
-        fp(c.c_xlinear_single_layer_predict_csr_f32, None, [POINTER(ScipyCsrF32)] + single)
-        fp(c.c_xlinear_single_layer_predict_drm_f32, None, [POINTER(ScipyDrmF32)] + single)
-        single_sel = [POINTER(ScipyCsrF32), POINTER(ScipyCsrF32), POINTER(ScipyCscF32), POINTER(ScipyCscF32), c_char_p, c_int, c_float,
-                      ScipyCompressedSparseAllocator.CFUNCTYPE]  # pecos/core/base.py:936-976
-        fp(c.c_xlinear_single_layer_predict_on_selected_outputs_csr_f32, None, [POINTER(ScipyCsrF32)] + single_sel)
-        fp(c.c_xlinear_single_layer_predict_on_selected_outputs_drm_f32, None, [POINTER(ScipyDrmF32)] + single_sel)
+        # the six predict operations per query type (pecos/core/base.py:541-606, :846-976)
+        csr, csc, alloc = POINTER(ScipyCsrF32), POINTER(ScipyCscF32), ScipyCompressedSparseAllocator.CFUNCTYPE
+        for data_type, mat in (("csr", csr), ("drm", POINTER(ScipyDrmF32))):
+            sfx = "_{}_f32".format(data_type)
+            fp(getattr(c, "c_xlinear_predict" + sfx), None, [c_void_p, mat, c_uint32, c_char_p, c_uint32, c_int, alloc])
+            fp(getattr(c, "c_xlinear_predict_on_selected_outputs" + sfx), None, [c_void_p, mat, csr, c_char_p, c_int, alloc])
+            fp(getattr(c, "c_mlmodel_predict" + sfx), None, [c_void_p, mat, csr, c_char_p, c_uint32, c_int, alloc])
+            fp(getattr(c, "c_mlmodel_predict_on_selected_outputs" + sfx), None, [c_void_p, mat, csr, csr, c_char_p, c_int, alloc])
+            fp(getattr(c, "c_xlinear_single_layer_predict" + sfx), None,
+               [mat, csr, csc, csc, c_char_p, c_uint32, c_int, c_float, alloc])
+            fp(getattr(c, "c_xlinear_single_layer_predict_on_selected_outputs" + sfx), None,
+               [mat, csr, csr, csc, csc, c_char_p, c_int, c_float, alloc])
         fp(c.pb200_xlinear_host_from_csc, c_void_p, [POINTER(ScipyCscF32), POINTER(ScipyCscF32), c_float])
         fp(c.pb200_layer_cache_clear, c_uint32, [])
         fp(c.pb200_layer_cache_info, None, [POINTER(c_uint64)])
 
-    def xlinear_single_layer_predict(self, X, csr_codes, W, C, post_processor_str, only_topk, num_threads, bias, pred_alloc):
-        """Same contract as corelib.xlinear_single_layer_predict (pecos/core/base.py:1160-1226): one layer of the python
-        prediction chain.  W / C: csc_matrix (or ScipyCscF32), csr_codes: csr_matrix or None."""
-        self.require_gpu()
-        clib = self.clib_float32
+    @staticmethod
+    def _query(X):
+        """(C view of the query matrix X, "csr" | "drm"): the symbol suffix of the C function that takes it."""
         if isinstance(X, smat.csr_matrix):
             if not X.has_sorted_indices:
                 raise ValueError("Query matrix does not have sorted indices!")
@@ -246,76 +233,48 @@ class B200CoreLib(object):
         elif isinstance(X, np.ndarray):
             X = ScipyDrmF32.init_from(X)
         if isinstance(X, ScipyCsrF32):
-            c_predict = clib.c_xlinear_single_layer_predict_csr_f32
-        elif isinstance(X, ScipyDrmF32):
-            c_predict = clib.c_xlinear_single_layer_predict_drm_f32
-        else:
-            raise NotImplementedError("type(X) = {} not implemented".format(type(X)))
+            return X, "csr"
+        if isinstance(X, ScipyDrmF32):
+            return X, "drm"
+        raise NotImplementedError("type(X) = {} not implemented".format(type(X)))
+
+    @staticmethod
+    def _layer_args(csr_codes, W, C):
+        """The csr_codes (None: a null pointer), W and C arguments of one layer of the python chain."""
         if isinstance(W, smat.csc_matrix):
             W = ScipyCscF32.init_from(W)
         if isinstance(C, smat.csc_matrix):
             C = ScipyCscF32.init_from(C)
         if not isinstance(W, ScipyCscF32) or not isinstance(C, ScipyCscF32):
             raise NotImplementedError("W and C must be csc_matrix / ScipyCscF32")
-        if csr_codes is not None and isinstance(csr_codes, smat.csr_matrix):
+        if isinstance(csr_codes, smat.csr_matrix):
             csr_codes = ScipyCsrF32.init_from(csr_codes)
         if csr_codes is not None and not isinstance(csr_codes, ScipyCsrF32):
             raise NotImplementedError("type(csr_codes) = {} not implemented".format(type(csr_codes)))
-        c_predict(
-            byref(X),
-            byref(csr_codes) if csr_codes is not None else None,
-            byref(W),
-            byref(C),
-            post_processor_str.encode("utf-8"),
-            only_topk,
-            num_threads,
-            bias,
-            pred_alloc.cfunc,
-        )
+        return byref(csr_codes) if csr_codes is not None else None, byref(W), byref(C)
+
+    def xlinear_single_layer_predict(self, X, csr_codes, W, C, post_processor_str, only_topk, num_threads, bias, pred_alloc):
+        """Same contract as corelib.xlinear_single_layer_predict (pecos/core/base.py:1160-1226): one layer of the python
+        prediction chain.  W / C: csc_matrix (or ScipyCscF32), csr_codes: csr_matrix or None."""
+        self.require_gpu()
+        X, data_type = self._query(X)
+        c_predict = getattr(self.clib_float32, "c_xlinear_single_layer_predict_{}_f32".format(data_type))
+        c_predict(byref(X), *self._layer_args(csr_codes, W, C), post_processor_str.encode("utf-8"), only_topk, num_threads,
+                  bias, pred_alloc.cfunc)
 
     def xlinear_single_layer_predict_on_selected_outputs(self, X, selected_outputs_csr, csr_codes, W, C, post_processor_str,
                                                          num_threads, bias, pred_alloc):
         """Same contract as corelib.xlinear_single_layer_predict_on_selected_outputs (pecos/core/base.py:1227-1300): one layer,
         scores of exactly the (instance, label) pairs of ``selected_outputs_csr``."""
         self.require_gpu()
-        clib = self.clib_float32
-        if isinstance(X, smat.csr_matrix):
-            if not X.has_sorted_indices:
-                raise ValueError("Query matrix does not have sorted indices!")
-            X = ScipyCsrF32.init_from(X)
-        elif isinstance(X, np.ndarray):
-            X = ScipyDrmF32.init_from(X)
-        if isinstance(X, ScipyCsrF32):
-            c_predict = clib.c_xlinear_single_layer_predict_on_selected_outputs_csr_f32
-        elif isinstance(X, ScipyDrmF32):
-            c_predict = clib.c_xlinear_single_layer_predict_on_selected_outputs_drm_f32
-        else:
-            raise NotImplementedError("type(X) = {} not implemented".format(type(X)))
+        X, data_type = self._query(X)
         if isinstance(selected_outputs_csr, smat.csr_matrix):
             selected_outputs_csr = ScipyCsrF32.init_from(selected_outputs_csr.astype(np.float32))
         if not isinstance(selected_outputs_csr, ScipyCsrF32):
             raise NotImplementedError("selected_outputs_csr must be a csr_matrix / ScipyCsrF32")
-        if isinstance(W, smat.csc_matrix):
-            W = ScipyCscF32.init_from(W)
-        if isinstance(C, smat.csc_matrix):
-            C = ScipyCscF32.init_from(C)
-        if not isinstance(W, ScipyCscF32) or not isinstance(C, ScipyCscF32):
-            raise NotImplementedError("W and C must be csc_matrix / ScipyCscF32")
-        if csr_codes is not None and isinstance(csr_codes, smat.csr_matrix):
-            csr_codes = ScipyCsrF32.init_from(csr_codes)
-        if csr_codes is not None and not isinstance(csr_codes, ScipyCsrF32):
-            raise NotImplementedError("type(csr_codes) = {} not implemented".format(type(csr_codes)))
-        c_predict(
-            byref(X),
-            byref(selected_outputs_csr),
-            byref(csr_codes) if csr_codes is not None else None,
-            byref(W),
-            byref(C),
-            post_processor_str.encode("utf-8"),
-            num_threads,
-            bias,
-            pred_alloc.cfunc,
-        )
+        c_predict = getattr(self.clib_float32, "c_xlinear_single_layer_predict_on_selected_outputs_{}_f32".format(data_type))
+        c_predict(byref(X), byref(selected_outputs_csr), *self._layer_args(csr_codes, W, C), post_processor_str.encode("utf-8"),
+                  num_threads, bias, pred_alloc.cfunc)
 
     def require_gpu(self):
         if self.clib_float32.pb200_device_count() <= 0:
@@ -343,19 +302,8 @@ class B200CoreLib(object):
     def xlinear_predict(self, c_model, X, overriden_beam_size, overriden_post_processor_str, overriden_only_topk,
                         threads, pred_alloc):
         """Same contract as corelib.xlinear_predict (base.py:1041-1095)."""
-        clib = self.clib_float32
-        if isinstance(X, smat.csr_matrix):
-            if not X.has_sorted_indices:
-                raise ValueError("Query matrix does not have sorted indices!")
-            X = ScipyCsrF32.init_from(X)
-        elif isinstance(X, np.ndarray):
-            X = ScipyDrmF32.init_from(X)
-        if isinstance(X, ScipyCsrF32):
-            c_predict = clib.c_xlinear_predict_csr_f32
-        elif isinstance(X, ScipyDrmF32):
-            c_predict = clib.c_xlinear_predict_drm_f32
-        else:
-            raise NotImplementedError("type(X) = {} not implemented".format(type(X)))
+        X, data_type = self._query(X)
+        c_predict = getattr(self.clib_float32, "c_xlinear_predict_{}_f32".format(data_type))
         c_predict(
             c_model,
             byref(X),
@@ -366,25 +314,13 @@ class B200CoreLib(object):
             pred_alloc.cfunc,
         )
 
-    # ---------------------------------------------------------------- HNSW (base.py:1865-1964)
     def xlinear_predict_on_selected_outputs(self, c_model, X, selected_outputs_csr, overriden_post_processor_str, threads, pred_alloc):
         """Argument handling of corelib.xlinear_predict_on_selected_outputs (pecos/core/base.py:1097-1160)."""
-        clib = self.clib_float32
-        if isinstance(X, smat.csr_matrix):
-            if not X.has_sorted_indices:
-                raise ValueError("Query matrix does not have sorted indices!")
-            X = ScipyCsrF32.init_from(X)
-        elif isinstance(X, np.ndarray):
-            X = ScipyDrmF32.init_from(X)
+        X, data_type = self._query(X)
         if not isinstance(selected_outputs_csr, smat.csr_matrix):
             raise ValueError("type(selected_outputs_csr) = {} not implemented".format(type(selected_outputs_csr)))
         selected = ScipyCsrF32.init_from(selected_outputs_csr)
-        if isinstance(X, ScipyCsrF32):
-            c_predict = clib.c_xlinear_predict_on_selected_outputs_csr_f32
-        elif isinstance(X, ScipyDrmF32):
-            c_predict = clib.c_xlinear_predict_on_selected_outputs_drm_f32
-        else:
-            raise NotImplementedError("type(X) = {} not implemented".format(type(X)))
+        c_predict = getattr(self.clib_float32, "c_xlinear_predict_on_selected_outputs_{}_f32".format(data_type))
         c_predict(
             c_model,
             byref(X),
@@ -394,6 +330,7 @@ class B200CoreLib(object):
             pred_alloc.cfunc,
         )
 
+    # ---------------------------------------------------------------- HNSW (base.py:1865-1964)
     def link_ann_hnsw_methods(self):
         c = self.clib_float32
         fp = B200CoreLib.fillprototype

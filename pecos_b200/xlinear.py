@@ -284,10 +284,8 @@ class HierarchicalMLModel(object):
     def get_pred_params(self):
         return copy.deepcopy(self.pred_params)
 
-    def predict(self, X, csr_codes=None, pred_params=None, **kwargs):
-        assert X.dtype == np.float32
-        assert isinstance(X, smat.csr_matrix) or (isinstance(X, np.ndarray) and X.flags["C_CONTIGUOUS"])
-        assert X.shape[1] == self.nr_features
+    def _pred_chains(self, pred_params, kwargs):
+        """(stored, requested) per-layer MLModelPredParams of a predict call."""
         if pred_params is None:
             pred_params = self.get_pred_params()
         elif isinstance(pred_params, self.PredParams):
@@ -297,18 +295,27 @@ class HierarchicalMLModel(object):
         else:
             raise ValueError("unknown type(pred_params)!!")
         pred_params.override_with_kwargs(kwargs)
+        return self.get_pred_params().model_chain, pred_params.model_chain
+
+    @staticmethod
+    def _overridden_post_processor(old_chain, new_chain):
+        """None if no layer's post_processor changed, else the one all layers now share (pecos/xmc/base.py:1630-1641)."""
+        if all(o.post_processor == n.post_processor for (o, n) in zip(old_chain, new_chain)):
+            return None
+        if all(new_chain[0].post_processor == n.post_processor for n in new_chain):
+            return new_chain[0].post_processor
+        raise NotImplementedError("when is_predict_only=True, post_processor is not supported for overriddng")
+
+    def predict(self, X, csr_codes=None, pred_params=None, **kwargs):
+        assert X.dtype == np.float32
+        assert isinstance(X, smat.csr_matrix) or (isinstance(X, np.ndarray) and X.flags["C_CONTIGUOUS"])
+        assert X.shape[1] == self.nr_features
+        old_chain, new_chain = self._pred_chains(pred_params, kwargs)
         if csr_codes is not None:
             raise NotImplementedError("is_predict_only=True did not support csr_codes being not None")
 
-        old_chain = self.get_pred_params().model_chain
-        new_chain = pred_params.model_chain
         # identical gating to pecos/xmc/base.py:1627-1654
-        if all(o.post_processor == n.post_processor for (o, n) in zip(old_chain, new_chain)):
-            overridden_post_processor = None
-        elif all(new_chain[0].post_processor == n.post_processor for n in new_chain):
-            overridden_post_processor = new_chain[0].post_processor
-        else:
-            raise NotImplementedError("when is_predict_only=True, post_processor is not supported for overriddng")
+        overridden_post_processor = self._overridden_post_processor(old_chain, new_chain)
         if all(o.only_topk == n.only_topk for (o, n) in zip(old_chain[:-1], new_chain[:-1])):
             overridden_beam_size = None
         elif all(new_chain[0].only_topk == n.only_topk for n in new_chain[:-1]):
@@ -348,23 +355,7 @@ class HierarchicalMLModel(object):
             raise ValueError("Instance dimension of query and selected output matrix do not match")
         if csr_codes is not None:
             raise NotImplementedError("is_predict_only=True did not support csr_codes being not None")
-        if pred_params is None:
-            pred_params = self.get_pred_params()
-        elif isinstance(pred_params, self.PredParams):
-            pred_params = copy.deepcopy(pred_params)
-            if len(pred_params.model_chain) != self.depth:
-                raise ValueError("len(pred_params.model_chain) != depth")
-        else:
-            raise ValueError("unknown type(pred_params)!!")
-        pred_params.override_with_kwargs(kwargs)
-        old_chain = self.get_pred_params().model_chain
-        new_chain = pred_params.model_chain
-        if all(o.post_processor == n.post_processor for (o, n) in zip(old_chain, new_chain)):
-            overridden_post_processor = None
-        elif all(new_chain[0].post_processor == n.post_processor for n in new_chain):
-            overridden_post_processor = new_chain[0].post_processor
-        else:
-            raise NotImplementedError("when is_predict_only=True, post_processor is not supported for overriddng")
+        overridden_post_processor = self._overridden_post_processor(*self._pred_chains(pred_params, kwargs))
         pred_alloc = ScipyCompressedSparseAllocator()
         self._clib.xlinear_predict_on_selected_outputs(
             self.model_chain, X, selected_outputs_csr, overridden_post_processor, kwargs.get("threads", -1), pred_alloc
