@@ -279,36 +279,83 @@ xl_cm_build_images_kernel(const LayerDev L, const CmShape S, unsigned char* __re
     }
 }
 
-// one warp per query: candidate position of every beam slot (prefix of the chunk widths) and pairs per chunk
-__global__ void __launch_bounds__(128)
-xl_cm_count_kernel(const LayerDev L, const QueryDev X, const uint32_t* __restrict__ beam_id,
-                   const uint32_t* __restrict__ beam_cnt, const uint32_t beam_stride, const uint32_t rows, CmWork w,
-                   const uint32_t* __restrict__ vc_ptr) {
-    const int lane = threadIdx.x & 31;
-    const uint32_t q = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    if (q >= rows) return;
-    const uint32_t cnt = beam_cnt[q];
-    uint32_t run = 0;
-    for (uint32_t j0 = 0; j0 < cnt; j0 += 32) {
-        const uint32_t j = j0 + lane;
-        uint32_t width = 0, p = 0;
-        bool scored = false;
-        if (j < cnt) {
-            p = beam_id[static_cast<uint64_t>(q) * beam_stride + j];
-            const uint4 h = *reinterpret_cast<const uint4*>(&L.chunks[p]);  // {col_begin, n_cols, nnz_rows, has_bias}
-            width = h.y;
-            scored = !(h.w & kChunkAbsent) && h.y > 0;
-        }
-        const uint32_t incl = warp_incl_scan(width, lane);
-        if (j < cnt) {
-            w.slot_pos[static_cast<uint64_t>(q) * beam_stride + j] = run + incl - width;
-            if (scored) {  // one pair per non-empty column range of the chunk
-                const uint32_t v0 = vc_ptr[p], nr = vc_ptr[p + 1] - v0;
-                const uint32_t cw = (width + nr - 1u) / max(nr, 1u);
-                for (uint32_t hh = 0; hh < nr && hh * cw < width; ++hh) atomicAdd(&w.count[v0 + hh], 1u);
+// Bucketing (count -> scan -> scatter).  Every pair of a layer lands in its virtual chunk's bucket, and tens of thousands
+// of pairs land on a few dozen chunks (eurlex-4k leaf: 154,490 pairs on 64; a layer-0 of one chunk: every query's pair on
+// one).  Atomics on one counter serialise in the L2, so the pairs are counted per CTA in a shared-memory histogram and
+// each CTA adds a non-empty bin to the global counter once.  A CTA walks a contiguous block of queries, one warp per query.
+// The histogram covers kCmBinWindow virtual chunks at a time; a layer with more makes one pass over the CTA's queries per
+// window, so shared memory stays bounded for any layer and any beam width.
+constexpr uint32_t kCmBinWindow = 8192;     // virtual chunks one bucketing pass histograms (32 KB of shared memory)
+constexpr int kCmBucketThreads = 1024;
+constexpr uint32_t kCmBucketCtasPerSm = 2;  // 64 warps per SM; one CTA per SM took 2.4 us longer on the eurlex-4k leaf
+
+// a CTA adds each of its bins once: few CTAs, few atomics on the same counter; at least one query per warp
+inline uint32_t cm_bucket_grid(uint32_t rows, uint32_t n_sm) {
+    return std::max(1u, std::min(kCmBucketCtasPerSm * n_sm, (rows + kCmBucketThreads / 32 - 1) / (kCmBucketThreads / 32)));
+}
+
+// the virtual chunks [lo, hi) of a beam slot on chunk p that fall into the bin window [b0, b0 + nb): one per non-empty
+// column range of a scored chunk (cw columns each, range v - v0 starts at column (v - v0) x cw); none for an absent or
+// empty chunk
+struct CmSlotRanges { uint32_t v0, lo, hi, cw; };
+__device__ __forceinline__ CmSlotRanges cm_slot_ranges(const uint4 h, const uint32_t* __restrict__ vc_ptr, uint32_t p,
+                                                       uint32_t b0, uint32_t nb) {
+    CmSlotRanges s{0, 0, 0, 0};
+    if ((h.w & kChunkAbsent) || h.y == 0) return s;
+    const uint32_t v0 = vc_ptr[p], nr = vc_ptr[p + 1] - v0;
+    if (nr == 0) return s;
+    s.v0 = v0;
+    s.cw = (h.y + nr - 1u) / nr;
+    const uint32_t n = min(nr, (h.y + s.cw - 1u) / s.cw);
+    s.lo = max(v0, b0);
+    s.hi = max(s.lo, min(v0 + n, b0 + nb));
+    return s;
+}
+
+// queries [q_begin, q_end) of this CTA
+__device__ __forceinline__ uint2 cm_bucket_block(uint32_t rows) {
+    const uint32_t per = (rows + gridDim.x - 1) / gridDim.x;
+    const uint32_t b = min(rows, blockIdx.x * per);
+    return make_uint2(b, min(rows, b + per));
+}
+
+// candidate position of every beam slot (prefix of the chunk widths; first window) and pairs per virtual chunk
+__global__ void __launch_bounds__(kCmBucketThreads, kCmBucketCtasPerSm)
+xl_cm_count_kernel(const LayerDev L, const uint32_t* __restrict__ beam_id, const uint32_t* __restrict__ beam_cnt,
+                   const uint32_t beam_stride, const uint32_t rows, CmWork w, const uint32_t* __restrict__ vc_ptr,
+                   const uint32_t n_vc) {
+    __shared__ uint32_t bins[kCmBinWindow];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, warps = blockDim.x >> 5;
+    const uint2 blk = cm_bucket_block(rows);
+    for (uint32_t b0 = 0; b0 < n_vc; b0 += kCmBinWindow) {
+        const uint32_t nb = min(kCmBinWindow, n_vc - b0);
+        for (uint32_t i = threadIdx.x; i < nb; i += blockDim.x) bins[i] = 0u;
+        __syncthreads();
+        for (uint32_t q = blk.x + warp; q < blk.y; q += warps) {
+            const uint32_t cnt = beam_cnt[q];
+            uint32_t run = 0;
+            for (uint32_t j0 = 0; j0 < cnt; j0 += 32) {
+                const uint32_t j = j0 + lane;
+                uint4 h = make_uint4(0, 0, 0, kChunkAbsent);  // {col_begin, n_cols, nnz_rows, has_bias}
+                uint32_t p = 0;
+                if (j < cnt) {
+                    p = beam_id[static_cast<uint64_t>(q) * beam_stride + j];
+                    h = *reinterpret_cast<const uint4*>(&L.chunks[p]);
+                }
+                if (b0 == 0) {
+                    const uint32_t width = (j < cnt) ? h.y : 0u;
+                    const uint32_t incl = warp_incl_scan(width, lane);
+                    if (j < cnt) w.slot_pos[static_cast<uint64_t>(q) * beam_stride + j] = run + incl - width;
+                    run += __shfl_sync(kFull, incl, 31);
+                }
+                const CmSlotRanges s = cm_slot_ranges(h, vc_ptr, p, b0, nb);
+                for (uint32_t v = s.lo; v < s.hi; ++v) atomicAdd(&bins[v - b0], 1u);
             }
         }
-        run += __shfl_sync(kFull, incl, 31);
+        __syncthreads();
+        for (uint32_t i = threadIdx.x; i < nb; i += blockDim.x)
+            if (bins[i]) atomicAdd(&w.count[b0 + i], bins[i]);
+        __syncthreads();
     }
 }
 
@@ -374,27 +421,48 @@ xl_cm_scan_kernel(const uint32_t n_chunks, CmWork w, const unsigned char* __rest
     if (threadIdx.x == 0) { w.bucket_ptr[n_chunks] = carry_pairs; w.cost_ptr[n_chunks] = carry_cost; }
 }
 
-// one warp per query: append (query, position) to the pair list of every scored slot's chunk (order inside a bucket is
-// irrelevant: a pair's result location is fixed by its query and position)
-__global__ void __launch_bounds__(128)
+// appends (query, candidate position) to the bucket of every virtual chunk a beam slot is scored on.  Per bin window a
+// CTA counts its pairs per virtual chunk, reserves one contiguous run of each non-empty bucket (one atomic on its cursor),
+// and places each pair at the run's next free place, counted by a shared-memory atomic; the bins hold the counts, then the
+// CTA's cursors, so shared memory stays at one window at any beam width.  The order inside a bucket is free: a pair's
+// result location is fixed by its query and position.
+__global__ void __launch_bounds__(kCmBucketThreads, kCmBucketCtasPerSm)
 xl_cm_scatter_kernel(const LayerDev L, const uint32_t* __restrict__ beam_id, const uint32_t* __restrict__ beam_cnt,
-                     const uint32_t beam_stride, const uint32_t rows, CmWork w, const uint32_t* __restrict__ vc_ptr) {
-    const int lane = threadIdx.x & 31;
-    const uint32_t q = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-    if (q >= rows) return;
-    const uint32_t cnt = beam_cnt[q];
-    for (uint32_t j = lane; j < cnt; j += 32) {
-        const uint32_t p = beam_id[static_cast<uint64_t>(q) * beam_stride + j];
-        const uint4 h = *reinterpret_cast<const uint4*>(&L.chunks[p]);
-        if ((h.w & kChunkAbsent) || h.y == 0) continue;
-        const uint32_t pos = w.slot_pos[static_cast<uint64_t>(q) * beam_stride + j];
-        const uint32_t v0 = vc_ptr[p], nr = vc_ptr[p + 1] - v0;
-        const uint32_t cw = (h.y + nr - 1u) / max(nr, 1u);
-        for (uint32_t hh = 0; hh < nr && hh * cw < h.y; ++hh) {
-            const uint32_t at = atomicAdd(&w.count[v0 + hh], 1u);
-            w.pair_q[at] = q;
-            w.pair_pos[at] = pos + hh * cw;  // first candidate of this column range
-        }
+                     const uint32_t beam_stride, const uint32_t rows, CmWork w, const uint32_t* __restrict__ vc_ptr,
+                     const uint32_t n_vc) {
+    __shared__ uint32_t bins[kCmBinWindow];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, warps = blockDim.x >> 5;
+    const uint2 blk = cm_bucket_block(rows);
+    for (uint32_t b0 = 0; b0 < n_vc; b0 += kCmBinWindow) {
+        const uint32_t nb = min(kCmBinWindow, n_vc - b0);
+        auto each_pair = [&](auto visit) {
+            for (uint32_t q = blk.x + warp; q < blk.y; q += warps) {
+                const uint32_t cnt = beam_cnt[q];
+                for (uint32_t j = lane; j < cnt; j += 32) {
+                    const uint32_t p = beam_id[static_cast<uint64_t>(q) * beam_stride + j];
+                    const CmSlotRanges s = cm_slot_ranges(*reinterpret_cast<const uint4*>(&L.chunks[p]), vc_ptr, p, b0, nb);
+                    if (s.lo < s.hi) visit(q, j, s);
+                }
+            }
+        };
+        for (uint32_t i = threadIdx.x; i < nb; i += blockDim.x) bins[i] = 0u;
+        __syncthreads();
+        each_pair([&](uint32_t, uint32_t, const CmSlotRanges& s) {
+            for (uint32_t v = s.lo; v < s.hi; ++v) atomicAdd(&bins[v - b0], 1u);
+        });
+        __syncthreads();
+        for (uint32_t i = threadIdx.x; i < nb; i += blockDim.x)
+            if (bins[i]) bins[i] = atomicAdd(&w.count[b0 + i], bins[i]);
+        __syncthreads();
+        each_pair([&](uint32_t q, uint32_t j, const CmSlotRanges& s) {
+            const uint32_t pos = w.slot_pos[static_cast<uint64_t>(q) * beam_stride + j];
+            for (uint32_t v = s.lo; v < s.hi; ++v) {
+                const uint32_t at = atomicAdd(&bins[v - b0], 1u);
+                w.pair_q[at] = q;
+                w.pair_pos[at] = pos + (v - s.v0) * s.cw;  // first candidate of this column range
+            }
+        });
+        __syncthreads();
     }
 }
 

@@ -1260,10 +1260,10 @@ int XLinearEngine::score_layer_(size_t d, const QueryDev& q, uint32_t b_prev, in
         CmWork w{cm_slot_pos_.get(), cm_count_.get(), cm_bucket_ptr_.get(), cm_cost_ptr_.get(), cm_pair_q_.get(), cm_pair_pos_.get(),
                  cm_claim_.get(), cm_active_.get()};
         PB200_CUDA(cudaMemsetAsync(w.count, 0, (static_cast<uint64_t>(n_vc) + 1) * 4, stream_));
-        const uint32_t warp_grid = (rows * 32u + 127u) / 128u;
-        xl_cm_count_kernel<<<warp_grid, 128, 0, stream_>>>(L, q, bid, bcnt, beam_stride_, rows, w, shape.vc_ptr);
+        const uint32_t bucket_grid = cm_bucket_grid(rows, n_sm_);
+        xl_cm_count_kernel<<<bucket_grid, kCmBucketThreads, 0, stream_>>>(L, bid, bcnt, beam_stride_, rows, w, shape.vc_ptr, n_vc);
         xl_cm_scan_kernel<<<1, 1024, 0, stream_>>>(n_vc, w, layers_[d].cm_images.get(), shape.img_bytes, L.w_rows);
-        xl_cm_scatter_kernel<<<warp_grid, 128, 0, stream_>>>(L, bid, bcnt, beam_stride_, rows, w, shape.vc_ptr);
+        xl_cm_scatter_kernel<<<bucket_grid, kCmBucketThreads, 0, stream_>>>(L, bid, bcnt, beam_stride_, rows, w, shape.vc_ptr, n_vc);
         auto launch_cm = [&](auto kernel) {
             kernel<<<cm.grid, cm.warps * 32, cm.smem, stream_>>>(L, q, w, shape, layers_[d].cm_images.get(), cand, cand_stride_q,
                                                                  CmPrefixOut{});
