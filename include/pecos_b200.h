@@ -312,8 +312,9 @@ void pb200_hnsw_set_foreign(int metric, void* destruct, void* searchers_create, 
  * serialised, tokens of one model may run concurrently.
  * predict: pair b uses query row (is_same_input ? 0 : b) and column label_keys[b]; slot k < min(only_topk, column length)
  * of row b of ret_* (batch_size x only_topk) receives {row id, distance, Y value, 1} in the reference's order, ties
- * included; every other slot is left as the caller had it.  A label key >= the model's number of labels is a fatal error
- * before any GPU work. */
+ * included; every other slot is left as the caller had it.  A label key >= the model's number of labels, or a dense model
+ * wider than pb200_pairwise_ann_dense_fits allows, is a fatal error before any GPU work.  NaN distances (a NaN component, or
+ * products that overflow to both +inf and -inf) are placed where the reference's heap sequence puts them. */
 void* c_pairwise_ann_train_drm_ip_f32(const ScipyDrmF32* pX, const ScipyCscF32* pY);
 void* c_pairwise_ann_train_csr_ip_f32(const ScipyCsrF32* pX, const ScipyCscF32* pY);
 void* c_pairwise_ann_load_drm_ip_f32(const char* model_dir, const bool lazy_load);
@@ -337,6 +338,17 @@ void c_pairwise_ann_predict_csr_ip_f32(void* searchers_ptr, uint32_t batch_size,
 void pb200_pairwise_ann_get_counters(void* searchers_ptr, uint64_t* out);
 /* device time (CUDA events) of the distance and select kernels of the token's last predict call, in ms */
 double pb200_pairwise_ann_kernel_ms(void* searchers_ptr);
+/* the token's last predict call: out[4] = {bulk-copy ring depth of the distance kernel (4, or 0 = direct loads), warps per
+ * CTA, shared-memory bytes per warp, tiles (consecutive pairs whose columns hold at most 2^25 entries together, or one longer
+ * column)}; all 0 when the call had nothing to search (batch_size or only_topk 0) */
+void pb200_pairwise_ann_launch_info(void* searchers_ptr, uint64_t* out);
+/* Width limit of dense models, host-only.  A warp of the distance kernel stages the query row (dense_vstride(d) floats: d
+ * rounded up to 64 when d % 16 == 0, else the 16-multiple part rounded up to 64 plus 16) and the distances of 128 rows in
+ * 200 KB of shared memory, with a ring of 4 more rows where that fits (d <= 10,191).  Every d up to 51,024 and every multiple
+ * of 16 up to 51,072 fits; nothing else does, and predict on such a model is a fatal error, so callers check first (the Python
+ * layer raises ValueError).  Training, saving and loading a wider model are allowed.  Returns 1 if a model of width feat_dim
+ * can be searched, else 0, and out[3] = {ring depth (4 or 0), per-warp bytes at that depth, row stride in floats}. */
+int pb200_pairwise_ann_dense_fits(uint32_t feat_dim, uint32_t* out);
 /* Host-only ingest check of a PairwiseANN folder (<model>/c_model), no GPU needed: pairwise_ann_t of the data type (sparse 0 =
  * drm, 1 = csr), version, block sizes, offsets, row ids of Y within X.  Returns 0 and out[6] = {num_input_keys, num_label_keys,
  * feat_dim, nnz of Y, nnz of X, longest column}, or 1 (reason on stderr). */

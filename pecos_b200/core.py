@@ -406,6 +406,29 @@ class B200CoreLib(object):
         self.clib_float32.pb200_pairwise_ann_get_counters(searchers_ptr, out)
         return dict(zip(("pairs", "distances", "sparse_entries", "replays"), [int(v) for v in out]))
 
+    def pairwise_ann_launch_info(self, searchers_ptr):
+        """{stages, warps, per_warp_bytes, tiles} of the searcher token's last predict call (ring depth of the distance kernel,
+        warps per CTA, shared-memory bytes per warp, tiles of at most 2^25 column entries)."""
+        out = (c_uint64 * 4)()
+        self.clib_float32.pb200_pairwise_ann_launch_info(searchers_ptr, out)
+        return dict(zip(("stages", "warps", "per_warp_bytes", "tiles"), [int(v) for v in out]))
+
+    def pairwise_ann_dense_fits(self, feat_dim):
+        """(fits, {stages, per_warp_bytes, vstride}) of a dense PairwiseANN model of width feat_dim.  Host-only."""
+        out = (c_uint32 * 3)()
+        fits = self.clib_float32.pb200_pairwise_ann_dense_fits(int(feat_dim), out)
+        return bool(fits), dict(zip(("stages", "per_warp_bytes", "vstride"), [int(v) for v in out]))
+
+    def pairwise_ann_check_dense(self, feat_dim):
+        """Raises ValueError unless a dense PairwiseANN model of width feat_dim can be searched.  Host-only, so it runs before
+        any native call that would search."""
+        fits, plan = self.pairwise_ann_dense_fits(feat_dim)
+        if not fits:
+            raise ValueError(
+                f"pecos_b200: a dense PairwiseANN model of feat_dim={feat_dim} cannot be searched: one warp stages the query "
+                f"row ({plan['vstride']} floats after padding) and 128 distances in at most 204,800 bytes of shared memory, "
+                f"which holds every feat_dim up to 51,024 and every multiple of 16 up to 51,072")
+
     def pairwise_ann_host_info(self, c_model_dir, data_type):
         """Host-only ingest check of a <model>/c_model folder; returns its sizes, raises ValueError if it does not load."""
         out = (c_uint64 * 6)()
@@ -463,6 +486,8 @@ class B200CoreLib(object):
         fp(c.pb200_hnsw_host_info, c_int, [c_char_p, c_int, c_int, POINTER(c_uint64)])
         fp(c.pb200_pairwise_ann_get_counters, None, [c_void_p, POINTER(c_uint64)])
         fp(c.pb200_pairwise_ann_kernel_ms, c_double, [c_void_p])
+        fp(c.pb200_pairwise_ann_launch_info, None, [c_void_p, POINTER(c_uint64)])
+        fp(c.pb200_pairwise_ann_dense_fits, c_int, [c_uint32, POINTER(c_uint32)])
         fp(c.pb200_pairwise_ann_host_info, c_int, [c_char_p, c_int, POINTER(c_uint64)])
         fp(c.pb200_sparse_block_distances, None, [c_int, c_int, c_void_p, c_void_p, c_void_p, c_uint32, c_void_p, c_void_p,
                                                   c_uint32, c_uint32, c_void_p, c_void_p, c_void_p])

@@ -1240,6 +1240,21 @@ double pb200_pairwise_ann_kernel_ms(void* searchers_ptr) {
     PB200_API_END("pb200_pairwise_ann_kernel_ms")
 }
 
+void pb200_pairwise_ann_launch_info(void* searchers_ptr, uint64_t* out) {
+    PB200_API_BEGIN
+    auto& t = pairwise_searchers_of(searchers_ptr);
+    std::lock_guard<std::mutex> lock(t.mu);
+    t.searcher->launch_info(out);
+    PB200_API_END("pb200_pairwise_ann_launch_info")
+}
+
+int pb200_pairwise_ann_dense_fits(uint32_t feat_dim, uint32_t* out) {
+    const uint32_t vstride = pb200::dense_vstride(feat_dim);
+    const pb200::PairwisePlan plan = pb200::pairwise_plan(false, vstride, 0);
+    if (out) { out[0] = static_cast<uint32_t>(plan.stages); out[1] = plan.per_warp; out[2] = vstride; }
+    return plan.fits ? 1 : 0;
+}
+
 int pb200_pairwise_ann_host_info(const char* model_dir, int sparse, uint64_t* out) {
     try {
         auto m = pb200::load_pairwise_model(model_dir, sparse != 0, false);

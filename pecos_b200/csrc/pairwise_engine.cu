@@ -6,8 +6,9 @@
 //      once per warp), evaluates the slice's distances with the HNSW distance code (batch_distances / batch_distances_sparse,
 //      the same bits as the reference's ip distances) and writes {distance bits, position} into the pair's scratch region.
 //   2. pw_select_kernel: one warp per pair, k = min(topk, n).  A radix select finds the k-th smallest distance T.  When
-//      exactly one entry equals T and the k smallest are pairwise distinct, every heap sequence ends in the same sorted
-//      list, so the k smallest sorted ascending ARE the reference's answer (fast path).  Otherwise one lane replays the
+//      the column holds no NaN distance, exactly one entry equals T and the k smallest are pairwise distinct, every heap
+//      sequence ends in the same sorted list, so the k smallest sorted ascending ARE the reference's answer (fast path; with
+//      a NaN, `<` is no strict weak order and the heap leaves it wherever the sequence puts it).  Otherwise one lane replays the
 //      reference's push-all / pop-to-k / sort_heap over the column in stored order with the restated libstdc++ heap
 //      algorithms (in shared memory when the column fits, in place in the pair's global scratch otherwise), which settles
 //      every tie exactly as the CPU code does.
@@ -131,14 +132,17 @@ pw_select_kernel(const uint4* __restrict__ pairs, const unsigned long long* __re
         const uint32_t k = min(topk, n);
         uint2* e = scratch + pair_off[p];
 
-        // ---- radix select of the k-th smallest key T, 8 bits per pass
+        // ---- radix select of the k-th smallest key T, 8 bits per pass; the first pass also looks for NaN distances
         uint32_t prefix = 0, rank = k, eq = 0;
+        bool nan = false;
         for (int shift = 24; shift >= 0; shift -= 8) {
             for (int b = lane; b < 256; b += 32) hist[b] = 0u;
             __syncwarp();
             const uint32_t hmask = (shift == 24) ? 0u : (0xFFFFFFFFu << (shift + 8));
             for (uint32_t i = lane; i < n; i += 32) {
-                const uint32_t key = dist_key(e[i].x);
+                const uint32_t bits = e[i].x;
+                if (shift == 24) nan |= (bits << 1) > 0xFF000000u;  // isnan, whatever the sign and payload
+                const uint32_t key = dist_key(bits);
                 if ((key & hmask) == prefix) atomicAdd(&hist[(key >> shift) & 255u], 1u);
             }
             __syncwarp();
@@ -170,8 +174,8 @@ pw_select_kernel(const uint4* __restrict__ pairs, const unsigned long long* __re
         }
         const uint32_t T = prefix;
 
-        // ---- fast path: the k entries with key <= T, sorted by (key, position), all keys distinct
-        bool fast = (eq == 1u) && (k <= kSelCap);
+        // ---- fast path: no NaN in the column, the k entries with key <= T sorted by (key, position), all keys distinct
+        bool fast = (eq == 1u) && (k <= kSelCap) && !__any_sync(kFull, nan);
         if (fast) {
             uint32_t got = 0;
             for (uint32_t b0 = 0; b0 < n; b0 += 32) {
@@ -250,6 +254,13 @@ pw_select_kernel(const uint4* __restrict__ pairs, const unsigned long long* __re
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------------------------
+PairwisePlan pairwise_plan(bool sparse, uint32_t vstride, uint32_t qcap) {
+    auto per_warp_bytes = [&](int stages) { return warp_smem_bytes(sparse, vstride, stages, qcap, kSlice * 4u); };
+    const int stages = (!sparse && vstride > 0 && per_warp_bytes(4) <= kWarpSmemMax) ? 4 : 0;
+    const uint32_t per_warp = per_warp_bytes(stages);
+    return PairwisePlan{per_warp <= kWarpSmemMax, stages, per_warp};
+}
+
 const HnswDev& PairwiseModel::device_view(int device) {
     std::lock_guard<std::mutex> lock(mu_);
     if (uploaded_) {
@@ -310,6 +321,7 @@ void PairwiseSearcher::predict(uint32_t batch, uint32_t topk, const HostMatrix& 
     const PairwiseHostModel& H = model_->host();
     counters_ = PairwiseCounters{};
     last_ms_ = 0.0;
+    std::fill(last_launch_, last_launch_ + 4, 0ull);
     if (batch == 0 || topk == 0) return;  // the reference writes nothing
     // every check before any GPU work: a bad label key would read out of bounds in the reference
     for (uint32_t b = 0; b < batch; ++b)
@@ -320,6 +332,9 @@ void PairwiseSearcher::predict(uint32_t batch, uint32_t topk, const HostMatrix& 
     if (q.rows < need_rows) throw std::runtime_error("pecos_b200: PairwiseANN query matrix has fewer rows than the batch needs");
     if (q.cols != H.feat_dim) throw std::runtime_error("pecos_b200: PairwiseANN query dimension != feat_dim");
     if ((q.row_ptr != nullptr) != H.sparse) throw std::runtime_error("pecos_b200: PairwiseANN query type differs from the model's");
+    if (!H.sparse && !pairwise_plan(false, dense_vstride(H.feat_dim), 0).fits)
+        throw std::runtime_error("pecos_b200: PairwiseANN feat_dim " + std::to_string(H.feat_dim) + " too large for the shared-memory "
+                                 "staging area (dense models serve every d up to 51,024 and multiples of 16 up to 51,072)");
 
     PB200_CUDA(cudaSetDevice(device_));
     const HnswDev ix = model_->device_view(device_);
@@ -334,13 +349,11 @@ void PairwiseSearcher::predict(uint32_t batch, uint32_t topk, const HostMatrix& 
     out_V_.upload(ret_V, n_out, stream_);
     PB200_CUDA(cudaMemsetAsync(ctrl_.get(), 0, 4 * sizeof(unsigned long long), stream_));
 
-    // launch geometry of the distance kernel: [staged query | distances of a slice] per warp; dense rows through a ring of 4
-    // where it fits, else direct loads
-    auto per_warp_bytes = [&](int stages) { return warp_smem_bytes(H.sparse, ix.vstride, stages, sq.qcap, kSlice * 4u); };
-    const int stages = (!H.sparse && ix.vstride > 0 && per_warp_bytes(4) <= kWarpSmemMax) ? 4 : 0;
-    const uint32_t per_warp = per_warp_bytes(stages);
-    if (per_warp > kWarpSmemMax)
-        throw std::runtime_error("pecos_b200: PairwiseANN feat_dim too large for the shared-memory staging area (about 50,000 at most)");
+    // launch geometry of the distance kernel (pairwise_plan): dense rows through a ring of 4 where it fits, else direct loads
+    const PairwisePlan plan = pairwise_plan(H.sparse, ix.vstride, sq.qcap);
+    if (!plan.fits) throw std::runtime_error("pecos_b200: PairwiseANN query too large for the shared-memory staging area");
+    const int stages = plan.stages;
+    const uint32_t per_warp = plan.per_warp;
     const CtaShape shape = cta_shape(device_, per_warp, 64u);
     const uint32_t warps = shape.warps, sms = shape.sms, ctas_per_sm = shape.ctas_per_sm;
     const uint32_t cta_smem = warps * per_warp;
@@ -369,6 +382,7 @@ void PairwiseSearcher::predict(uint32_t batch, uint32_t topk, const HostMatrix& 
         }
         const uint32_t np = p1 - p0;
         counters_.n_dist += total;
+        ++last_launch_[3];
         if (total) {
             pairs_.upload(pairs.data(), np, stream_);
             pair_off_.upload(offs.data(), np, stream_);
@@ -405,6 +419,11 @@ void PairwiseSearcher::predict(uint32_t batch, uint32_t topk, const HostMatrix& 
     counters_.n_entries = h[1];
     counters_.replays = h[2];
     last_ms_ = total_ms;
+    last_launch_[0] = static_cast<uint64_t>(stages);
+    last_launch_[1] = warps;
+    last_launch_[2] = per_warp;
 }
+
+void PairwiseSearcher::launch_info(uint64_t* out) const { std::copy(last_launch_, last_launch_ + 4, out); }
 
 }  // namespace pb200

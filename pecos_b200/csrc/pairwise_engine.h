@@ -43,6 +43,17 @@ private:
     DeviceBuffer<float> y_val_;
 };
 
+// The distance kernel's per-warp shared-memory slice: [staged query | ring rows | distances of a 128-row slice].  Dense rows
+// go through a bulk-copy ring of 4 rows where the slice then fits kWarpSmemMax, else they are loaded directly; a dense model
+// whose row stride (dense_vstride) overflows the slice even then cannot be searched: every d up to 51,024 and every multiple of
+// 16 up to 51,072 fits, nothing else does.  Host arithmetic only; the engine launches with exactly this plan.
+struct PairwisePlan {
+    bool fits;
+    int stages;         // ring depth: 4, or 0 (direct loads)
+    uint32_t per_warp;  // bytes of one warp's slice at that depth
+};
+PairwisePlan pairwise_plan(bool sparse, uint32_t vstride, uint32_t qcap);
+
 struct PairwiseCounters {  // totals over the searcher's last predict call
     unsigned long long pairs = 0;
     unsigned long long n_dist = 0;     // distances evaluated (sum of the pairs' column lengths)
@@ -61,6 +72,9 @@ public:
                  float* ret_D, float* ret_V, bool is_same_input);
     PairwiseCounters counters() const { return counters_; }
     double last_kernel_ms() const { return last_ms_; }
+    // the last predict call: {ring depth of the distance kernel, warps per CTA, per-warp shared-memory bytes, tiles}; all 0
+    // when it had nothing to search (batch or topk 0)
+    void launch_info(uint64_t* out) const;
 
 private:
     PairwiseModel* model_;
@@ -77,6 +91,7 @@ private:
     DeviceBuffer<unsigned long long> ctrl_;  // [0] item counter, [1] sparse entries, [2] replays
     PairwiseCounters counters_;
     double last_ms_ = 0.0;
+    uint64_t last_launch_[4] = {0, 0, 0, 0};
 };
 
 }  // namespace pb200

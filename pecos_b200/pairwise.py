@@ -90,6 +90,10 @@ class PairwiseANN(object):
             by replaying the reference's heap sequence)."""
             return get_clib().pairwise_ann_counters(self.searchers_ptr)
 
+        def launch_info(self):
+            """{stages, warps, per_warp_bytes, tiles} of the last predict call (see core.pairwise_ann_launch_info)."""
+            return get_clib().pairwise_ann_launch_info(self.searchers_ptr)
+
     def __init__(self, model_ptr, num_input_keys, num_label_keys, feat_dim, fn_dict, pred_params=None):
         self.model_ptr = model_ptr
         self.num_input_keys = num_input_keys
@@ -178,7 +182,13 @@ class PairwiseANN(object):
         if num_searcher <= 0:
             raise ValueError("num_searcher={} <= 0 is NOT valid".format(num_searcher))
         pred_params = self.get_pred_params() if pred_params is None else self.PredParams.from_dict(pred_params)
+        self._check_searchable()
         return PairwiseANN.Searchers(self, pred_params, num_searcher)
+
+    def _check_searchable(self):
+        """Dense models wider than the engine's staging area can be trained and saved, not searched: ValueError here."""
+        if self.data_type == "drm":
+            get_clib().pairwise_ann_check_dense(self.feat_dim)
 
     def predict(self, input_feat, label_keys, searchers, is_same_input=False):
         """Returns Imat, Mmat, Dmat, Vmat, each (len(label_keys), only_topk): input ids, 1/0 presence mask, distances and Y
@@ -203,6 +213,7 @@ class PairwiseANN(object):
         if cur_bsz and (not np.issubdtype(label_keys.dtype, np.integer) or label_keys.min() < 0
                         or label_keys.max() >= self.num_label_keys):
             raise ValueError("label_keys must be integers in [0, num_label_keys={})".format(self.num_label_keys))
+        self._check_searchable()
         keys = np.ascontiguousarray(label_keys, dtype=np.uint32)
         only_topk = searchers.pred_params.only_topk
         cur_nnz = cur_bsz * only_topk
