@@ -415,6 +415,11 @@ void pb200_xlinear_host_layer_export(void* hptr, uint32_t layer, void* chunks32,
  * (0xFFFFFFFF: all)}.  Host-only: hptr is a pb200_xlinear_host_* handle, ptr a loaded model (c_xlinear_load_*). */
 int pb200_xlinear_host_plan_fits(void* hptr, uint32_t beam_size, uint32_t only_topk, uint32_t* out);
 int pb200_xlinear_plan_fits(void* ptr, uint32_t beam_size, uint32_t only_topk, uint32_t* out);
+/* Width of a result row of a (beam_size, only_topk) call: the last layer's top-k capacity max(1, min(k, beam entering the
+ * leaf x its widest chunk)), k = only_topk or the stored one.  It is the stride of the index-sharded exchange records, so
+ * callers check world x stride against the merge capacity (1024 records per query) before any GPU work.  Host-only: ptr is
+ * a loaded model, or with host != 0 a pb200_xlinear_host_* handle. */
+uint32_t pb200_xlinear_plan_stride(void* ptr, int host, uint32_t beam_size, uint32_t only_topk);
 /* The limit itself: 15,701 when the layer selects a top-k (topk != 0), else 32,768.  One layer of the python chain
  * (c_xlinear_single_layer_predict_*) enters with a beam of max(row nnz of csr_codes) nodes, or C.cols without codes. */
 uint32_t pb200_xlinear_beam_limit(int topk);

@@ -501,6 +501,7 @@ class B200CoreLib(object):
         fp(c.pb200_xlinear_host_layer_export, None, [c_void_p, c_uint32, c_void_p, c_void_p, c_void_p, c_void_p])
         fp(c.pb200_xlinear_host_plan_fits, c_int, [c_void_p, c_uint32, c_uint32, POINTER(c_uint32)])
         fp(c.pb200_xlinear_plan_fits, c_int, [c_void_p, c_uint32, c_uint32, POINTER(c_uint32)])
+        fp(c.pb200_xlinear_plan_stride, c_uint32, [c_void_p, c_int, c_uint32, c_uint32])
         fp(c.pb200_xlinear_beam_limit, c_uint32, [c_int])
         fp(c.pb200_xlinear_cm_info, c_int, [c_void_p, c_int, POINTER(c_uint64)])
 
@@ -526,6 +527,12 @@ class B200CoreLib(object):
                 f"pecos_b200: the beam entering layer {layer} would hold {width} nodes, more than the supported maximum of "
                 f"{limit}" + (f"; the widest beam_size that fits this model is {widest}" if widest else ""))
         return None if widest == 0xFFFFFFFF else widest
+
+    def xlinear_plan_stride(self, c_model, beam_size, only_topk, host=False):
+        """Width of a result row of a predict call on `c_model` (host=True: a pb200_xlinear_host_* handle) with this
+        beam_size / only_topk (0 or None: the stored values): min(k, beam entering the leaf x its widest chunk), at least 1.
+        Host-only."""
+        return int(self.clib_float32.pb200_xlinear_plan_stride(c_model, 1 if host else 0, int(beam_size or 0), int(only_topk or 0)))
 
     def device_count(self):
         return int(self.clib_float32.pb200_device_count())

@@ -808,6 +808,15 @@ int pb200_xlinear_plan_fits(void* ptr, uint32_t beam_size, uint32_t only_topk, u
     PB200_API_END("pb200_xlinear_plan_fits")
 }
 
+uint32_t pb200_xlinear_plan_stride(void* ptr, int host, uint32_t beam_size, uint32_t only_topk) {
+    PB200_API_BEGIN
+    if (!ptr) throw std::runtime_error("null model handle");
+    // host model only: callable while the device is busy
+    const pb200::XLinearHostModel& m = host ? *static_cast<pb200::XLinearHostModel*>(ptr) : xlinear_of(ptr).primary().host();
+    return pb200::xlinear_plan_stride(m, beam_size, only_topk);
+    PB200_API_END("pb200_xlinear_plan_stride")
+}
+
 uint32_t pb200_xlinear_host_depth(void* hptr) { return static_cast<pb200::XLinearHostModel*>(hptr)->depth(); }
 
 void pb200_xlinear_host_layer_dims(void* hptr, uint32_t layer, uint64_t* out) {

@@ -876,8 +876,9 @@ static_assert(kSortCap * 8 + (kXlBeamMaxTopk * 3 + 1) * 4 <= 200 * 1024 && kSort
               "kXlBeamMaxTopk is the widest beam whose block top-k fits 200 KB of shared memory");
 
 // Widths of the beams entering each layer (the b_prev / k_cap chain of make_plan_); false at the first one over `limit`.
+// k_last: the last layer's k_cap when every beam fits.
 bool beam_chain_fits(const XLinearHostModel& m, uint32_t beam_size, uint32_t only_topk, const std::vector<uint32_t>& b_in,
-                     uint32_t limit, uint32_t* layer, uint32_t* width) {
+                     uint32_t limit, uint32_t* layer, uint32_t* width, uint32_t* k_last = nullptr) {
     const size_t depth = m.layers.size();
     uint32_t b_prev = 1;
     for (size_t d = 0; d < depth; ++d) {
@@ -893,10 +894,17 @@ bool beam_chain_fits(const XLinearHostModel& m, uint32_t beam_size, uint32_t onl
         const uint64_t cand_max = static_cast<uint64_t>(b_prev) * std::max<uint32_t>(L.c_max, 1u);
         b_prev = static_cast<uint32_t>(std::max<uint64_t>(1, std::min<uint64_t>(k, cand_max)));
     }
+    if (k_last) *k_last = b_prev;
     return true;
 }
 
 }  // namespace
+
+uint32_t xlinear_plan_stride(const XLinearHostModel& m, uint32_t beam_size, uint32_t only_topk) {
+    uint32_t k_last = 1;
+    beam_chain_fits(m, beam_size, only_topk, {}, 0xFFFFFFFFu, nullptr, nullptr, &k_last);
+    return k_last;
+}
 
 XLinearBeamCheck xlinear_check_beam(const XLinearHostModel& m, uint32_t beam_size, uint32_t only_topk,
                                     const std::vector<uint32_t>& b_in, bool topk) {

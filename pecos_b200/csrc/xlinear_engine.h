@@ -94,6 +94,9 @@ struct XLinearBeamCheck {
 };
 XLinearBeamCheck xlinear_check_beam(const XLinearHostModel& m, uint32_t beam_size, uint32_t only_topk,
                                     const std::vector<uint32_t>& b_in = {}, bool topk = true);
+// Width of a result row of a (beam_size, only_topk) prediction: the last layer's k_cap in make_plan_, max(1, min(k, beam
+// entering the leaf x its widest chunk)).  It is also the stride of the index-sharded exchange records.  Host model only.
+uint32_t xlinear_plan_stride(const XLinearHostModel& m, uint32_t beam_size, uint32_t only_topk);
 
 class XLinearEngine {
 public:

@@ -26,6 +26,8 @@ import scipy.sparse as smat
 
 from .core import ScipyCompressedSparseAllocator, ScipyCsrF32, XLINEAR_INFERENCE_MODEL_TYPES, get_clib
 
+MERGE_CAPACITY = 1024  # world * stride records per query that the merge kernel holds (kSelKeys in csrc/shard_merge.cuh)
+
 
 def split_rows_by_nnz(indptr, world):
     """Contiguous row blocks with (nearly) equal non-zeros: returns ``world + 1`` row boundaries."""
@@ -103,25 +105,35 @@ class ShardedXLinearModel(object):
         return tuple(int(x) for x in out)
 
     def predict(self, X, beam_size=None, only_topk=None, post_processor=None):
-        """Every rank passes the same ``X`` (float32 CSR with sorted indices)."""
+        """Every rank passes the same ``X`` (float32 CSR with sorted indices).  Raises ValueError before any GPU work when
+        the queries are not such a matrix, the beam is too wide, or world x stride exceeds the merge capacity."""
         import torch
 
-        assert X.dtype == np.float32 and X.has_sorted_indices
+        if not isinstance(X, smat.csr_matrix):
+            raise ValueError(f"type(X) = {type(X)} is not supported: index-sharded prediction takes csr queries only")
+        if not X.has_sorted_indices:
+            raise ValueError("Query matrix does not have sorted indices!")
+        cx = ScipyCsrF32.init_from(X)  # refuses any dtype but float32, as XLinearModel.predict does
         self._clib.xlinear_check_plan(self.model_chain, beam_size, only_topk)
-        c = self._clib.clib_float32
         k = int(only_topk or self.pred_params[-1]["only_topk"])
+        # every rank sends `stride` records per query: k, or fewer where fewer candidates can exist at all
+        stride = self._clib.xlinear_plan_stride(self.model_chain, beam_size, only_topk)
+        if self.world * stride > MERGE_CAPACITY:
+            narrow = f" (stride {stride} of top-k {k}: the most candidates a leaf row can hold)" if stride != k else ""
+            raise ValueError(f"world * top-k = {self.world * stride}{narrow} exceeds the merge capacity of {MERGE_CAPACITY} "
+                             f"records per query")
+        c = self._clib.clib_float32
         rows = X.shape[0]
         dev = torch.device("cuda", c.pb200_get_device())
         # send buffer of the exchange: 16-byte {u64 key, u32 id, f32 value} records, viewed as int64 pairs for torch
-        rec = torch.zeros((rows, k, 2), dtype=torch.int64, device=dev)
+        rec = torch.zeros((rows, stride, 2), dtype=torch.int64, device=dev)
         torch.cuda.synchronize(dev)
-        cx = ScipyCsrF32.init_from(X)
         pp = post_processor.encode("utf-8") if post_processor else None
-        stride = c.pb200_xlinear_sharded_local_csr_packed(self.model_chain, byref(cx), beam_size or 0, pp, only_topk or 0, k,
-                                                          rec.data_ptr())
-        if stride != k:  # fewer candidates than k can exist at all: the engine used a narrower stride
-            rec = rec.view(-1)[: rows * stride * 2].view(rows, stride, 2)
-        g_rec = self.comm.all_gather(rec.contiguous())  # THE exchange: one all-gather of one buffer
+        used = c.pb200_xlinear_sharded_local_csr_packed(self.model_chain, byref(cx), beam_size or 0, pp, only_topk or 0, stride,
+                                                        rec.data_ptr())
+        if used != stride:
+            raise RuntimeError(f"pecos_b200: the engine used a stride of {used} records, the host plan {stride}")
+        g_rec = self.comm.all_gather(rec)  # THE exchange: one all-gather of one buffer
         torch.cuda.synchronize(dev)
         self.last_exchange_bytes = int(rec.numel() * 8)
         alloc = ScipyCompressedSparseAllocator()
@@ -137,7 +149,7 @@ class ShardedHNSW(object):
     bit for bit, the merge of the per-shard searches ordered by (distance, shard rank, slot within the shard), with global
     ids ``row_begin[r] + local id``.  At world 1 it is the unsharded search."""
 
-    MERGE_CAPACITY = 1024  # world * topk records per query (kSelKeys in csrc/shard_merge.cuh)
+    MERGE_CAPACITY = MERGE_CAPACITY
 
     def __init__(self, index, manifest, rank, world, comm, clib):
         self.index = index
