@@ -354,6 +354,34 @@ int pb200_pairwise_ann_dense_fits(uint32_t feat_dim, uint32_t* out);
  * feat_dim, nnz of Y, nnz of X, longest column}, or 1 (reason on stderr). */
 int pb200_pairwise_ann_host_info(const char* model_dir, int sparse, uint64_t* out);
 
+/* ============================================ sparse x sparse products ============================================ */
+/* libpecos.cpp:320-335, smat_x_smat (pecos/core/utils/matrix.hpp:1062-1290).  csr: Z = X Y, row i of Z from row i of X and
+ * the rows of Y, pred_alloc(false, X.rows, Y.cols, nnz); csc: column i of Z from column i of Y and the columns of X,
+ * pred_alloc(true, X.rows, Y.cols, nnz).  Bit-identical to the reference: each output entry starts at +0.0f and receives
+ * acc = acc + a_s * b_t (separate roundings) for every contribution in traversal order (entries s of the A row in stored
+ * order, then entries t of B row A.idx[s] in stored order); repeated and unsorted indices are separate contributions.  Indices
+ * of an output row come ascending (sorted_indices) or in first-touch order.  pred_alloc gets the number of distinct indices
+ * touched; with eliminate_zeros, entries equal to +-0 are then compacted out (NaN stays) and indptr describes what is left.
+ * pred_alloc is called exactly once, from the calling thread, also for empty products; threads is accepted and ignored.
+ * X.cols != Y.rows, an index of the left operand (csr: X, csc: Y) beyond the right operand's rows, or one of the right operand
+ * beyond the output width is a fatal error before any GPU work.  Runs on the pb200_set_device device; calls on one device are
+ * serialised.  The device workspace (hash accumulators, output staging, A tiles) is bounded by PB200_SPMM_WORKSPACE_MB
+ * (read on every call, default 1024); a single row that needs more runs as a tile of its own. */
+void c_sparse_matmul_csr_f32(const ScipyCsrF32* pX, const ScipyCsrF32* pY, py_sparse_allocator_t pred_alloc,
+                             const bool eliminate_zeros, const bool sorted_indices, int threads);
+void c_sparse_matmul_csc_f32(const ScipyCscF32* pX, const ScipyCscF32* pY, py_sparse_allocator_t pred_alloc,
+                             const bool eliminate_zeros, const bool sorted_indices, int threads);
+/* 1 if a product whose right operand (csr: Y, csc: X, as rows of the traversal) has b_rows rows and b_nnz entries fits the
+ * current device: its arrays, one flag byte per row and 64 MB of workspace within cudaMemGetInfo's free bytes; else 0 (also
+ * without a device).  out[2] = {bytes needed, free bytes}. */
+int pb200_spmm_fits(uint32_t b_rows, uint64_t b_nnz, uint64_t* out);
+/* The calling thread's last product: out[10] = {A rows (csr: X.rows, csc: Y.cols), products (sum over A entries of their B
+ * row lengths), nnz handed to pred_alloc, nnz kept after eliminate_zeros, rows counted by the warp / CTA symbolic kernels,
+ * rows folded by the warp / CTA numeric kernels, tiles, kernel launches}. */
+void pb200_spmm_last_info(uint64_t* out);
+/* device time (CUDA events) of the calling thread's last product's kernels, in ms */
+double pb200_spmm_last_kernel_ms(void);
+
 /* base-vector rows kept in flight per warp by the bulk-copy (TMA) ring: 0 = direct loads, 4 (default) or 8; returns the
  * value in effect.  Results are identical for every setting.  A search whose per-warp shared-memory slice (query + ring
  * rows + result heap) would exceed 200 KB at this depth runs the next shallower one that fits (8 -> 4 -> 0); dense indices

@@ -7,6 +7,7 @@ Mirrors, for the two hot paths only, the reference's Python-side FFI layer:
 * ``corelib.xlinear_*`` helpers ......................... pecos/core/base.py:990-1095
 * ``corelib.link_ann_hnsw_methods`` / fn_dict ........... pecos/core/base.py:1865-1964
 * ``corelib.link_pairwise_ann_methods`` / fn_dict ....... pecos/core/base.py:1966-2066
+* ``corelib.sparse_matmul`` ............................... pecos/core/base.py:1461-1534
 
 There is no CPU fallback: if the CUDA library is missing, or no GPU is visible when a model is loaded,
 a ``RuntimeError`` is raised.
@@ -83,6 +84,10 @@ class ScipyCsrF32(ctypes.Structure):
         self.data = data.ctypes.data_as(POINTER(c_float))
         return self
 
+    @property
+    def shape(self):
+        return (self.rows, self.cols)
+
 
 class ScipyCscF32(ctypes.Structure):
     """C view of a float32 scipy CSC matrix (pecos/core/base.py:177-216); same layout as ScipyCsrF32 with col_ptr /
@@ -113,6 +118,10 @@ class ScipyCscF32(ctypes.Structure):
         self.indices = self.py_buf["indices"].ctypes.data_as(POINTER(c_uint32))
         self.data = self.py_buf["data"].ctypes.data_as(POINTER(c_float))
         return self
+
+    @property
+    def shape(self):
+        return (self.rows, self.cols)
 
 
 class ScipyDrmF32(ctypes.Structure):
@@ -184,6 +193,7 @@ class B200CoreLib(object):
         self.link_xlinear_methods()
         self.link_ann_hnsw_methods()
         self.link_pairwise_ann_methods()
+        self.link_sparse_matmul_methods()
         self.link_b200_methods()
 
     @staticmethod
@@ -435,6 +445,72 @@ class B200CoreLib(object):
         if self.clib_float32.pb200_pairwise_ann_host_info(c_model_dir.encode("utf-8"), 1 if data_type == "csr" else 0, out) != 0:
             raise ValueError("pecos_b200: {} is not a loadable PairwiseANN {} folder".format(c_model_dir, data_type))
         keys = ("num_input_keys", "num_label_keys", "feat_dim", "nnz_of_Y", "nnz_of_X", "longest_column")
+        return dict(zip(keys, [int(v) for v in out]))
+
+    # ---------------------------------------------------------------- sparse x sparse products (base.py:1461-1534)
+    def link_sparse_matmul_methods(self):
+        c = self.clib_float32
+        fp = B200CoreLib.fillprototype
+        alloc = ScipyCompressedSparseAllocator.CFUNCTYPE
+        fp(c.c_sparse_matmul_csr_f32, None, [POINTER(ScipyCsrF32), POINTER(ScipyCsrF32), alloc, c_bool, c_bool, c_int])
+        fp(c.c_sparse_matmul_csc_f32, None, [POINTER(ScipyCscF32), POINTER(ScipyCscF32), alloc, c_bool, c_bool, c_int])
+        fp(c.pb200_spmm_fits, c_int, [c_uint32, c_uint64, POINTER(c_uint64)])
+        fp(c.pb200_spmm_last_info, None, [POINTER(c_uint64)])
+        fp(c.pb200_spmm_last_kernel_ms, c_double, [])
+
+    def sparse_matmul(self, X, Y, eliminate_zeros=False, sorted_indices=True, threads=-1):
+        """Same contract as corelib.sparse_matmul (pecos/core/base.py:1461-1534): X @ Y for csr_matrix / csc_matrix /
+        ScipyCsrF32 / ScipyCscF32 operands, the same four dispatch branches, a csr_matrix or csc_matrix back.  Bit-identical to
+        the reference.  Raises ValueError on a shape mismatch, RuntimeError without a GPU and MemoryError when the right operand
+        of the call does not fit the device (pb200_spmm_fits); none of them after any GPU work."""
+        if X.shape[1] != Y.shape[0]:
+            raise ValueError("X.shape[1]={} != Y.shape[0]={}".format(X.shape[1], Y.shape[0]))
+        self.require_gpu()
+        clib = self.clib_float32
+        pred_alloc = ScipyCompressedSparseAllocator()
+
+        def is_col_major(M):
+            return isinstance(M, smat.csc_matrix) or isinstance(M, ScipyCscF32)
+
+        def is_row_major(M):
+            return isinstance(M, smat.csr_matrix) or isinstance(M, ScipyCsrF32)
+
+        if is_col_major(X) and is_col_major(Y):
+            fmt = "csc"
+        elif is_row_major(X) and is_row_major(Y):
+            fmt = "csr"
+        elif is_col_major(X) and is_row_major(Y):
+            if X.nnz > Y.nnz:
+                Y, fmt = Y.tocsc(), "csc"
+            else:
+                X, fmt = X.tocsr(), "csr"
+        elif is_row_major(X) and is_col_major(Y):
+            if X.nnz > Y.nnz:
+                Y, fmt = Y.tocsr(), "csr"
+            else:
+                X, fmt = X.tocsc(), "csc"
+        else:
+            raise ValueError("X and Y should be either csr_matrix/csc_matrix/ScipyCscF32/ScipyCsrF32 !")
+        view = ScipyCscF32 if fmt == "csc" else ScipyCsrF32
+        pX = X if isinstance(X, view) else view.init_from(X)
+        pY = Y if isinstance(Y, view) else view.init_from(Y)
+        # the operand whose rows the traversal reads (csr: Y's rows, csc: X's columns) stays on the device for the call
+        b_rows, b_nnz = (pY.rows, int(pY.indptr[pY.rows])) if fmt == "csr" else (pX.cols, int(pX.indptr[pX.cols]))
+        need = (c_uint64 * 2)()
+        if not clib.pb200_spmm_fits(b_rows, b_nnz, need):
+            raise MemoryError("pecos_b200: sparse_matmul needs {} device bytes for its right operand and workspace, {} are "
+                              "free".format(int(need[0]), int(need[1])))
+        fn = clib.c_sparse_matmul_csc_f32 if fmt == "csc" else clib.c_sparse_matmul_csr_f32
+        fn(byref(pX), byref(pY), pred_alloc.cfunc, eliminate_zeros, sorted_indices, threads)
+        return pred_alloc.get()
+
+    def sparse_matmul_last_info(self):
+        """The calling thread's last product: {a_rows, products, alloc_nnz, kept_nnz, count_warp_rows, count_cta_rows,
+        fold_warp_rows, fold_cta_rows, tiles, launches}."""
+        out = (c_uint64 * 10)()
+        self.clib_float32.pb200_spmm_last_info(out)
+        keys = ("a_rows", "products", "alloc_nnz", "kept_nnz", "count_warp_rows", "count_cta_rows", "fold_warp_rows",
+                "fold_cta_rows", "tiles", "launches")
         return dict(zip(keys, [int(v) for v in out]))
 
     # ---------------------------------------------------------------- pb200_* additions

@@ -18,6 +18,7 @@
 #include "hnsw_build_sparse.h"
 #include "hnsw_engine.h"
 #include "pairwise_engine.h"
+#include "spmm_engine.h"
 #include "xlinear_engine.h"
 
 namespace {
@@ -1277,5 +1278,53 @@ int pb200_pairwise_ann_host_info(const char* model_dir, int sparse, uint64_t* ou
         return 1;
     }
 }
+
+// ------------------------------------------------ sparse x sparse products ------------------------------------------
+// The calling thread's last product: pb200_spmm_last_info / pb200_spmm_last_kernel_ms.
+static thread_local uint64_t t_spmm_info[pb200::kSpmmInfoLen] = {};
+static thread_local double t_spmm_kernel_ms = 0.0;
+
+// csr: Z = X Y row by row of X (rows of Y); csc: column by column of Y (columns of X) -- libpecos.cpp:320-335
+static void sparse_matmul(const uint32_t x_rows, const uint32_t x_cols, const uint32_t y_rows, const uint32_t y_cols,
+                          const pb200::SpmmOperand& a, const pb200::SpmmOperand& b, uint32_t width, bool col_major,
+                          py_sparse_allocator_t pred_alloc, bool eliminate_zeros, bool sorted_indices) {
+    if (x_cols != y_rows)
+        throw std::runtime_error("X.cols = " + std::to_string(x_cols) + " != Y.rows = " + std::to_string(y_rows));
+    pb200::spmm_run(g_device.load(), a, b, width, col_major, x_rows, y_cols, pred_alloc, eliminate_zeros, sorted_indices,
+                    t_spmm_info, &t_spmm_kernel_ms);
+}
+
+void c_sparse_matmul_csr_f32(const ScipyCsrF32* pX, const ScipyCsrF32* pY, py_sparse_allocator_t pred_alloc,
+                             const bool eliminate_zeros, const bool sorted_indices, int threads) {
+    PB200_API_BEGIN
+    (void)threads;
+    sparse_matmul(pX->rows, pX->cols, pY->rows, pY->cols, {pX->rows, pX->row_ptr, pX->col_idx, pX->val},
+                  {pY->rows, pY->row_ptr, pY->col_idx, pY->val}, pY->cols, false, pred_alloc, eliminate_zeros, sorted_indices);
+    PB200_API_END("c_sparse_matmul_csr_f32")
+}
+
+void c_sparse_matmul_csc_f32(const ScipyCscF32* pX, const ScipyCscF32* pY, py_sparse_allocator_t pred_alloc,
+                             const bool eliminate_zeros, const bool sorted_indices, int threads) {
+    PB200_API_BEGIN
+    (void)threads;
+    sparse_matmul(pX->rows, pX->cols, pY->rows, pY->cols, {pY->cols, pY->col_ptr, pY->row_idx, pY->val},
+                  {pX->cols, pX->col_ptr, pX->row_idx, pX->val}, pX->rows, true, pred_alloc, eliminate_zeros, sorted_indices);
+    PB200_API_END("c_sparse_matmul_csc_f32")
+}
+
+int pb200_spmm_fits(uint32_t b_rows, uint64_t b_nnz, uint64_t* out) {
+    const uint64_t need = (b_nnz >> 60) ? ~0ull : pb200::spmm_min_bytes(b_rows, b_nnz);
+    size_t free_b = 0, total_b = 0;
+    const bool ok = cudaSetDevice(g_device.load()) == cudaSuccess && cudaMemGetInfo(&free_b, &total_b) == cudaSuccess;
+    if (!ok) cudaGetLastError();
+    if (out) { out[0] = need; out[1] = ok ? free_b : 0; }
+    return ok && need <= free_b ? 1 : 0;
+}
+
+void pb200_spmm_last_info(uint64_t* out) {
+    for (int i = 0; i < pb200::kSpmmInfoLen; ++i) out[i] = t_spmm_info[i];
+}
+
+double pb200_spmm_last_kernel_ms(void) { return t_spmm_kernel_ms; }
 
 }  // extern "C"

@@ -2,7 +2,8 @@
 
 ``overlay(clib)`` re-points the XR-Linear predict-only and HNSW (dense and sparse) search function pointers of the reference's
 ``corelib`` instance (pecos/core/base.py:481-539, :1951-1964), and all seven PairwiseANN slots (base.py:1966-2051), at
-``libpecos_b200_float32.so``; every other symbol keeps using the reference CPU library.  The reference package itself is not imported here: pass its ``clib`` object in.
+``libpecos_b200_float32.so``; with ``sparse_matmul=True`` also ``c_sparse_matmul_{csr,csc}_f32`` (base.py:1461-1534).  Every other
+symbol keeps using the reference CPU library.  The reference package itself is not imported here: pass its ``clib`` object in.
 """
 import ctypes
 
@@ -39,11 +40,14 @@ XLINEAR_SYMBOLS = (
 HNSW_SLOTS = ("load", "destruct", "searchers_create", "searchers_destruct", "predict", "save")
 # PairwiseANN handles all come from one library (train is a deep copy and is served here), so every slot is swapped together
 PAIRWISE_SLOTS = ("train", "load", "save", "destruct", "searchers_create", "searchers_destruct", "predict")
+# opt-in: for small products (the python chain's `selected x C`) the host<->device copies can outweigh the CPU product
+SPARSE_MATMUL_SYMBOLS = ("c_sparse_matmul_csr_f32", "c_sparse_matmul_csc_f32")
 
 
-def overlay(clib, lib_path=LIB_PATH, require_gpu=True):
+def overlay(clib, lib_path=LIB_PATH, require_gpu=True, sparse_matmul=False):
     """Returns the list of symbols that were re-pointed.  require_gpu=False only re-points (binding tests on a box without a
-    GPU); any call into the re-pointed symbols then aborts with "no CUDA device visible" -- there is no CPU fallback."""
+    GPU); any call into the re-pointed symbols then aborts with "no CUDA device visible" -- there is no CPU fallback.
+    sparse_matmul=True also re-points the two sparse x sparse product symbols (off by default)."""
     b200 = ctypes.CDLL(lib_path)
     if require_gpu and b200.pb200_device_count() <= 0:
         raise RuntimeError("pecos_b200: no CUDA device visible and there is no CPU fallback")
@@ -88,5 +92,11 @@ def overlay(clib, lib_path=LIB_PATH, require_gpu=True):
             pw_dict[key][slot] = fn
             setattr(clib.clib_float32, name, fn)
             swapped.append(name)
+    for name in SPARSE_MATMUL_SYMBOLS if sparse_matmul else ():
+        ref = getattr(clib.clib_float32, name)
+        fn = getattr(b200, name)
+        fn.restype, fn.argtypes = ref.restype, ref.argtypes
+        setattr(clib.clib_float32, name, fn)
+        swapped.append(name)
     clib.clib_b200 = b200
     return swapped
