@@ -229,18 +229,13 @@ void pb200_xlinear_sharded_merge_packed(void* ptr, uint32_t world, uint32_t rows
  *   profile: out[2*d] = chunk-score kernel ms, out[2*d+1] = top-k kernel ms   (accumulated since reset)
  *   stats:   out[7*d + {0..6}] = chunks, sum R, sum m, sum e, sum c, sum nnz(x), sum beam-out   (last stats pass) */
 void pb200_xlinear_set_profile(void* ptr, int on);
-/* Kernel generation selector for A/B tests (results are identical): 0 = row-list streaming + block-wide sort,
- * 1 = default (feature-map kernels + warp top-k; query-warp kernel for beams of many narrow chunks; chunk-major kernel on
- * layers whose chunk images fit and whose chunks are visited by enough pairs), 2 = as 1 but feature-map lookups with one
- * warp per chunk in place of the query-warp kernel, 3 = as 1 but the query-warp kernel wherever it is eligible and the
- * chunk-major kernel is not chosen, 4 = as 1 but the warp top-k evaluates the post-processor for every candidate (no
- * single-precision estimate filter), 5 = as 1 plus the chunk-major kernel on every layer with chunk images (its reuse and
- * occupancy heuristics ignored, and the prefix kernel below on tiles of any size), 6 = as 1 without the chunk-major kernel
- * (query-major kernels only, no prefix kernel), 7 = as 1 without the prefix kernel.  Any other value behaves as 1.
- * Prefix kernel (modes 1 - 5): where layer 0 is one chunk, every query's beam holds all of layer 0, neither upper layer is
- * rearranged, both share their bias and their merged image fits in shared memory, a sparse tile of enough queries scores
- * layers 0 and 1 in ONE chunk-major launch (kernel id 4 in layer 0's score slot; layer 0's top-k slot and layer 1's score
- * slot then read 0 ms).  Results are identical with and without it.
+/* Kernel mode for A/B tests (results are identical in every mode): 0 first generation (row-list streaming + block-wide
+ * sort), 1 default, 2 no query-warp kernel, 3 query-warp kernel wherever it fits, 4 no top-k estimate filter, 5 chunk-major
+ * kernel wherever a layer has chunk images and the prefix launch on tiles of any size, 6 query-major kernels only, 7 no
+ * prefix launch.  Any other value behaves as 1.  XLinearEngine::pick_kernels_ (pecos_b200/csrc/xlinear_engine.cu) states
+ * what each mode lets a layer take and the order in which the kernels are preferred.
+ * Prefix launch (modes 1 - 5): a sparse tile of enough queries scores layers 0 and 1 in ONE chunk-major launch (kernel id 4
+ * for both layers; layer 0's top-k slot and layer 1's score slot then read 0 ms).
  * Returns 1 when every layer has a feature map (PB200_FEATMAP_MB caps their total size at load time, default 32768). */
 int pb200_xlinear_set_lookup(void* ptr, int on);
 void pb200_xlinear_reset_profile(void* ptr);

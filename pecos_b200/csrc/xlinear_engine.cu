@@ -1126,24 +1126,6 @@ XLinearEngine::~XLinearEngine() {
     if (stream_) cudaStreamDestroy(stream_);
 }
 
-void XLinearEngine::set_kernel_mode(int mode) {
-    // 0: first generation (row-list streaming + block-wide sort); 1: default (query-warp / feature-map kernels + warp top-k);
-    // 2: feature-map lookups with one warp per chunk (no query-warp kernel); 3: query-warp kernel wherever eligible;
-    // 4: as 1 but the warp top-k evaluates the post-processor for every candidate (no estimate filter);
-    // 5: as 1, and the chunk-major score kernel wherever it FITS (its reuse / occupancy heuristics ignored; tests);
-    // 6: as 1 WITHOUT the chunk-major score kernel (query-major kernels only, no prefix kernel, for A/B tests);
-    // 7: as 1 without the prefix kernel (layers 0 and 1 scored and selected one by one, for A/B tests)
-    const bool on = mode != 0;
-    for (auto& l : layers_) l.view.featmap = (on && l.featmap.capacity()) ? l.featmap.get() : nullptr;
-    force_block_topk_ = !on;
-    no_query_warp_ = (mode == 2);
-    force_query_warp_ = (mode == 3);
-    no_topk_filter_ = (mode == 4);
-    chunk_major_ = on && (mode != 6);
-    cm_force_ = (mode == 5);
-    no_prefix_ = (mode == 7);
-}
-
 bool XLinearEngine::has_feature_maps() const {
     for (auto& l : layers_) if (!l.featmap.capacity()) return false;
     return true;
@@ -1191,7 +1173,7 @@ uint32_t XLinearEngine::ensure_workspace_(const std::vector<LayerPlan>& plan, ui
         b_max = std::max<uint64_t>(b_max, plan[d].b_prev);
         chunks_max = std::max<uint64_t>(chunks_max, host_->layers[d].n_chunks);
     }
-    const bool cm = chunk_major_ && has_feature_maps();
+    const bool cm = chunk_major_workspace_();
     const uint64_t pairs = b_max * 4;  // up to 4 column ranges per chunk
     const uint64_t per_query = 16 + 2 * beam_stride * 8 + cand_max * 4 + sort_max * 8 + (cm ? beam_stride * 4 + pairs * 8 : 0);
     uint64_t budget = 8ull << 30;
@@ -1220,11 +1202,91 @@ uint32_t XLinearEngine::ensure_workspace_(const std::vector<LayerPlan>& plan, ui
     return static_cast<uint32_t>(tile);
 }
 
-// Launches the score kernel of layer d for the beam held in beam_*_[cur] (capacity b_prev slots per query): fills
-// cand_[(ws_row + q) * b_prev * c_max + slot_base(j) + c] with the raw scores of every child of every beam node, in prolongation order.
-// Chooses between the chunk-major, query-warp, feature-map, row-list and dense kernels.  Returns the kernel id.
-int XLinearEngine::score_layer_(size_t d, const QueryDev& q, uint32_t b_prev, int cur, uint32_t ws_row, bool collect_stats) {
+// Kernel ids, as XLinearLayerProfile and pb200_xlinear_get_kernel_ids report them.
+enum : int { kScoreRowList = 0, kScoreLookup = 1, kScoreDense = 2, kScoreQueryWarp = 3, kScoreChunkMajor = 4 };
+enum : int { kNoTopk = -1, kTopkBlock = 0, kTopkWarp = 1, kTopkFilter = 2 };
+
+struct XLinearEngine::TileShape {  // run_tile_'s arguments; topk = false: no top-k kernel follows the scores (selected outputs)
+    bool ext_beam;
+    int combine_first;
+    size_t d_begin, d_end;
+    bool collect_stats, topk;
+};
+
+struct XLinearEngine::LayerKernels {
+    int score = kScoreRowList;
+    CmPlan cm;            // launch shape of the chunk-major score kernel (score == kScoreChunkMajor without the prefix)
+    int topk = kNoTopk;   // kNoTopk: no top-k kernel runs, and the layer's reported top-k id keeps its last value
+    bool prefix = false;  // layers 0 and 1 of the tile are scored by one prefix launch, issued at layer 0
+};
+
+// Chooses the kernels of layer d for one tile, from the kernel mode, the model and the call alone.
+//
+// Kernel modes (set_kernel_mode, PB200_XL_KERNEL_MODE), all with the same results: 0 first generation (every layer treated
+// as having no feature map, block top-k); 1 default; 2 no query-warp kernel; 3 the query-warp kernel wherever it fits;
+// 4 no estimate filter (the warp select evaluates every candidate); 5 the chunk-major kernel wherever a layer has images,
+// and the prefix launch on tiles of any size (tests); 6 query-major kernels only (no chunk-major, no prefix); 7 no prefix.
+//
+// Order of preference [reported id]: score prefix [4] > chunk-major [4] > query-warp [3] > dense [2] > lookup [1] >
+// row-list [0]; top-k filter [2] > warp select [1] > block sort [0], none for selected outputs nor for layer 0 under the
+// prefix.  Candidate limits compare b_prev x c_max, the widest row the beam can produce.
+XLinearEngine::LayerKernels XLinearEngine::pick_kernels_(size_t d, const QueryDev& q, const std::vector<LayerPlan>& plan,
+                                                         const TileShape& t) const {
+    const LayerStore& S = layers_[d];
+    const LayerPlan& lp = plan[d];
+    const uint64_t cand_stride_q = static_cast<uint64_t>(lp.b_prev) * std::max<uint32_t>(S.view.c_max, 1u);
+    const bool sparse = q.row_ptr != nullptr;
+    const bool first_gen = mode_ == KernelMode::kFirstGeneration;
+    const bool force_cm = mode_ == KernelMode::kChunkMajorWherever;
+    const bool cm_offsets_fit = static_cast<uint64_t>(q.rows) * std::max<uint32_t>(q.max_row_nnz, 1u) < (1ull << 32);  // 32-bit feature offsets
+    LayerKernels k;
+
+    // The prefix image exists only where layers 0 and 1 have feature maps.  Layer 0's top-k must keep all of layer 0, so that
+    // layer 1's beam is all of layer 1 in layer 0's rank order.  A small tile leaves most SMs idle in the one-pass kernel,
+    // while the per-layer kernels spread its pairs wider.
+    const bool root_tile = !t.ext_beam && t.d_begin == 0 && t.d_end >= 2 && t.combine_first == 0 && !t.collect_stats;
+    const bool prefix_mode = !first_gen && mode_ != KernelMode::kQueryMajorOnly && mode_ != KernelMode::kNoPrefix;
+    const bool keeps_layer0 = plan[0].k >= host_->layers[0].n_cols;
+    const bool fills_gpu = force_cm || q.rows >= kCmMinPairsPerSm * n_sm_;
+    k.prefix = d < 2 && root_tile && prefix_mode && prefix_.cm_shape.ok && sparse && keeps_layer0 && cm_offsets_fit && fills_gpu;
+
+    const bool lookup = sparse && !first_gen && S.featmap.capacity() != 0;  // mode 0: as if no layer had a feature map
+    // the statistics pass runs the query-major kernels: their counters are the canonical ones
+    if (!k.prefix && lookup && !t.collect_stats && cm_offsets_fit && chunk_major_workspace_() && S.cm_images.capacity())
+        k.cm = cm_plan(S.cm_shape, S.view.n_chunks, static_cast<uint64_t>(q.rows) * lp.b_prev, n_sm_, force_cm);
+    // One warp per query over the whole beam (feature-major) wins when the beam consists of MANY NARROW chunks (per-chunk
+    // bookkeeping dominates: S layers 1-4, 20 x 8 columns), and loses on wide chunks where one warp per chunk keeps more
+    // loads in flight (E and S leaves).
+    const bool qw_fits = lookup && lp.b_prev <= static_cast<uint32_t>(kQwSlots) &&
+                         cand_stride_q <= static_cast<uint64_t>(kQwNCap) && q.max_row_nnz <= kQwQCap;
+    const bool query_warp = qw_fits && mode_ != KernelMode::kNoQueryWarp &&
+                            (mode_ == KernelMode::kQueryWarpWherever || (lp.b_prev >= 16u && cand_stride_q <= 256u));
+    k.score = (k.prefix || k.cm.eligible) ? kScoreChunkMajor : query_warp ? kScoreQueryWarp : !sparse ? kScoreDense
+                                                             : lookup ? kScoreLookup : kScoreRowList;
+
+    if (!t.topk || (k.prefix && d == 0)) return k;  // layer 0's beam comes out of the prefix launch
+    const bool hinge = lp.pp.kind == PP_LP_HINGE || lp.pp.kind == PP_LOG_LP_HINGE;
+    const bool exact_power = !hinge || (lp.pp.p >= 0 && lp.pp.p <= 4);  // the filter forms hinge powers up to 4 exactly
+    const bool filter = !first_gen && mode_ != KernelMode::kNoTopkFilter && lp.k <= 32u && exact_power &&
+                        lp.b_prev <= static_cast<uint32_t>(kFltSlots) && cand_stride_q <= static_cast<uint64_t>(kFltKeysMax);
+    const bool warp_select = !first_gen && lp.b_prev <= static_cast<uint32_t>(kSelSlots) &&
+                             cand_stride_q <= static_cast<uint64_t>(kSelKeysMax) && lp.k <= static_cast<uint32_t>(kSelK);
+    k.topk = filter ? kTopkFilter : warp_select ? kTopkWarp : kTopkBlock;
+    return k;
+}
+
+// Launches the score kernel k chose for layer d over the beam held in beam_*_[cur] (capacity b_prev slots per query): fills
+// cand_[(ws_row + q) * b_prev * c_max + slot_base(j) + c] with the raw scores of every child of every beam node, in
+// prolongation order.  Under the prefix, layer 0's launch also scores layer 1, and layer 1 launches nothing.
+void XLinearEngine::score_layer_(size_t d, const QueryDev& q, const std::vector<LayerPlan>& plan, const LayerKernels& k, int cur,
+                                 uint32_t ws_row, bool collect_stats) {
+    layer_profile_[d].scores_kernel = k.score;
+    if (k.prefix) {
+        if (d == 0) launch_prefix_(q, plan, ws_row);
+        return;
+    }
     const LayerDev& L = layers_[d].view;
+    const uint32_t b_prev = plan[d].b_prev;
     const uint32_t rows = q.rows;
     const bool dense = (q.row_ptr == nullptr);
     const uint32_t c_stride = std::max<uint32_t>(L.c_max, 1u);
@@ -1237,7 +1299,7 @@ int XLinearEngine::score_layer_(size_t d, const QueryDev& q, uint32_t b_prev, in
     const uint32_t rounds = (b_prev + kWarpsMax - 1) / kWarpsMax;
     const int warps = static_cast<int>(std::max<uint32_t>(1, (b_prev + rounds - 1) / std::max<uint32_t>(rounds, 1)));
     const dim3 grid(rows), block(warps * 32);
-    const bool lookup = !dense && L.featmap != nullptr;
+    const bool lookup = k.score == kScoreLookup;
     // query staging area: as small as the batch's longest row allows (occupancy), at most kQCap non-zeros
     const uint32_t q_cap = dense ? 32u : std::min<uint32_t>(kQCap, std::max<uint32_t>(32u, (q.max_row_nnz + 31u) & ~31u));
     const uint32_t sb_cap = (b_prev + 1u + 3u) & ~3u;
@@ -1247,22 +1309,8 @@ int XLinearEngine::score_layer_(size_t d, const QueryDev& q, uint32_t b_prev, in
         kernel<<<grid, block, smem1, stream_>>>(L, q, bid, bcnt, beam_stride_, cand,
                                                cand_stride_q, c_stride, stats, q_cap, sb_cap, hdr_cap);
     };
-    // One warp per query over the whole beam (feature-major).  It wins when the beam consists of MANY NARROW chunks
-    // (per-chunk bookkeeping dominates: S layers 1-4, 20 x 8 columns), and loses on wide chunks where one warp per chunk
-    // keeps more loads in flight (E and S leaves).  force_query_warp_ (kernel mode 3) selects it whenever it is eligible, for tests.
-    const bool qw_eligible = lookup && b_prev <= static_cast<uint32_t>(kQwSlots) &&
-                             cand_stride_q <= static_cast<uint64_t>(kQwNCap) && q.max_row_nnz <= kQwQCap;
-    const bool query_warp = qw_eligible && !no_query_warp_ &&
-                            (force_query_warp_ || (b_prev >= 16u && cand_stride_q <= 256u));
-    // Chunk-major scoring (xlinear_cm_kernel.cuh) wherever the layer's feature map + largest chunk fit in shared memory
-    // and the chunks are visited by enough pairs to amortise the staging; otherwise the query-major kernels below.
-    // (the statistics pass always runs the query-major kernels: their counters are the canonical ones)
-    const bool cm_offsets_fit = static_cast<uint64_t>(rows) * std::max<uint32_t>(q.max_row_nnz, 1u) < (1ull << 32);  // 32-bit feature offsets
-    const CmPlan cm = (chunk_major_ && lookup && !collect_stats && cm_offsets_fit && cm_slot_pos_.capacity() && layers_[d].cm_images.capacity())
-                          ? cm_plan(layers_[d].cm_shape, L.n_chunks, static_cast<uint64_t>(rows) * b_prev, n_sm_, cm_force_)
-                          : CmPlan{};
-    const bool chunk_major = cm.eligible;
-    if (chunk_major) {
+    if (k.score == kScoreChunkMajor) {
+        const CmPlan& cm = k.cm;
         const CmShape& shape = layers_[d].cm_shape;
         const uint32_t n_vc = shape.n_vc;
         CmWork w{cm_slot_pos_.get(), cm_count_.get(), cm_bucket_ptr_.get(), cm_cost_ptr_.get(), cm_pair_q_.get(), cm_pair_pos_.get(),
@@ -1279,7 +1327,7 @@ int XLinearEngine::score_layer_(size_t d, const QueryDev& q, uint32_t b_prev, in
         if (shape.direct) { if (shape.stages == 4) launch_cm(xl_cm_scores_kernel<true, 4>); else launch_cm(xl_cm_scores_kernel<true, 2>); }
         else { if (shape.stages == 4) launch_cm(xl_cm_scores_kernel<false, 4>); else launch_cm(xl_cm_scores_kernel<false, 2>); }
         launches_ += 3;  // + the score kernel counted below
-    } else if (query_warp) {
+    } else if (k.score == kScoreQueryWarp) {
         const uint32_t qw_qcap = std::max<uint32_t>(32u, (q.max_row_nnz + 31u) & ~31u);
         const uint32_t qw_ncap = static_cast<uint32_t>((cand_stride_q + 31) & ~static_cast<uint64_t>(31));
         const size_t qw_smem = kQwWarps * ((qw_warp_bytes(qw_qcap, qw_ncap) + 15) & ~static_cast<size_t>(15));
@@ -1290,7 +1338,7 @@ int XLinearEngine::score_layer_(size_t d, const QueryDev& q, uint32_t b_prev, in
         else
             xl_query_warp_scores_kernel<false><<<qw_grid, kQwWarps * 32, qw_smem, stream_>>>(
                 L, q, bid, bcnt, beam_stride_, cand, cand_stride_q, stats, qw_qcap, qw_ncap, rows);
-    } else if (dense) {
+    } else if (k.score == kScoreDense) {
         if (collect_stats) launch(xl_chunk_scores_kernel<true, true, false>);
         else launch(xl_chunk_scores_kernel<true, false, false>);
     } else if (lookup) {
@@ -1302,19 +1350,6 @@ int XLinearEngine::score_layer_(size_t d, const QueryDev& q, uint32_t b_prev, in
     }
     PB200_CUDA(cudaGetLastError());
     ++launches_;
-    layer_profile_[d].scores_kernel = chunk_major ? 4 : query_warp ? 3 : dense ? 2 : lookup ? 1 : 0;
-    return layer_profile_[d].scores_kernel;
-}
-
-// The prefix launch needs the merged image, sparse queries, a layer-0 top-k that keeps every layer-0 node (so that layer 1's
-// beam is all of layer 1, in layer 0's rank order) and enough rows to fill the GPU: a small tile leaves most SMs idle in
-// the one-pass kernel, while the per-layer kernels spread its pairs wider (kernel mode 5 ignores the row count, for tests).
-bool XLinearEngine::use_prefix_(const QueryDev& q, const std::vector<LayerPlan>& plan) const {
-    if (!prefix_.cm_shape.ok || !chunk_major_ || no_prefix_ || q.row_ptr == nullptr || !layers_[0].view.featmap || plan.size() < 2)
-        return false;
-    if (plan[0].k < host_->layers[0].n_cols) return false;
-    if (static_cast<uint64_t>(q.rows) * std::max<uint32_t>(q.max_row_nnz, 1u) >= (1ull << 32)) return false;  // 32-bit feature offsets
-    return cm_force_ || q.rows >= kCmMinPairsPerSm * n_sm_;
 }
 
 void XLinearEngine::launch_prefix_(const QueryDev& q, const std::vector<LayerPlan>& plan, uint32_t ws_row) {
@@ -1353,86 +1388,63 @@ void XLinearEngine::run_tile_(const QueryDev& q, const std::vector<LayerPlan>& p
     int cur = static_cast<int>(d_begin & 1);  // every layer flips the ping-pong beam buffers once
     const size_t depth = plan.size();
     d_end = std::min(d_end, depth);
-    const bool prefix = !ext_beam && d_begin == 0 && d_end >= 2 && combine_first == 0 && !collect_stats && use_prefix_(q, plan);
-    if (!ext_beam && d_begin == 0 && !prefix) {
-        xl_init_beam_kernel<<<(rows + 255) / 256, 256, 0, stream_>>>(bid_(cur, ws_row), bval_(cur, ws_row),
-                                                                     bcnt_(cur, ws_row), beam_stride_, rows);
-        ++launches_;
-    }
+    const TileShape t{ext_beam, combine_first, d_begin, d_end, collect_stats, true};
     for (size_t d = d_begin; d < d_end; ++d) {
-        if (prefix && d == 0) {  // layer 0's scores, beam and layer 1's raw scores: one launch, timed in layer 0's score slot
-            if (profile_) PB200_CUDA(cudaEventRecord(ev_[0], stream_));
-            launch_prefix_(q, plan, ws_row);
-            layer_profile_[0].scores_kernel = 4;
-            if (profile_) {
-                PB200_CUDA(cudaEventRecord(ev_[1], stream_));
-                PB200_CUDA(cudaEventSynchronize(ev_[1]));
-                float a = 0.f;
-                PB200_CUDA(cudaEventElapsedTime(&a, ev_[0], ev_[1]));
-                layer_profile_[0].scores_ms += a;
-                layer_profile_[0].launches += 1;
-            }
-            cur ^= 1;
-            continue;
+        const LayerKernels k = pick_kernels_(d, q, plan, t);
+        if (d == 0 && !ext_beam && !k.prefix) {  // the root beam (the prefix launch writes layer 0's beam itself)
+            xl_init_beam_kernel<<<(rows + 255) / 256, 256, 0, stream_>>>(bid_(cur, ws_row), bval_(cur, ws_row),
+                                                                         bcnt_(cur, ws_row), beam_stride_, rows);
+            ++launches_;
         }
-        const LayerDev& L = layers_[d].view;
-        const LayerPlan& lp = plan[d];
-        const int combine = (d == 0) ? combine_first : 1;
-        const uint32_t c_stride = std::max<uint32_t>(L.c_max, 1u);
-        const uint64_t cand_stride_q = static_cast<uint64_t>(lp.b_prev) * c_stride;
-        const float* cand = cand_.get() + ws_row * cand_stride_q;
-        const uint32_t* bid = bid_(cur, ws_row);
-        const float* bval = bval_(cur, ws_row);
-        const uint32_t* bcnt = bcnt_(cur, ws_row);
-        unsigned long long* stats = collect_stats ? stats_dev_.get() + 8 * d : nullptr;
         if (profile_) PB200_CUDA(cudaEventRecord(ev_[0], stream_));
-        const dim3 grid(rows);
-        const bool scored = prefix && d == 1;  // by the prefix launch
-        if (scored) layer_profile_[1].scores_kernel = 4;
-        else score_layer_(d, q, lp.b_prev, cur, ws_row, collect_stats);
+        score_layer_(d, q, plan, k, cur, ws_row, collect_stats);
         if (profile_) PB200_CUDA(cudaEventRecord(ev_[1], stream_));
-
-        const OutTarget o = (d + 1 == depth) ? out
-                                             : OutTarget{bid_(cur ^ 1, ws_row), bval_(cur ^ 1, ws_row), bcnt_(cur ^ 1, ws_row),
-                                                         nullptr, beam_stride_};
-        const uint64_t sort_stride = next_pow2_host(cand_stride_q);
-        const bool warp_select = !force_block_topk_ && lp.b_prev <= static_cast<uint32_t>(kSelSlots) &&
-                                 cand_stride_q <= static_cast<uint64_t>(kSelKeysMax) && lp.k <= static_cast<uint32_t>(kSelK);
-        const bool hinge = lp.pp.kind == PP_LP_HINGE || lp.pp.kind == PP_LOG_LP_HINGE;
-        const bool filter_select = !force_block_topk_ && !no_topk_filter_ && lp.k <= 32u &&
-                                   lp.b_prev <= static_cast<uint32_t>(kFltSlots) &&
-                                   cand_stride_q <= static_cast<uint64_t>(kFltKeysMax) &&
-                                   (!hinge || (lp.pp.p >= 0 && lp.pp.p <= 4));
-        if (filter_select) {
-            const uint32_t key_cap = static_cast<uint32_t>((cand_stride_q + 127) & ~static_cast<uint64_t>(127));
-            const size_t flt_smem = kFltWarps * flt_warp_bytes(key_cap);
-            xl_topk_filter_kernel<<<(rows + kFltWarps - 1) / kFltWarps, kFltWarps * 32, flt_smem, stream_>>>(
-                L, lp.pp.kind, lp.pp.p, combine, lp.k, bid, bval, bcnt,
-                beam_stride_, cand, cand_stride_q, o.ids, o.vals, o.cnt, o.stride, rows, stats, o.keys, key_cap);
-        } else if (warp_select) {
-            const uint32_t key_cap = static_cast<uint32_t>((cand_stride_q + 31) & ~static_cast<uint64_t>(31));
-            const size_t sel_smem = kSelWarps * ((sel_warp_bytes(key_cap) + 15) & ~static_cast<size_t>(15));
-            xl_topk_warp_kernel<<<(rows + kSelWarps - 1) / kSelWarps, kSelWarps * 32, sel_smem, stream_>>>(
-                L, lp.pp.kind, lp.pp.p, combine, lp.k, bid, bval, bcnt,
-                beam_stride_, cand, cand_stride_q, c_stride, o.ids, o.vals, o.cnt, o.stride, rows, stats, o.keys, key_cap);
-        } else {
-            xl_topk_kernel<<<grid, kTopkThreads, topk_kernel_smem(lp.b_prev), stream_>>>(
-                L, lp.pp.kind, lp.pp.p, combine, lp.k, bid, bval, bcnt,
-                beam_stride_, cand, cand_stride_q, c_stride, o.ids, o.vals, o.cnt, o.stride, sortbuf_.get(), sort_stride,
-                lp.b_prev, stats, o.keys);
+        if (k.topk != kNoTopk) {
+            const LayerDev& L = layers_[d].view;
+            const LayerPlan& lp = plan[d];
+            const int combine = (d == 0) ? combine_first : 1;
+            const uint32_t c_stride = std::max<uint32_t>(L.c_max, 1u);
+            const uint64_t cand_stride_q = static_cast<uint64_t>(lp.b_prev) * c_stride;
+            const float* cand = cand_.get() + ws_row * cand_stride_q;
+            const uint32_t* bid = bid_(cur, ws_row);
+            const float* bval = bval_(cur, ws_row);
+            const uint32_t* bcnt = bcnt_(cur, ws_row);
+            unsigned long long* stats = collect_stats ? stats_dev_.get() + 8 * d : nullptr;
+            const OutTarget o = (d + 1 == depth) ? out
+                                                 : OutTarget{bid_(cur ^ 1, ws_row), bval_(cur ^ 1, ws_row), bcnt_(cur ^ 1, ws_row),
+                                                             nullptr, beam_stride_};
+            if (k.topk == kTopkFilter) {
+                const uint32_t key_cap = static_cast<uint32_t>((cand_stride_q + 127) & ~static_cast<uint64_t>(127));
+                const size_t flt_smem = kFltWarps * flt_warp_bytes(key_cap);
+                xl_topk_filter_kernel<<<(rows + kFltWarps - 1) / kFltWarps, kFltWarps * 32, flt_smem, stream_>>>(
+                    L, lp.pp.kind, lp.pp.p, combine, lp.k, bid, bval, bcnt,
+                    beam_stride_, cand, cand_stride_q, o.ids, o.vals, o.cnt, o.stride, rows, stats, o.keys, key_cap);
+            } else if (k.topk == kTopkWarp) {
+                const uint32_t key_cap = static_cast<uint32_t>((cand_stride_q + 31) & ~static_cast<uint64_t>(31));
+                const size_t sel_smem = kSelWarps * ((sel_warp_bytes(key_cap) + 15) & ~static_cast<size_t>(15));
+                xl_topk_warp_kernel<<<(rows + kSelWarps - 1) / kSelWarps, kSelWarps * 32, sel_smem, stream_>>>(
+                    L, lp.pp.kind, lp.pp.p, combine, lp.k, bid, bval, bcnt,
+                    beam_stride_, cand, cand_stride_q, c_stride, o.ids, o.vals, o.cnt, o.stride, rows, stats, o.keys, key_cap);
+            } else {
+                xl_topk_kernel<<<rows, kTopkThreads, topk_kernel_smem(lp.b_prev), stream_>>>(
+                    L, lp.pp.kind, lp.pp.p, combine, lp.k, bid, bval, bcnt,
+                    beam_stride_, cand, cand_stride_q, c_stride, o.ids, o.vals, o.cnt, o.stride, sortbuf_.get(),
+                    next_pow2_host(cand_stride_q), lp.b_prev, stats, o.keys);
+            }
+            PB200_CUDA(cudaGetLastError());
+            ++launches_;
+            layer_profile_[d].topk_kernel = k.topk;
         }
-        PB200_CUDA(cudaGetLastError());
-        ++launches_;
-        layer_profile_[d].topk_kernel = filter_select ? 2 : warp_select ? 1 : 0;
         if (profile_) {
             PB200_CUDA(cudaEventRecord(ev_[2], stream_));
             PB200_CUDA(cudaEventSynchronize(ev_[2]));
             float a = 0.f, b = 0.f;
             PB200_CUDA(cudaEventElapsedTime(&a, ev_[0], ev_[1]));
             PB200_CUDA(cudaEventElapsedTime(&b, ev_[1], ev_[2]));
-            if (!scored) layer_profile_[d].scores_ms += a;  // the slot stays at 0 ms: the prefix launch is layer 0's
-            layer_profile_[d].topk_ms += b;
-            layer_profile_[d].launches += scored ? 1 : 2;
+            XLinearLayerProfile& p = layer_profile_[d];
+            // under the prefix, layer 1's score slot stays at 0 ms (the launch is layer 0's), and layer 0's top-k slot too
+            if (!(k.prefix && d == 1)) { p.scores_ms += a; ++p.launches; }
+            if (k.topk != kNoTopk) { p.topk_ms += b; ++p.launches; }
         }
         cur ^= 1;
     }
@@ -1907,7 +1919,8 @@ XLinearEngine::SelectedResult XLinearEngine::predict_selected(const HostMatrix& 
                 std::memcpy(ids, (d > 0 ? lists[d - 1].id.data() : codes.col_idx) + b, n * 4);
                 return static_cast<uint32_t>(n);
             });
-            score_layer_(d, qd, plan[d].b_prev, 0, 0, false);
+            const TileShape one_layer{/*ext_beam=*/true, 0, d, d + 1, false, /*topk=*/false};
+            score_layer_(d, qd, plan, pick_kernels_(d, qd, plan, one_layer), 0, 0, false);
             const auto& Ls = lists[d];
             const uint64_t e0 = Ls.ptr[r0], e1 = Ls.ptr[r0 + tr];
             rel_ptr.resize(static_cast<size_t>(tr) + 1);

@@ -152,8 +152,10 @@ public:
     Result sharded_merge_packed(uint32_t world, uint32_t rows, uint32_t stride, uint32_t only_topk, const void* g_rec);
 
     void set_profile(bool on) { profile_ = on; }
-    // kernel selection for A/B runs and cross-checks: modes 0 - 7, listed at the definition; any other value behaves as 1
-    void set_kernel_mode(int mode);
+    // Kernel selection for A/B runs and cross-checks, described at pick_kernels_ (xlinear_engine.cu); any other value behaves as 1.
+    enum class KernelMode : int { kFirstGeneration = 0, kDefault = 1, kNoQueryWarp = 2, kQueryWarpWherever = 3, kNoTopkFilter = 4,
+                                  kChunkMajorWherever = 5, kQueryMajorOnly = 6, kNoPrefix = 7 };
+    void set_kernel_mode(int mode) { mode_ = mode >= 0 && mode <= 7 ? static_cast<KernelMode>(mode) : KernelMode::kDefault; }
     bool has_feature_maps() const;
     // chunk-major image geometry chosen at load time for layer d (d < 0: the prefix image); ok == false: no images
     const CmShape* cm_shape_of(int d) const {
@@ -225,7 +227,17 @@ private:
     uint32_t* bid_(int b, uint32_t row) const { return beam_id_[b].get() + static_cast<uint64_t>(row) * beam_stride_; }
     float* bval_(int b, uint32_t row) const { return beam_val_[b].get() + static_cast<uint64_t>(row) * beam_stride_; }
     uint32_t* bcnt_(int b, uint32_t row) const { return beam_cnt_[b].get() + row; }
-    int score_layer_(size_t d, const QueryDev& q, uint32_t b_prev, int cur, uint32_t ws_row, bool collect_stats);
+    struct TileShape;     // the facts of a call that bear on the choice of kernels (xlinear_engine.cu)
+    struct LayerKernels;  // the kernels chosen for one layer of a tile (xlinear_engine.cu)
+    LayerKernels pick_kernels_(size_t d, const QueryDev& q, const std::vector<LayerPlan>& plan, const TileShape& t) const;
+    // The chunk-major buffers are sized, and the chunk-major score kernel may run, when the mode allows it and EVERY layer
+    // has a feature map: a feature-map budget (PB200_FEATMAP_MB) that drops some layers' maps runs no layer chunk-major.
+    // Letting the layers that kept their maps take it would change which kernel runs; that is for a measured change.
+    bool chunk_major_workspace_() const {
+        return mode_ != KernelMode::kFirstGeneration && mode_ != KernelMode::kQueryMajorOnly && has_feature_maps();
+    }
+    void score_layer_(size_t d, const QueryDev& q, const std::vector<LayerPlan>& plan, const LayerKernels& k, int cur,
+                      uint32_t ws_row, bool collect_stats);
     OutTarget reserve_results_(uint32_t rows, uint32_t stride);
     Result finish_result_(uint32_t rows, uint32_t stride);
 
@@ -279,24 +291,15 @@ private:
     PinnedBuffer<uint32_t> out_cnt_;
 
     bool profile_ = false;
-    bool no_query_warp_ = false;
-    bool force_query_warp_ = false;
-    bool no_topk_filter_ = false;
-    bool chunk_major_ = true;   // chunk-major scoring wherever cm_plan() finds it eligible (kernel mode 6 switches it off)
-    bool cm_force_ = false;     // kernel mode 5
-    bool no_prefix_ = false;    // kernel mode 7
+    KernelMode mode_ = KernelMode::kDefault;
     // Merged one-chunk layer of layers 0 and 1 (build_prefix_layer) and its chunk-major image: scores both layers of a tile
     // in one launch (prefix_.cm_images empty: the model is not eligible)
     LayerStore prefix_;
-    // Whether one prefix launch may replace layer 0 and layer 1's scoring for this tile (the caller checks that the tile
-    // enters at layer 0 with the root beam, runs both layers and collects no statistics).
-    bool use_prefix_(const QueryDev& q, const std::vector<LayerPlan>& plan) const;
     // Layer 0's beam into beam_*_[1] and layer 1's raw scores into its candidate rows, for rows [ws_row, ws_row + q.rows).
     void launch_prefix_(const QueryDev& q, const std::vector<LayerPlan>& plan, uint32_t ws_row);
     uint32_t n_sm_ = 132;
     DeviceBuffer<uint32_t> cm_slot_pos_, cm_count_, cm_claim_, cm_active_, cm_bucket_ptr_, cm_pair_q_, cm_pair_pos_;
     DeviceBuffer<uint64_t> cm_cost_ptr_;
-    bool force_block_topk_ = false;  // A/B switch: first-generation kernels (row-list streaming + block-wide sort)
     std::vector<XLinearLayerProfile> layer_profile_;
     std::vector<XLinearStats> layer_stats_;
     uint64_t launches_ = 0;

@@ -669,6 +669,41 @@ def test_prefix_limits(tmp_path, gpu_clib, have_ref, sizes, prefix):
     mdl.run(X, 10, 10, [7, 5, 6], expect, what=f"prefix {sizes}", profile=True)
 
 
+def test_feature_map_budget_that_drops_only_the_leaf(tmp_path, gpu_clib, have_ref, monkeypatch):
+    """PB200_FEATMAP_MB = 1 at load: a layer's map takes n_chunks x ceil(W rows / 32) x 8 bytes, so with W rows = 16,384
+    layers 0 - 2 (1 / 8 / 128 chunks: 4 + 32 + 512 KB) keep their maps and the leaf (1,024 chunks: 4 MB) loses its own.
+    The chunk-major kernel needs EVERY layer's map, so no layer takes it, not even in mode 5; the prefix launch needs only
+    layers 0 and 1 and still serves them (id 4); the leaf streams row lists.  On a full-budget handle the same batch (sub-tiles
+    of 6,528 rows, above 48 per SM) runs the prefix and chunk-major kernels everywhere.  Both handles return the same bits
+    in every mode."""
+    D = 16383
+    layers = random_tree(531, [8, 128, 1024, 4096], D, 16)
+    folder = _save(str(tmp_path / "m"), layers)
+    X = synth.make_queries(532, 26000, D, 40)
+    sub = np.r_[0:30, X.shape[0] - 10:X.shape[0]]
+    full = _Model(gpu_clib, have_ref, folder, layers)
+    monkeypatch.setenv("PB200_FEATMAP_MB", "1")
+    part = _Model(gpu_clib, have_ref, folder, layers)
+    assert full.c.pb200_xlinear_set_lookup(full.h, 1) == 1
+    assert part.c.pb200_xlinear_set_lookup(part.h, 1) == 0, "the leaf must lose its feature map"
+
+    def expect(table):
+        def check(mode, pp, info):
+            ids, used = info
+            want_scores, want_used = table[mode]
+            assert [s for s, _ in ids] == want_scores, f"mode {mode} {pp}: score kernels {ids}, expected {want_scores}"
+            assert used == want_used, f"mode {mode} {pp}: prefix {'' if used else 'not '}used"
+        return check
+
+    want = full.run(X, 10, 10, [1, 0], expect({1: ([4, 4, 4, 4], True), 0: ([0, 0, 0, 0], False)}),
+                    what="full feature-map budget", sub=sub, profile=True)
+    got = part.run(X, 10, 10, [1, 5, 7, 0],
+                   expect({1: ([4, 4, 1, 0], True), 5: ([4, 4, 1, 0], True), 7: ([1, 1, 1, 0], False), 0: ([0, 0, 0, 0], False)}),
+                   what="leaf without a feature map", sub=sub, f64=False, profile=True)
+    for pp in want:
+        _same_bits(got[pp], want[pp], f"{pp}: leaf without a feature map vs the full budget")
+
+
 # ------------------------------------------------------------------------------------------------ wide beam
 def test_wide_beam_runs_at_the_limit_and_raises_past_it(tmp_path, gpu_clib, have_ref):
     """kXlBeamMaxTopk = 15,701: the block top-k's shared memory (2048 keys + 3 words per beam slot <= 200 KB).  A beam of
