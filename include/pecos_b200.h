@@ -201,7 +201,8 @@ void pb200_host_free(void* ptr);
 /* Overwrite a scratch buffer larger than L2 (50 MB on an H100) so the next timed iteration starts cold. */
 void pb200_l2_flush(void);
 
-/* Device-resident query batch: upload once, run the layers with inputs already in HBM, fetch when wanted. */
+/* Device-resident query batch: upload once, run the layers with inputs already in HBM, fetch when wanted.  The batch and
+ * its results have their own device buffers: host-buffer calls on the same handle in between change neither. */
 void pb200_xlinear_resident_upload_csr(void* ptr, const ScipyCsrF32* input_x);
 /* Returns the device time (ms, CUDA events on the engine's stream) of one pass over the resident batch. */
 double pb200_xlinear_resident_predict(void* ptr, uint32_t overridden_beam_size, const char* overridden_post_processor_str,
@@ -258,7 +259,8 @@ uint64_t pb200_xlinear_model_bytes(void* ptr);
 uint32_t pb200_xlinear_replicas(void* ptr);
 uint32_t pb200_hnsw_replicas(void* model_ptr);
 
-/* HNSW: device-resident query batch, search-kernel time (ms, CUDA events), algorithmic counters of the last search
+/* HNSW: device-resident query batch (its queries and results survive host-buffer calls on the same handle), search-kernel
+ * time (ms, CUDA events), algorithmic counters of the last search
  *   counters out[4] = {distance evaluations, level-0 expansions, upper-level neighbourhood reads, queries}
  *   info     out[8] = {num_node, feat_dim, maxM, maxM0, max_level, init_node, index bytes in HBM, kernel launches} */
 void pb200_hnsw_resident_upload(void* model_ptr, const ScipyDrmF32* pX);

@@ -20,7 +20,8 @@ inline void cuda_check(cudaError_t err, const char* what, const char* file, int 
 }
 #define PB200_CUDA(call) ::pb200::cuda_check((call), #call, __FILE__, __LINE__)
 
-// Owning device buffer (cudaMalloc / cudaFree). Grows geometrically on reserve().
+// Owning device buffer (cudaMalloc / cudaFree).  reserve(n) beyond the capacity frees the allocation and makes a new one of
+// exactly n elements: the address changes and the contents are dropped.
 template <typename T>
 class DeviceBuffer {
 public:

@@ -455,12 +455,12 @@ HnswEngine::~HnswEngine() {
     if (stream_) cudaStreamDestroy(stream_);
 }
 
-uint32_t HnswEngine::per_warp_smem_(uint32_t ef, int stages, uint32_t* nbmax_out) const {
+uint32_t HnswEngine::per_warp_smem_(uint32_t ef, int stages, uint32_t qcap, uint32_t* nbmax_out) const {
     const HnswHostIndex& H = *host_;
     const uint32_t nbmax = ((std::max(H.l0_max_degree, H.l1_max_degree) + 31u) / 32u) * 32u;
     if (nbmax_out) *nbmax_out = nbmax;
     // [staged query | ids | distances | result heap]
-    return warp_smem_bytes(H.sparse, view_.vstride, stages, queries_.qcap(), nbmax * 8 + (ef <= kEfSmemMax ? (ef + 1) * 8 : 0));
+    return warp_smem_bytes(H.sparse, view_.vstride, stages, qcap, nbmax * 8 + (ef <= kEfSmemMax ? (ef + 1) * 8 : 0));
 }
 
 void HnswEngine::set_stages(int stages) {
@@ -471,14 +471,14 @@ void HnswEngine::set_stages(int stages) {
 // One warp's shared-memory slice must fit kWarpSmemMax.  The ring takes stages + 1 rows of 4 * vstride bytes, so wide vectors
 // run the deepest ring that fits: the configured depth, else 8 -> 4 -> 0 (direct loads: one row, dense d up to about 50,000).
 // Results do not depend on the depth.
-void HnswEngine::ensure_scratch_(uint32_t ef) {
+void HnswEngine::ensure_scratch_(uint32_t ef, uint32_t qcap) {
     const HnswHostIndex& H = *host_;
     const bool top_in_smem = ef <= kEfSmemMax;
     int stages = stages_;
-    uint32_t per_warp = per_warp_smem_(ef, stages, nullptr);
+    uint32_t per_warp = per_warp_smem_(ef, stages, qcap, nullptr);
     while (stages > 0 && per_warp > kWarpSmemMax) {
         stages = stages > 4 ? 4 : 0;
-        per_warp = per_warp_smem_(ef, stages, nullptr);
+        per_warp = per_warp_smem_(ef, stages, qcap, nullptr);
     }
     if (per_warp > kWarpSmemMax)
         throw std::runtime_error("pecos_b200: HNSW query dimension too large for the shared-memory staging area, even with "
@@ -515,25 +515,25 @@ void HnswEngine::launch_info(uint64_t* out) const {
     out[4] = topk_heap_.capacity();
 }
 
-double HnswEngine::launch_once_(uint32_t nq, uint32_t efS, uint32_t topk, int idx_fill, bool* overflow) {
+double HnswEngine::launch_once_(const SearchIo& io, uint32_t efS, uint32_t topk, int idx_fill, bool* overflow) {
     const HnswHostIndex& H = *host_;
-    const uint32_t ef = std::max(efS, topk);
+    const uint32_t ef = std::max(efS, topk), nq = io.nq;
     if (ef == 0) throw std::runtime_error("pecos_b200: efS and topk are both zero");
-    ensure_scratch_(ef);
+    ensure_scratch_(ef, io.queries->qcap());
     uint32_t nbmax = 0;
     const bool top_in_smem = ef <= kEfSmemMax;
-    const uint32_t per_warp = per_warp_smem_(ef, run_stages_, &nbmax);
+    const uint32_t per_warp = per_warp_smem_(ef, run_stages_, io.queries->qcap(), &nbmax);
     const uint32_t words = static_cast<uint32_t>((static_cast<uint64_t>(H.num_node) + 31) / 32);
     PB200_CUDA(cudaMemsetAsync(ctrl_.get(), 0, 8 * sizeof(unsigned long long), stream_));
-    PB200_CUDA(cudaMemsetAsync(out_idx_.get(), idx_fill, static_cast<uint64_t>(nq) * topk * 4, stream_));
-    PB200_CUDA(cudaMemsetAsync(out_val_.get(), 0, static_cast<uint64_t>(nq) * topk * 4, stream_));
+    PB200_CUDA(cudaMemsetAsync(io.idx, idx_fill, static_cast<uint64_t>(nq) * topk * 4, stream_));
+    PB200_CUDA(cudaMemsetAsync(io.val, 0, static_cast<uint64_t>(nq) * topk * 4, stream_));
     const uint32_t ctas = std::max<uint32_t>(1, std::min<uint32_t>(n_ctas_, (nq + warps_per_cta_ - 1) / warps_per_cta_));
     const size_t smem = static_cast<size_t>(warps_per_cta_) * per_warp;
-    const float* q_dev = queries_.dense();
-    const HnswSparseQueries sq = queries_.sparse();
+    const float* q_dev = io.queries->dense();
+    const HnswSparseQueries sq = io.queries->sparse();
     PB200_CUDA(cudaEventRecord(ev_[0], stream_));
     auto launch = [&](auto kernel) {
-        kernel<<<ctas, warps_per_cta_ * 32, smem, stream_>>>(view_, q_dev, sq, nq, efS, topk, ef, out_idx_.get(), out_val_.get(),
+        kernel<<<ctas, warps_per_cta_ * 32, smem, stream_>>>(view_, q_dev, sq, nq, efS, topk, ef, io.idx, io.val,
                                                              bitmap_.get(), words, vlist_.get(), cand_.get(), vcap_,
                                                              top_in_smem ? nullptr : topk_heap_.get(), nbmax, per_warp, ctrl_.get());
     };
@@ -560,10 +560,10 @@ double HnswEngine::launch_once_(uint32_t nq, uint32_t efS, uint32_t topk, int id
 // A query whose candidate queue outgrows the per-warp scratch (vcap entries) flags an overflow; the batch is then re-run with
 // twice the capacity (at most num_node + 1 entries, which can never overflow: a node enters the queue at most once), instead
 // of aborting the host process.
-double HnswEngine::launch_(uint32_t nq, uint32_t efS, uint32_t topk, int idx_fill) {
+double HnswEngine::launch_(const SearchIo& io, uint32_t efS, uint32_t topk, int idx_fill) {
     for (;;) {
         bool overflow = false;
-        const double ms = launch_once_(nq, efS, topk, idx_fill, &overflow);
+        const double ms = launch_once_(io, efS, topk, idx_fill, &overflow);
         if (!overflow) return ms;
         const uint64_t cap_max = static_cast<uint64_t>(host_->num_node) + 1;
         if (vcap_ >= cap_max) throw std::runtime_error("pecos_b200: HNSW candidate queue overflow at full capacity (internal error)");
@@ -573,24 +573,22 @@ double HnswEngine::launch_(uint32_t nq, uint32_t efS, uint32_t topk, int idx_fil
 }
 
 
-bool HnswEngine::upload_(const HostMatrix& x, uint32_t topk) {
+bool HnswEngine::upload_(const HostMatrix& x, uint32_t topk, DeviceQueries& into) {
     PB200_CUDA(cudaSetDevice(device_));
     if (host_->sparse && !x.row_ptr) throw std::runtime_error("pecos_b200: dense queries against a sparse (csr) HNSW index");
     if (!host_->sparse && x.row_ptr) throw std::runtime_error("pecos_b200: csr queries against a dense HNSW index");
     if (x.cols != host_->feat_dim) throw std::runtime_error("pecos_b200: query dimension != index dimension");
     if (x.rows == 0 || topk == 0) return false;
-    const uint32_t qcap = queries_.qcap();
-    queries_.upload(x, x.rows, stream_);
-    if (queries_.qcap() != qcap) n_warps_ = 0;  // launch geometry depends on the staging capacity
+    into.upload(x, x.rows, stream_);
     return true;
 }
 
 void HnswEngine::predict(const HostMatrix& x, uint32_t efS, uint32_t topk, uint32_t* ret_idx, float* ret_val) {
-    if (!upload_(x, topk)) return;
+    if (!upload_(x, topk, queries_)) return;
     const uint64_t n = static_cast<uint64_t>(x.rows) * topk;
     out_idx_.reserve(n);
     out_val_.reserve(n);
-    launch_(x.rows, efS, topk);
+    launch_({&queries_, x.rows, out_idx_.get(), out_val_.get()}, efS, topk);
     // rows with fewer than topk results keep the caller's zeros (libpecos.cpp:554-558): our buffers were zeroed too
     PB200_CUDA(cudaMemcpyAsync(ret_idx, out_idx_.get(), n * 4, cudaMemcpyDeviceToHost, stream_));
     PB200_CUDA(cudaMemcpyAsync(ret_val, out_val_.get(), n * 4, cudaMemcpyDeviceToHost, stream_));
@@ -598,34 +596,35 @@ void HnswEngine::predict(const HostMatrix& x, uint32_t efS, uint32_t topk, uint3
 }
 
 void HnswEngine::resident_upload(const HostMatrix& x) {
-    upload_(x, 1);  // searched later with resident_predict's topk
+    res_nq_ = 0;
+    upload_(x, 1, res_queries_);  // searched later with resident_predict's topk
     res_nq_ = x.rows;
 }
 
 double HnswEngine::resident_predict(uint32_t efS, uint32_t topk) {
     PB200_CUDA(cudaSetDevice(device_));
     if (!res_nq_) throw std::runtime_error("pecos_b200: no resident query batch uploaded");
-    out_idx_.reserve(static_cast<uint64_t>(res_nq_) * topk);
-    out_val_.reserve(static_cast<uint64_t>(res_nq_) * topk);
+    res_idx_.reserve(static_cast<uint64_t>(res_nq_) * topk);
+    res_val_.reserve(static_cast<uint64_t>(res_nq_) * topk);
     res_topk_ = topk;
-    return launch_(res_nq_, efS, topk);
+    return launch_({&res_queries_, res_nq_, res_idx_.get(), res_val_.get()}, efS, topk);
 }
 
 void HnswEngine::resident_fetch(uint32_t* ret_idx, float* ret_val) {
     PB200_CUDA(cudaSetDevice(device_));
-    PB200_CUDA(cudaMemcpy(ret_idx, out_idx_.get(), static_cast<uint64_t>(res_nq_) * res_topk_ * 4, cudaMemcpyDeviceToHost));
-    PB200_CUDA(cudaMemcpy(ret_val, out_val_.get(), static_cast<uint64_t>(res_nq_) * res_topk_ * 4, cudaMemcpyDeviceToHost));
+    PB200_CUDA(cudaMemcpy(ret_idx, res_idx_.get(), static_cast<uint64_t>(res_nq_) * res_topk_ * 4, cudaMemcpyDeviceToHost));
+    PB200_CUDA(cudaMemcpy(ret_val, res_val_.get(), static_cast<uint64_t>(res_nq_) * res_topk_ * 4, cudaMemcpyDeviceToHost));
 }
 
 // search into out_idx_ / out_val_ (empty slots 0xFFFFFFFF), then pack the records into the caller's device buffer
 void HnswEngine::sharded_local_packed(const HostMatrix& x, uint32_t efS, uint32_t topk, uint32_t rank, uint32_t id_offset,
                                       void* rec_dev) {
     check_shard_slots(rank, topk);
-    if (!upload_(x, topk)) return;
+    if (!upload_(x, topk, queries_)) return;
     const uint64_t n = static_cast<uint64_t>(x.rows) * topk;
     out_idx_.reserve(n);
     out_val_.reserve(n);
-    launch_(x.rows, efS, topk, 0xFF);
+    launch_({&queries_, x.rows, out_idx_.get(), out_val_.get()}, efS, topk, 0xFF);
     hnsw_shard_pack_kernel<<<static_cast<uint32_t>((n + 255) / 256), 256, 0, stream_>>>(out_idx_.get(), out_val_.get(), n, topk, rank,
                                                                                       id_offset, static_cast<ShardRecord*>(rec_dev));
     PB200_CUDA(cudaGetLastError());

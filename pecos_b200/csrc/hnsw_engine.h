@@ -133,15 +133,22 @@ public:
     void launch_info(uint64_t* out) const;
 
 private:
-    // selects the device, checks x against the index and uploads it, unless there is nothing to search (no rows or topk 0):
-    // returns whether it did
-    bool upload_(const HostMatrix& x, uint32_t topk);
-    void ensure_scratch_(uint32_t ef);
-    uint32_t per_warp_smem_(uint32_t ef, int stages, uint32_t* nbmax_out) const;
-    // idx_fill: byte value out_idx_ is filled with before the search (0: the reference's zeros; 0xFF: empty slots read
+    // selects the device, checks x against the index and uploads it into `into`, unless there is nothing to search (no rows
+    // or topk 0): returns whether it did
+    bool upload_(const HostMatrix& x, uint32_t topk, DeviceQueries& into);
+    // the launch geometry follows the staging capacity qcap of the queries searched
+    void ensure_scratch_(uint32_t ef, uint32_t qcap);
+    uint32_t per_warp_smem_(uint32_t ef, int stages, uint32_t qcap, uint32_t* nbmax_out) const;
+    struct SearchIo {  // the first nq rows of *queries, searched into idx / val ([nq][topk])
+        const DeviceQueries* queries;
+        uint32_t nq;
+        uint32_t* idx;
+        float* val;
+    };
+    // idx_fill: byte value io.idx is filled with before the search (0: the reference's zeros; 0xFF: empty slots read
     // 0xFFFFFFFF, which no node id can be, for the shard pack kernel)
-    double launch_(uint32_t nq, uint32_t efS, uint32_t topk, int idx_fill = 0);
-    double launch_once_(uint32_t nq, uint32_t efS, uint32_t topk, int idx_fill, bool* overflow);
+    double launch_(const SearchIo& io, uint32_t efS, uint32_t topk, int idx_fill = 0);
+    double launch_once_(const SearchIo& io, uint32_t efS, uint32_t topk, int idx_fill, bool* overflow);
 
     std::unique_ptr<HnswHostIndex> host_;
     int device_ = 0;
@@ -166,10 +173,14 @@ private:
     DeviceBuffer<uint2> topk_heap_;
     DeviceBuffer<unsigned long long> ctrl_;  // [0] query counter, [1] error flag, [2..5] counters
 
-    DeviceQueries queries_;
+    DeviceQueries queries_;  // host-buffer calls
     DeviceBuffer<uint32_t> out_idx_;
     DeviceBuffer<float> out_val_;
     DeviceBuffer<uint32_t> merge_cnt_;  // per-query result counts of the shard merge
+    // the resident batch owns its queries and results: host-buffer calls in between change neither
+    DeviceQueries res_queries_;
+    DeviceBuffer<uint32_t> res_idx_;
+    DeviceBuffer<float> res_val_;
     uint32_t res_nq_ = 0, res_topk_ = 0;
 
     uint64_t launches_ = 0;

@@ -933,8 +933,10 @@ XLinearEngine::XLinearEngine(std::unique_ptr<XLinearHostModel> host, int device)
     PB200_CUDA(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
     for (auto& e : ev_) PB200_CUDA(cudaEventCreate(&e));
     PB200_CUDA(cudaStreamCreateWithFlags(&copy_stream_, cudaStreamNonBlocking));
-    for (auto& e : up_ev_) PB200_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    for (auto& e : use_ev_) PB200_CUDA(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+    for (auto& s : stage_) {
+        PB200_CUDA(cudaEventCreateWithFlags(&s.landed, cudaEventDisableTiming));
+        PB200_CUDA(cudaEventCreateWithFlags(&s.consumed, cudaEventDisableTiming));
+    }
     layers_.resize(host_->layers.size());
     uint64_t cmimg_budget = 8ull << 30;     // bytes of HBM the chunk images of the chunk-major kernel may take in total
     if (const char* env = std::getenv("PB200_CMIMG_MB")) cmimg_budget = std::strtoull(env, nullptr, 10) << 20;
@@ -1120,8 +1122,7 @@ XLinearEngine::~XLinearEngine() {
     if (stream_) cudaStreamSynchronize(stream_);
     for (auto& e : ev_) if (e) cudaEventDestroy(e);
     if (copy_stream_) cudaStreamSynchronize(copy_stream_);
-    for (auto& e : up_ev_) if (e) cudaEventDestroy(e);
-    for (auto& e : use_ev_) if (e) cudaEventDestroy(e);
+    for (auto& s : stage_) for (cudaEvent_t e : {s.landed, s.consumed}) if (e) cudaEventDestroy(e);
     if (copy_stream_) cudaStreamDestroy(copy_stream_);
     if (stream_) cudaStreamDestroy(stream_);
 }
@@ -1450,14 +1451,14 @@ void XLinearEngine::run_tile_(const QueryDev& q, const std::vector<LayerPlan>& p
     }
 }
 
-XLinearEngine::Result XLinearEngine::finish_result_(uint32_t rows, uint32_t stride) {
+XLinearEngine::Result XLinearEngine::finish_result_(const ResultBuffers& res, uint32_t rows, uint32_t stride) {
     out_ids_.reserve(static_cast<uint64_t>(rows) * stride + 1);
     out_vals_.reserve(static_cast<uint64_t>(rows) * stride + 1);
     out_cnt_.reserve(static_cast<uint64_t>(rows) + 1);
     if (rows) {
-        PB200_CUDA(cudaMemcpyAsync(out_ids_.get(), res_ids_dev_.get(), static_cast<uint64_t>(rows) * stride * 4, cudaMemcpyDeviceToHost, stream_));
-        PB200_CUDA(cudaMemcpyAsync(out_vals_.get(), res_vals_dev_.get(), static_cast<uint64_t>(rows) * stride * 4, cudaMemcpyDeviceToHost, stream_));
-        PB200_CUDA(cudaMemcpyAsync(out_cnt_.get(), res_cnt_dev_.get(), static_cast<uint64_t>(rows) * 4, cudaMemcpyDeviceToHost, stream_));
+        PB200_CUDA(cudaMemcpyAsync(out_ids_.get(), res.ids.get(), static_cast<uint64_t>(rows) * stride * 4, cudaMemcpyDeviceToHost, stream_));
+        PB200_CUDA(cudaMemcpyAsync(out_vals_.get(), res.vals.get(), static_cast<uint64_t>(rows) * stride * 4, cudaMemcpyDeviceToHost, stream_));
+        PB200_CUDA(cudaMemcpyAsync(out_cnt_.get(), res.cnt.get(), static_cast<uint64_t>(rows) * 4, cudaMemcpyDeviceToHost, stream_));
     }
     PB200_CUDA(cudaStreamSynchronize(stream_));
     Result r;
@@ -1470,33 +1471,92 @@ XLinearEngine::Result XLinearEngine::finish_result_(uint32_t rows, uint32_t stri
     return r;
 }
 
-XLinearEngine::OutTarget XLinearEngine::reserve_results_(uint32_t rows, uint32_t stride) {
-    res_ids_dev_.reserve(static_cast<uint64_t>(rows) * stride + 1);
-    res_vals_dev_.reserve(static_cast<uint64_t>(rows) * stride + 1);
-    res_cnt_dev_.reserve(static_cast<uint64_t>(rows) + 1);
-    return OutTarget{res_ids_dev_.get(), res_vals_dev_.get(), res_cnt_dev_.get(), nullptr, stride};
+XLinearEngine::OutTarget XLinearEngine::reserve_results_(ResultBuffers& res, uint32_t rows, uint32_t stride) {
+    res.ids.reserve(static_cast<uint64_t>(rows) * stride + 1);
+    res.vals.reserve(static_cast<uint64_t>(rows) * stride + 1);
+    res.cnt.reserve(static_cast<uint64_t>(rows) + 1);
+    return OutTarget{res.ids.get(), res.vals.get(), res.cnt.get(), nullptr, stride};
 }
 
-void XLinearEngine::for_each_tile_(uint32_t tile, const HostMatrix* x, const TileFn& run) {
-    const uint32_t rows = x ? x->rows : resident_.rows;
-    for (uint32_t r0 = 0; r0 < rows; r0 += tile) {
-        const uint32_t tr = std::min(tile, rows - r0);
-        QueryDev q = resident_;
-        if (!x) {
-            q.row_ptr = resident_.row_ptr + r0;
-            q.rows = tr;
-        } else if (x->dense) {
-            x_val_.upload(x->dense + static_cast<uint64_t>(r0) * x->cols, static_cast<uint64_t>(tr) * x->cols, stream_);
-            q = QueryDev{nullptr, nullptr, x_val_.get(), 0, tr, x->cols, x->cols};
-        } else {
-            const uint64_t base = x->row_ptr[r0], end = x->row_ptr[r0 + tr];
-            x_row_ptr_.upload(x->row_ptr + r0, static_cast<uint64_t>(tr) + 1, stream_);
-            x_col_idx_.upload(x->col_idx + base, end - base, stream_);
-            x_val_.upload(x->val + base, end - base, stream_);
-            q = QueryDev{x_row_ptr_.get(), x_col_idx_.get(), x_val_.get(), base, tr, x->cols, max_row_nnz(x->row_ptr + r0, tr)};
-        }
-        run(q, r0);
+void XLinearEngine::QueryStage::reserve(const HostMatrix& x, uint32_t rows, uint64_t n) {
+    if (!x.dense) {
+        row_ptr.reserve(static_cast<uint64_t>(rows) + 1);
+        col_idx.reserve(n);
     }
+    val.reserve(n);
+}
+
+QueryDev XLinearEngine::QueryStage::place(const HostMatrix& x, uint32_t first, uint32_t r0, uint32_t tr, cudaStream_t stream) {
+    if (x.dense) {
+        const uint64_t n = static_cast<uint64_t>(tr) * x.cols;
+        if (n) PB200_CUDA(cudaMemcpyAsync(val.get() + static_cast<uint64_t>(r0 - first) * x.cols, x.dense + static_cast<uint64_t>(r0) * x.cols,
+                                          n * 4, cudaMemcpyHostToDevice, stream));
+    } else {
+        const uint64_t base = x.row_ptr[first], b = x.row_ptr[r0] - base, n = x.row_ptr[r0 + tr] - base - b;
+        PB200_CUDA(cudaMemcpyAsync(row_ptr.get() + (r0 - first), x.row_ptr + r0, (static_cast<uint64_t>(tr) + 1) * 8, cudaMemcpyHostToDevice, stream));
+        if (n) {
+            PB200_CUDA(cudaMemcpyAsync(col_idx.get() + b, x.col_idx + base + b, n * 4, cudaMemcpyHostToDevice, stream));
+            PB200_CUDA(cudaMemcpyAsync(val.get() + b, x.val + base + b, n * 4, cudaMemcpyHostToDevice, stream));
+        }
+    }
+    return view(x, first, r0, tr);
+}
+
+QueryDev XLinearEngine::QueryStage::view(const HostMatrix& x, uint32_t first, uint32_t r0, uint32_t tr) const {
+    if (x.dense) return QueryDev{nullptr, nullptr, val.get() + static_cast<uint64_t>(r0 - first) * x.cols, 0, tr, x.cols, x.cols};
+    return QueryDev{row_ptr.get() + (r0 - first), col_idx.get(), val.get(), x.row_ptr[first], tr, x.cols, max_row_nnz(x.row_ptr + r0, tr)};
+}
+
+// Dense queries are staged tile by tile on the compute stream.  A CSR batch is cut into sub-tiles of `tile` rows or, with
+// split (predict), of about a quarter of a batch of >= 4096 rows (at least 1024 rows, at most `tile`), and staged by one of
+// three schedules:
+//  - whole batch (split, >= 4096 rows, all of them in one tile: predict's common case): the sub-tiles are uploaded on the
+//    copy stream into ONE staging set; the UPPER layers (cheap) run per sub-tile as it lands, overlapping the rest of the
+//    upload, and the LAST layer -- where the time goes, and where the chunk-major kernel wants as many pairs per launch as
+//    it can get -- runs once over the whole batch;
+//  - several sub-tiles: they alternate between the two staging sets on the copy stream, the upload of one overlapping the
+//    scoring of the previous one;
+//  - one sub-tile: one staging set on the compute stream.
+void XLinearEngine::for_each_tile_(uint32_t tile, const HostMatrix* x, const TileFn& run, bool split) {
+    const size_t all = layers_.size();
+    if (!x) {
+        for (uint32_t r0 = 0; r0 < resident_.rows; r0 += tile) {
+            QueryDev q = resident_;
+            q.row_ptr += r0;
+            q.rows = std::min(tile, resident_.rows - r0);
+            run(Tile{q, r0, 0, 0, all});
+        }
+        return;
+    }
+    const uint32_t rows = x->rows, part = ((rows + 3u) / 4u + 31u) & ~31u;
+    split = split && !x->dense && rows >= 4096u;
+    const bool whole = split && tile >= rows;
+    const uint32_t sub = whole ? part : split ? std::min(tile, std::max<uint32_t>(1024u, part)) : tile;
+    const bool overlap = !x->dense && rows > sub;
+    // room for the largest sub-tile (whole batch: for all of it) before the pipeline starts: a reallocation synchronises
+    const uint32_t span = whole ? rows : sub;
+    uint64_t n_max = 0;
+    for (uint32_t r0 = 0; r0 < rows; r0 += span) {
+        const uint32_t tr = std::min(span, rows - r0);
+        n_max = std::max(n_max, x->dense ? static_cast<uint64_t>(tr) * x->cols : x->row_ptr[r0 + tr] - x->row_ptr[r0]);
+    }
+    for (int b = 0; b < (overlap && !whole ? 2 : 1); ++b) stage_[b].reserve(*x, span, n_max);
+    uint32_t t = 0;
+    for (uint32_t r0 = 0; r0 < rows; r0 += sub, ++t) {
+        const uint32_t tr = std::min(sub, rows - r0);
+        QueryStage& s = stage_[overlap && !whole ? t & 1u : 0u];
+        if (!overlap) {
+            run(Tile{s.place(*x, r0, r0, tr, stream_), r0, 0, 0, all});
+            continue;
+        }
+        if (!whole && t >= 2) PB200_CUDA(cudaStreamWaitEvent(copy_stream_, s.consumed, 0));
+        const QueryDev q = s.place(*x, whole ? 0 : r0, r0, tr, copy_stream_);
+        PB200_CUDA(cudaEventRecord(s.landed, copy_stream_));
+        PB200_CUDA(cudaStreamWaitEvent(stream_, s.landed, 0));
+        run(whole ? Tile{q, r0, r0, 0, all - 1} : Tile{q, r0, 0, 0, all});
+        if (!whole) PB200_CUDA(cudaEventRecord(s.consumed, stream_));
+    }
+    if (whole) run(Tile{stage_[0].view(*x, 0, 0, rows), 0, 0, all - 1, all});
 }
 
 void XLinearEngine::stage_beam_(uint32_t rows, bool with_vals, const BeamFn& fill) {
@@ -1517,89 +1577,12 @@ void XLinearEngine::stage_beam_(uint32_t rows, bool with_vals, const BeamFn& fil
 XLinearEngine::Result XLinearEngine::predict(const HostMatrix& x, uint32_t beam_size, const char* post_processor, uint32_t only_topk) {
     PB200_CUDA(cudaSetDevice(device_));
     const auto plan = make_plan_(beam_size, post_processor, only_topk);
-    const uint32_t rows = x.rows, cols = x.cols, stride = plan.back().k_cap;
-    const OutTarget out = reserve_results_(rows, stride);
-    if (x.dense) {
-        for_each_tile_(ensure_workspace_(plan, rows, cols), &x,
-                       [&](const QueryDev& q, uint32_t r0) { run_tile_(q, plan, out.at(r0)); });
-        return finish_result_(rows, stride);
-    }
-    // CSR: the uploads overlap the scoring.  Batches of >= 4096 rows are cut into sub-tiles of about a quarter of the batch.
-    const uint64_t* row_ptr = x.row_ptr;
-    const uint32_t* col_idx = x.col_idx;
-    const float* val = x.val;
-    const uint32_t tile = ensure_workspace_(plan, rows, 0);
-    const uint32_t part = ((rows + 3u) / 4u + 31u) & ~31u;
-    // Whole batch fits the workspace (the common case): the sub-tiles are uploaded on the copy stream into ONE staging set;
-    // the UPPER layers (cheap) run per sub-tile as it lands, overlapping the rest of the upload, and the LAST layer -- where
-    // the time goes, and where the chunk-major kernel wants as many pairs per launch as it can get -- runs once over the
-    // whole batch.
-    if (rows >= 4096u && tile >= rows) {
-        const size_t depth = plan.size();
-        const uint64_t nnz0 = row_ptr[0], nnz = row_ptr[rows] - nnz0;
-        x_row_ptr_.reserve(static_cast<uint64_t>(rows) + 1);
-        x_col_idx_.reserve(nnz);
-        x_val_.reserve(nnz);
-        std::vector<cudaEvent_t> evs;
-        for (uint32_t r0 = 0; r0 < rows; r0 += part) {
-            const uint32_t tr = std::min(part, rows - r0);
-            const uint64_t b = row_ptr[r0] - nnz0, e = row_ptr[r0 + tr] - nnz0;
-            PB200_CUDA(cudaMemcpyAsync(x_row_ptr_.get() + r0, row_ptr + r0, (static_cast<uint64_t>(tr) + 1) * 8, cudaMemcpyHostToDevice, copy_stream_));
-            PB200_CUDA(cudaMemcpyAsync(x_col_idx_.get() + b, col_idx + nnz0 + b, (e - b) * 4, cudaMemcpyHostToDevice, copy_stream_));
-            PB200_CUDA(cudaMemcpyAsync(x_val_.get() + b, val + nnz0 + b, (e - b) * 4, cudaMemcpyHostToDevice, copy_stream_));
-            cudaEvent_t ev;
-            PB200_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-            PB200_CUDA(cudaEventRecord(ev, copy_stream_));
-            evs.push_back(ev);
-        }
-        size_t t = 0;
-        for (uint32_t r0 = 0; r0 < rows; r0 += part, ++t) {
-            const uint32_t tr = std::min(part, rows - r0);
-            PB200_CUDA(cudaStreamWaitEvent(stream_, evs[t], 0));
-            if (depth > 1) {
-                QueryDev q{x_row_ptr_.get() + r0, x_col_idx_.get(), x_val_.get(), nnz0, tr, cols, max_row_nnz(row_ptr + r0, tr)};
-                run_tile_(q, plan, out.at(r0), r0, false, false, 0, 0, depth - 1);
-            }
-        }
-        QueryDev q{x_row_ptr_.get(), x_col_idx_.get(), x_val_.get(), nnz0, rows, cols, max_row_nnz(row_ptr, rows)};
-        run_tile_(q, plan, out, 0, false, false, 0, depth - 1, depth);
-        Result r = finish_result_(rows, stride);
-        for (auto ev : evs) cudaEventDestroy(ev);
-        return r;
-    }
-    // Otherwise the sub-tiles' uploads (copy stream, two staging sets) overlap the scoring of the previous sub-tile; results
-    // stay on the device until the last sub-tile is done.
-    const uint32_t sub = rows >= 4096u ? std::min(tile, std::max<uint32_t>(1024u, part)) : tile;
-    uint64_t max_nnz = 0;
-    for (uint32_t r0 = 0; r0 < rows; r0 += sub) max_nnz = std::max(max_nnz, row_ptr[r0 + std::min(sub, rows - r0)] - row_ptr[r0]);
-    DeviceBuffer<uint64_t>* s_rp[2] = {&x_row_ptr_, &x2_row_ptr_};
-    DeviceBuffer<uint32_t>* s_ci[2] = {&x_col_idx_, &x2_col_idx_};
-    DeviceBuffer<float>* s_va[2] = {&x_val_, &x2_val_};
-    const bool two_sets = rows > sub;
-    for (int b = 0; b < (two_sets ? 2 : 1); ++b) {  // no (synchronising) reallocation inside the pipeline
-        s_rp[b]->reserve(static_cast<uint64_t>(sub) + 1);
-        s_ci[b]->reserve(max_nnz);
-        s_va[b]->reserve(max_nnz);
-    }
-    uint32_t t = 0;
-    for (uint32_t r0 = 0; r0 < rows; r0 += sub, ++t) {
-        const uint32_t tr = std::min(sub, rows - r0);
-        const uint64_t base = row_ptr[r0], end = row_ptr[r0 + tr];
-        const int b = two_sets ? static_cast<int>(t & 1u) : 0;
-        cudaStream_t up = two_sets ? copy_stream_ : stream_;
-        if (two_sets && t >= 2) PB200_CUDA(cudaStreamWaitEvent(copy_stream_, use_ev_[b], 0));
-        s_rp[b]->upload(row_ptr + r0, static_cast<uint64_t>(tr) + 1, up);
-        s_ci[b]->upload(col_idx + base, end - base, up);
-        s_va[b]->upload(val + base, end - base, up);
-        if (two_sets) {
-            PB200_CUDA(cudaEventRecord(up_ev_[b], copy_stream_));
-            PB200_CUDA(cudaStreamWaitEvent(stream_, up_ev_[b], 0));
-        }
-        QueryDev q{s_rp[b]->get(), s_ci[b]->get(), s_va[b]->get(), base, tr, cols, max_row_nnz(row_ptr + r0, tr)};
-        run_tile_(q, plan, out.at(r0));
-        if (two_sets) PB200_CUDA(cudaEventRecord(use_ev_[b], stream_));
-    }
-    return finish_result_(rows, stride);
+    const uint32_t rows = x.rows, stride = plan.back().k_cap;
+    const OutTarget out = reserve_results_(results_, rows, stride);
+    for_each_tile_(ensure_workspace_(plan, rows, x.dense ? x.cols : 0u), &x, [&](const Tile& t) {
+        run_tile_(t.q, plan, out.at(t.r0), t.ws_row, false, false, 0, t.d_begin, t.d_end);
+    }, /*split=*/true);
+    return finish_result_(results_, rows, stride);
 }
 
 XLinearEngine::Result XLinearEngine::predict_single_layer(const HostMatrix& x, const HostMatrix& codes, const char* post_processor,
@@ -1622,13 +1605,14 @@ XLinearEngine::Result XLinearEngine::predict_single_layer(const HostMatrix& x, c
     // only_topk_to_use = overridden > 0 ? overridden : metadata.only_topk, both = this argument
     const auto plan = make_plan_(0, post_processor, only_topk, {b_prev});
     const uint32_t stride = plan[0].k_cap;
-    const OutTarget out = reserve_results_(rows, stride);
+    const OutTarget out = reserve_results_(results_, rows, stride);
     if (only_topk == 0) {  // sorted_csr keeps min(nnz, 0) entries per row (inference.hpp:1237)
-        if (rows) PB200_CUDA(cudaMemsetAsync(res_cnt_dev_.get(), 0, static_cast<uint64_t>(rows) * 4, stream_));
-        return finish_result_(rows, stride);
+        if (rows) PB200_CUDA(cudaMemsetAsync(out.cnt, 0, static_cast<uint64_t>(rows) * 4, stream_));
+        return finish_result_(results_, rows, stride);
     }
-    for_each_tile_(ensure_workspace_(plan, rows, x.dense ? x.cols : 0u), &x, [&](const QueryDev& q, uint32_t r0) {
-        stage_beam_(q.rows, true, [&](uint32_t r, uint32_t* ids, float* vals) {
+    for_each_tile_(ensure_workspace_(plan, rows, x.dense ? x.cols : 0u), &x, [&](const Tile& t) {
+        const uint32_t r0 = t.r0;
+        stage_beam_(t.q.rows, true, [&](uint32_t r, uint32_t* ids, float* vals) {
             if (have_codes) {
                 const uint64_t b = codes.row_ptr[r0 + r], e = codes.row_ptr[r0 + r + 1];
                 std::memcpy(ids, codes.col_idx + b, (e - b) * 4);
@@ -1638,19 +1622,17 @@ XLinearEngine::Result XLinearEngine::predict_single_layer(const HostMatrix& x, c
             for (uint32_t j = 0; j < HL.n_chunks; ++j) { ids[j] = j; vals[j] = 1.0f; }
             return HL.n_chunks;
         });
-        run_tile_(q, plan, out.at(r0), 0, false, /*ext_beam=*/true, /*combine_first=*/have_codes ? 1 : 0);
+        run_tile_(t.q, plan, out.at(r0), 0, false, /*ext_beam=*/true, /*combine_first=*/have_codes ? 1 : 0);
     });
-    return finish_result_(rows, stride);
+    return finish_result_(results_, rows, stride);
 }
 
 void XLinearEngine::resident_upload_csr(const HostMatrix& x) {
     PB200_CUDA(cudaSetDevice(device_));
-    const uint64_t nnz = x.row_ptr[x.rows];
-    x_row_ptr_.upload(x.row_ptr, static_cast<uint64_t>(x.rows) + 1, stream_);
-    x_col_idx_.upload(x.col_idx, nnz, stream_);
-    x_val_.upload(x.val, nnz, stream_);
+    has_resident_ = false;
+    resident_stage_.reserve(x, x.rows, x.row_ptr[x.rows] - x.row_ptr[0]);
+    resident_ = resident_stage_.place(x, 0, 0, x.rows, stream_);
     PB200_CUDA(cudaStreamSynchronize(stream_));
-    resident_ = QueryDev{x_row_ptr_.get(), x_col_idx_.get(), x_val_.get(), 0, x.rows, x.cols, max_row_nnz(x.row_ptr, x.rows)};
     has_resident_ = true;
 }
 
@@ -1659,13 +1641,13 @@ double XLinearEngine::resident_predict(uint32_t beam_size, const char* post_proc
     PB200_CUDA(cudaSetDevice(device_));
     const auto plan = make_plan_(beam_size, post_processor, only_topk);
     resident_stride_ = plan.back().k_cap;
-    const OutTarget out = reserve_results_(resident_.rows, resident_stride_);
+    const OutTarget out = reserve_results_(resident_results_, resident_.rows, resident_stride_);
     const uint32_t tile = ensure_workspace_(plan, resident_.rows, 0);
     if (collect_stats) PB200_CUDA(cudaMemsetAsync(stats_dev_.get(), 0, stats_dev_.bytes(), stream_));
     PB200_CUDA(cudaEventRecord(ev_[3], stream_));
     cudaEvent_t stop;
     PB200_CUDA(cudaEventCreate(&stop));
-    for_each_tile_(tile, nullptr, [&](const QueryDev& q, uint32_t r0) { run_tile_(q, plan, out.at(r0), 0, collect_stats); });
+    for_each_tile_(tile, nullptr, [&](const Tile& t) { run_tile_(t.q, plan, out.at(t.r0), 0, collect_stats); });
     PB200_CUDA(cudaEventRecord(stop, stream_));
     PB200_CUDA(cudaEventSynchronize(stop));
     float ms = 0.f;
@@ -1696,8 +1678,7 @@ uint32_t XLinearEngine::sharded_local_csr_packed(const HostMatrix& x, uint32_t b
     shard_vals_.reserve(n + 1);
     shard_cnt_.reserve(static_cast<uint64_t>(rows) + 1);
     const OutTarget out{shard_ids_.get(), shard_vals_.get(), shard_cnt_.get(), shard_keys_.get(), stride};
-    for_each_tile_(ensure_workspace_(plan, rows, 0), &x,
-                   [&](const QueryDev& q, uint32_t r0) { run_tile_(q, plan, out.at(r0)); });
+    for_each_tile_(ensure_workspace_(plan, rows, 0), &x, [&](const Tile& t) { run_tile_(t.q, plan, out.at(t.r0)); });
     if (n) {
         xl_shard_pack_kernel<<<static_cast<uint32_t>((n + 255) / 256), 256, 0, stream_>>>(
             shard_keys_.get(), shard_ids_.get(), shard_vals_.get(), shard_cnt_.get(), rows, stride, static_cast<ShardRecord*>(rec_dev));
@@ -1715,19 +1696,19 @@ XLinearEngine::Result XLinearEngine::sharded_merge_packed(uint32_t world, uint32
         throw std::runtime_error("pecos_b200: world * top-k exceeds the merge kernel's capacity");
     const uint32_t k = only_topk ? only_topk : static_cast<uint32_t>(host_->layers.back().only_topk);
     const uint32_t k_out = std::min<uint32_t>(k, world * stride);
-    const OutTarget out = reserve_results_(rows, k_out);
+    const OutTarget out = reserve_results_(results_, rows, k_out);
     if (rows) {
         shard_merge_packed_kernel<<<(rows + kSelWarps - 1) / kSelWarps, kSelWarps * 32, 0, stream_>>>(
             static_cast<const ShardRecord*>(g_rec), world, rows, stride, k_out, out.ids, out.vals, out.cnt);
         PB200_CUDA(cudaGetLastError());
         ++launches_;
     }
-    return finish_result_(rows, k_out);
+    return finish_result_(results_, rows, k_out);
 }
 
 XLinearEngine::Result XLinearEngine::resident_fetch() {
     PB200_CUDA(cudaSetDevice(device_));
-    return finish_result_(resident_.rows, resident_stride_);
+    return finish_result_(resident_results_, resident_.rows, resident_stride_);
 }
 
 // predict_on_selected_outputs on the device (SURVEY 8f-2).
@@ -1896,8 +1877,9 @@ XLinearEngine::SelectedResult XLinearEngine::predict_selected(const HostMatrix& 
     DeviceBuffer<float> d_val[2];
     std::vector<uint64_t> rel_ptr;
     std::vector<float> leaf_vals;
-    for_each_tile_(ensure_workspace_(plan, rows, x.dense ? x.cols : 0u), &x, [&](const QueryDev& qd, uint32_t r0) {
-        const uint32_t tr = qd.rows;
+    for_each_tile_(ensure_workspace_(plan, rows, x.dense ? x.cols : 0u), &x, [&](const Tile& t) {
+        const QueryDev& qd = t.q;
+        const uint32_t r0 = t.r0, tr = qd.rows;
         int cur = 0;  // which d_ptr / d_val set holds the previous layer
         if (have_codes) {  // the given previous prediction plays "layer -1"
             const uint64_t c0 = codes.row_ptr[r0], c1 = codes.row_ptr[r0 + tr];

@@ -201,7 +201,25 @@ private:
             return {ids + o, vals + o, cnt + row, keys ? keys + o : nullptr, stride};
         }
     };
-    using TileFn = std::function<void(const QueryDev& q, uint32_t r0)>;
+    // Query rows on the device; place() is the engine's only copy of host query rows.
+    struct QueryStage {
+        DeviceBuffer<uint64_t> row_ptr;
+        DeviceBuffer<uint32_t> col_idx;
+        DeviceBuffer<float> val;  // CSR values, or the dense rows
+        // placed rows are on the device (copy stream); the kernels reading them are issued (compute stream)
+        cudaEvent_t landed = nullptr, consumed = nullptr;
+        // room for `rows` rows of x holding n values (CSR non-zeros, or rows x cols); reallocating drops the placed rows
+        void reserve(const HostMatrix& x, uint32_t rows, uint64_t n);
+        // Rows [r0, r0 + tr) of x as the kernels take them, in a stage that holds x's rows from row `first` on (CSR offsets
+        // stay absolute: nnz_base = x.row_ptr[first]); place() first copies them there on `stream`.
+        QueryDev view(const HostMatrix& x, uint32_t first, uint32_t r0, uint32_t tr) const;
+        QueryDev place(const HostMatrix& x, uint32_t first, uint32_t r0, uint32_t tr, cudaStream_t stream);
+    };
+    struct ResultBuffers { DeviceBuffer<uint32_t> ids, cnt; DeviceBuffer<float> vals; };  // device result rows of a call
+    // for_each_tile_'s callback: layers [d_begin, d_end) over rows [r0, r0 + q.rows) of the batch, held in workspace rows
+    // from ws_row on
+    struct Tile { QueryDev q; uint32_t r0, ws_row; size_t d_begin, d_end; };
+    using TileFn = std::function<void(const Tile& t)>;
     using BeamFn = std::function<uint32_t(uint32_t row, uint32_t* ids, float* vals)>;
 
     // b_in[d] (where given and > 0): the beam capacity entering layer d, set by the caller (single layer: the codes rows or
@@ -212,9 +230,9 @@ private:
     // Sizes the tiles of a `rows`-query call so that the workspace of one tile stays within PB200_WORKSPACE_MB, allocates
     // that workspace and returns the tile's rows.  dense_cols > 0: dense queries, whose staged tile is also capped at 4 GiB.
     uint32_t ensure_workspace_(const std::vector<LayerPlan>& plan, uint32_t rows, uint32_t dense_cols);
-    // Tiled pass over the queries x (host CSR or dense; nullptr: the resident batch) in tiles of `tile` rows (from
-    // ensure_workspace_): stages every tile on the device and calls run(q, first row of the tile).
-    void for_each_tile_(uint32_t tile, const HostMatrix* x, const TileFn& run);
+    // The one pass over a batch of queries x (host CSR or dense; nullptr: the resident batch) in tiles of at most `tile` rows
+    // (from ensure_workspace_): stages each and hands it to run().  split: predict's CSR schedules (see the definition).
+    void for_each_tile_(uint32_t tile, const HostMatrix* x, const TileFn& run, bool split = false);
     // The beam entering the first layer of a tile (rows [0, rows) of beam_*_[0]), from fill(row, ids, vals) = its length;
     // vals is nullptr unless with_vals.
     void stage_beam_(uint32_t rows, bool with_vals, const BeamFn& fill);
@@ -238,8 +256,8 @@ private:
     }
     void score_layer_(size_t d, const QueryDev& q, const std::vector<LayerPlan>& plan, const LayerKernels& k, int cur,
                       uint32_t ws_row, bool collect_stats);
-    OutTarget reserve_results_(uint32_t rows, uint32_t stride);
-    Result finish_result_(uint32_t rows, uint32_t stride);
+    OutTarget reserve_results_(ResultBuffers& r, uint32_t rows, uint32_t stride);
+    Result finish_result_(const ResultBuffers& r, uint32_t rows, uint32_t stride);
 
     struct SelIndex {  // per layer: label -> (chunk, column offset); built on the first predict_selected call
         std::vector<uint32_t> chunk_of_label, offset_of_label;
@@ -261,25 +279,18 @@ private:
     DeviceBuffer<unsigned long long> stats_dev_;
     uint32_t beam_stride_ = 0;
 
-    // staged inputs (host-buffer path) and resident batch
-    DeviceBuffer<uint64_t> x_row_ptr_;
-    DeviceBuffer<uint32_t> x_col_idx_;
-    DeviceBuffer<float> x_val_;
-    // second staging set + copy stream: predict() uploads sub-tile t+1 of a CSR batch while sub-tile t is being scored
-    DeviceBuffer<uint64_t> x2_row_ptr_;
-    DeviceBuffer<uint32_t> x2_col_idx_;
-    DeviceBuffer<float> x2_val_;
+    // host-buffer calls: two staging sets (with copy_stream_, one is uploaded while the other is scored) and the results
+    QueryStage stage_[2];
     cudaStream_t copy_stream_ = nullptr;
-    cudaEvent_t up_ev_[2] = {nullptr, nullptr};   // staging set uploaded
-    cudaEvent_t use_ev_[2] = {nullptr, nullptr};  // staging set consumed by the score kernels
+    ResultBuffers results_;
     PinnedBuffer<uint32_t> beam_id_host_;   // stage_beam_: the given beam, staged per tile
     PinnedBuffer<float> beam_val_host_;
     PinnedBuffer<uint32_t> beam_cnt_host_;
+    // the resident batch owns its queries and results: host-buffer calls in between change neither
+    QueryStage resident_stage_;
     QueryDev resident_{};
     bool has_resident_ = false;
-    DeviceBuffer<uint32_t> res_ids_dev_;
-    DeviceBuffer<float> res_vals_dev_;
-    DeviceBuffer<uint32_t> res_cnt_dev_;
+    ResultBuffers resident_results_;
     uint32_t resident_stride_ = 0;  // top-k stride of the last resident_predict
     DeviceBuffer<unsigned long long> shard_keys_;  // local top-k of an index-sharded run before packing
     DeviceBuffer<uint32_t> shard_ids_, shard_cnt_;

@@ -53,6 +53,35 @@ def test_xlinear_fanout_equals_single_engine(tmp_path, gpu_clib, devices_env):
                           what=f"ragged result rows {devs}")
 
 
+def test_xlinear_fanout_through_both_csr_schedules(tmp_path, gpu_clib, devices_env, monkeypatch):
+    """10,000 CSR rows over two replicas: each replica's row block holds >= 4096 rows, and the second one starts at
+    row_ptr[0] != 0.  At the default workspace each block takes the whole-batch upload schedule; at PB200_WORKSPACE_MB=64
+    (about 1,000 queries per tile at beam 64 over 16,384 labels) the two-set schedule.  Both equal one engine bit for bit."""
+    from pecos_b200.xlinear import XLinearModel
+
+    folder = str(tmp_path / "m")
+    layers = random_tree(231, [64, 16384], 300, 20, bias=1.0)
+    synth.save_xlinear_model(folder, layers, bias=1.0, only_topk=10)
+    X = synth.make_queries(232, 10000, 300, 30)
+    c = gpu_clib.clib_float32
+    monkeypatch.delenv("PB200_WORKSPACE_MB", raising=False)
+    os.environ.pop("PB200_DEVICES", None)
+    want = XLinearModel.load(folder, is_predict_only=True).predict(X, beam_size=64, only_topk=10)
+    os.environ["PB200_DEVICES"] = "0,0"
+    m = XLinearModel.load(folder, is_predict_only=True)
+    h = m.model.model_chain
+    assert c.pb200_xlinear_replicas(h) == 2
+    launches = []
+    for mb in (None, "64"):
+        if mb:
+            monkeypatch.setenv("PB200_WORKSPACE_MB", mb)
+        l0 = c.pb200_xlinear_launches(h)
+        got = m.predict(X, beam_size=64, only_topk=10)
+        launches.append(c.pb200_xlinear_launches(h) - l0)
+        assert assert_csr_parity(got, want, rtol=0.0, what=f"fan-out 0,0, workspace {mb or 'default'} MiB") == 1.0
+    assert launches[1] > launches[0], f"launches {launches}: the 64 MiB workspace did not cut the blocks into tiles"
+
+
 def test_hnsw_fanout_equals_single_engine(gpu_clib, devices_env):
     from pecos_b200.hnsw import HNSW
 

@@ -218,3 +218,34 @@ def test_candidate_queue_overflow_is_retried_not_fatal(gpu_clib):
                os.path.join(MID, "ip_d70", "Q.npy"), os.path.join(MID, "expected.npz")))
     r = subprocess.run([sys.executable, "-c", code], stdout=subprocess.PIPE, stderr=subprocess.PIPE, text=True)
     assert r.returncode == 0 and "retries" in r.stdout, r.stderr[-1500:]
+
+
+def test_resident_batch_survives_host_buffer_calls(golden, gpu_clib):
+    """The resident batch and its results have their own device buffers: host-buffer searches in between, one larger and
+    one smaller than the resident batch, change neither what resident_fetch returns nor the next resident_predict."""
+    from ctypes import POINTER, byref, c_float, c_uint32
+
+    from pecos_b200.core import ScipyDrmF32
+
+    E, _, Xt, _ = golden
+    m = _load(os.path.join(GOLD, "model_l2"))
+    c = gpu_clib.clib_float32
+    px = ScipyDrmF32.init_from(np.ascontiguousarray(Xt))
+    c.pb200_hnsw_resident_upload(m.model_ptr, byref(px))
+
+    def fetch():
+        idx = np.zeros((Xt.shape[0], 10), dtype=np.uint32)
+        val = np.zeros((Xt.shape[0], 10), dtype=np.float32)
+        c.pb200_hnsw_resident_fetch(m.model_ptr, idx.ctypes.data_as(POINTER(c_uint32)), val.ctypes.data_as(POINTER(c_float)))
+        return idx, val.view(np.uint32)
+
+    c.pb200_hnsw_resident_predict(m.model_ptr, 50, 10)
+    idx, val = fetch()
+    assert np.array_equal(idx, E["model_l2|50|10|idx"])
+    m.predict(np.ascontiguousarray(np.vstack([Xt, Xt, Xt])), pred_params=_pp(100, 20), ret_csr=False)
+    m.predict(np.ascontiguousarray(Xt[:3]), pred_params=_pp(50, 5), ret_csr=False)
+    for what in ("fetch", "resident_predict"):
+        if what == "resident_predict":
+            c.pb200_hnsw_resident_predict(m.model_ptr, 50, 10)
+        i2, v2 = fetch()
+        assert np.array_equal(i2, idx) and np.array_equal(v2, val), f"{what} after host-buffer calls"

@@ -153,3 +153,42 @@ def test_sparse_resident_batch_counters_and_save(tmp_path, gpu_clib):
     m2 = _load(out)
     i2, d2 = m2.predict(Q, pred_params=_pp(200, 10), ret_csr=False)
     assert np.array_equal(i2, idx) and np.array_equal(d2, val)
+
+
+def test_sparse_resident_batch_survives_host_buffer_calls(gpu_clib):
+    """As for dense indices: host-buffer searches between the resident calls, one larger (more rows and longer rows, so the
+    query staging grows) and one smaller, change neither what resident_fetch returns nor the next resident_predict."""
+    from ctypes import POINTER, byref, c_float, c_uint32
+
+    from pecos_b200.core import ScipyCsrF32
+
+    folder = os.path.join(SPARSE, "ip_tfidf")
+    E = np.load(os.path.join(SPARSE, "expected.npz"))
+    m = _load(folder)
+    Q = smat.load_npz(os.path.join(folder, "Q.npz")).tocsr()
+    Q.sort_indices()
+    c = gpu_clib.clib_float32
+    px = ScipyCsrF32.init_from(Q)
+    c.pb200_hnsw_resident_upload_csr(m.model_ptr, byref(px))
+
+    def fetch():
+        idx = np.zeros((Q.shape[0], 10), dtype=np.uint32)
+        val = np.zeros((Q.shape[0], 10), dtype=np.float32)
+        c.pb200_hnsw_resident_fetch(m.model_ptr, idx.ctypes.data_as(POINTER(c_uint32)), val.ctypes.data_as(POINTER(c_float)))
+        return idx, val.view(np.uint32)
+
+    c.pb200_hnsw_resident_predict(m.model_ptr, 200, 10)
+    idx, val = fetch()
+    assert np.array_equal(idx, E["ip_tfidf|200|10|idx"])
+    # more rows, and longer ones: each row of `big` is the sum of two rows of Q
+    both = (Q + Q[np.random.default_rng(7).permutation(Q.shape[0])]).tocsr()
+    big = smat.vstack([both, both, both]).tocsr().astype(np.float32)
+    big.sort_indices()
+    assert big.shape[0] > Q.shape[0] and np.diff(big.indptr).max() > np.diff(Q.indptr).max()
+    m.predict(big, pred_params=_pp(100, 20), ret_csr=False)
+    m.predict(Q[:3], pred_params=_pp(50, 5), ret_csr=False)
+    for what in ("fetch", "resident_predict"):
+        if what == "resident_predict":
+            c.pb200_hnsw_resident_predict(m.model_ptr, 200, 10)
+        i2, v2 = fetch()
+        assert np.array_equal(i2, idx) and np.array_equal(v2, val), f"{what} after host-buffer calls"

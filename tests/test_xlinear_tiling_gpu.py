@@ -134,3 +134,35 @@ def test_index_sharded_run_tiles(tiling_model, gpu_clib, monkeypatch):
     finally:
         for h in handles:
             c.c_xlinear_destruct_model(h)
+
+
+def test_resident_batch_survives_host_buffer_calls(tiling_model, gpu_clib):
+    """The resident batch and its results have their own device buffers: host-buffer predict calls in between -- one larger
+    in rows and non-zeros than the resident batch, so every staging buffer grows, and one smaller -- change neither what
+    resident_fetch returns nor what the next resident_predict computes."""
+    from pecos_b200.core import ScipyCompressedSparseAllocator, ScipyCsrF32
+    from pecos_b200.xlinear import XLinearModel
+
+    folder, _, X, _ = tiling_model
+    c = gpu_clib.clib_float32
+    m = XLinearModel.load(folder, is_predict_only=True)
+    h = m.model.model_chain
+    Xr = X[:2000]
+    assert X.nnz > Xr.nnz
+    cx = ScipyCsrF32.init_from(Xr)
+    c.pb200_xlinear_resident_upload_csr(h, byref(cx))
+
+    def fetch():
+        alloc = ScipyCompressedSparseAllocator()
+        c.pb200_xlinear_resident_fetch(h, alloc.cfunc)
+        return alloc.get()
+
+    c.pb200_xlinear_resident_predict(h, BEAM, None, TOPK, 0)
+    first = fetch()
+    assert first.nnz > 0
+    assert assert_csr_parity(first, m.predict(Xr, beam_size=BEAM, only_topk=TOPK), rtol=0.0, what="resident") == 1.0
+    m.predict(X, beam_size=BEAM, only_topk=TOPK)
+    m.predict(X[:300], beam_size=BEAM, only_topk=TOPK)
+    assert assert_csr_parity(fetch(), first, rtol=0.0, what="fetch after host-buffer calls") == 1.0
+    c.pb200_xlinear_resident_predict(h, BEAM, None, TOPK, 0)
+    assert assert_csr_parity(fetch(), first, rtol=0.0, what="resident_predict after host-buffer calls") == 1.0
