@@ -173,7 +173,8 @@ void c_ann_hnsw_predict_drm_l2_f32(void* model_ptr, const ScipyDrmF32* pX, uint3
  * :508-513, :522-523, :563-564; distances pecos/core/ann/feat_vectors.hpp:186-210 + distance_impl/common.hpp:15-86).  Rows of the
  * index and of the queries carry strictly ascending column indices (what scipy's sort_indices()/sum_duplicates() give and
  * the reference's block intersection assumes).  The reference's sparse "l2" evaluates to -2<x,y> (feat_vectors.hpp:186-192: the
- * squared norms are taken as do_l2_distance_simd(x, x) = 0); this library returns the same values. */
+ * squared norms are taken as do_l2_distance_simd(x, x), 0 for finite rows, NaN when a row stores a NaN or +-inf anywhere);
+ * this library returns the same values, NaN for such pairs included. */
 void* c_ann_hnsw_load_csr_ip_f32(const char* model_dir, const bool lazy_load);
 void* c_ann_hnsw_load_csr_l2_f32(const char* model_dir, const bool lazy_load);
 void c_ann_hnsw_destruct_csr_ip_f32(void* model_ptr);
@@ -274,12 +275,15 @@ uint64_t pb200_hnsw_sparse_entries(void* model_ptr);
  * per GPU).  model_ptr is a c_ann_hnsw_load_* handle of this rank's shard; only its primary engine is used.
  *   local:  searches the shard and writes its top-k as 16-byte records {u64 key, u32 id, f32 value}[rows][topk] into the
  *           CALLER-OWNED DEVICE buffer rec_dev (the send buffer of ONE all-gather).  id = id_offset + local id (the shard's
- *           first global row), value = distance, key = (~orderable(distance) << 32) | ~(rank * topk + slot); key 0 marks an
- *           empty slot.  Requires (rank + 1) * topk <= 1024.
- *   merge:  gathered [world][rows][topk] records g_rec -> ret_idx / ret_val [rows][topk] (host), ordered by distance, then
- *           shard rank, then slot; rows with fewer than topk results end in zeros, like c_ann_hnsw_predict_*.
+ *           first global row), value = distance, key = (~orderable(distance) << 32) | ~(rank * topk + slot), where every NaN
+ *           takes orderable = 0xFFFFFFFF whatever its sign and payload; key 0 marks an empty slot.  Requires
+ *           (rank + 1) * topk <= 1024.
+ *   merge:  gathered [world][rows][topk] records g_rec -> ret_idx / ret_val [rows][topk] (host), ordered by (distance with
+ *           NaN last, shard rank, slot); rows with fewer than topk results end in zeros, like c_ann_hnsw_predict_*.
  *           Requires world * topk <= 1024.
- * The result equals, bit for bit, the merge by that order of the per-shard c_ann_hnsw_predict_* results. */
+ * The result equals, bit for bit, the merge by that order of the per-shard c_ann_hnsw_predict_* results.  At world 1 this
+ * is the unsharded search when no NaN is returned; otherwise it is the unsharded search's entries ordered by (distance with
+ * NaN last, position): a NaN in the search heaps can leave the unsharded result out of order, and the merge sorts it. */
 void pb200_hnsw_sharded_local_packed_drm(void* model_ptr, const ScipyDrmF32* pX, uint32_t efS, uint32_t topk, uint32_t rank,
                                          uint32_t id_offset, void* rec_dev);
 void pb200_hnsw_sharded_local_packed_csr(void* model_ptr, const ScipyCsrF32* pX, uint32_t efS, uint32_t topk, uint32_t rank,
@@ -381,11 +385,24 @@ double pb200_spmm_last_kernel_ms(void);
 
 /* base-vector rows kept in flight per warp by the bulk-copy (TMA) ring: 0 = direct loads, 4 (default) or 8; returns the
  * value in effect.  Results are identical for every setting.  A search whose per-warp shared-memory slice (query + ring
- * rows + result heap) would exceed 200 KB at this depth runs the next shallower one that fits (8 -> 4 -> 0); dense indices
- * with d beyond about 50,000 fit none and raise. */
+ * rows + neighbour slots + result heap) would exceed 200 KB at this depth runs the next shallower one that fits
+ * (8 -> 4 -> 0), and where depth 0 does not fit either, the result heap moves to global memory (as for every ef > 512). */
 int pb200_hnsw_set_stages(void* model_ptr, int stages);
+/* Width limit of dense indices, host-only.  With ef = max(efS, topk) and nbmax = the longest neighbour list (level 0 or
+ * above) rounded up to 32, a warp's slice holds the query row (dense_vstride(d) floats, see
+ * pb200_pairwise_ann_dense_fits), 8 * nbmax bytes of neighbour ids and distances, the ring rows and, while ef <= 512 and it
+ * fits, the (ef + 1)-entry result heap.  A dense index is searchable for every ef iff 4 * dense_vstride(d) + 8 * nbmax
+ * <= 204,800 (M = 16: every d up to 51,087 and every multiple of 16 up to 51,136); a wider one loads, saves and creates
+ * searchers, but predict on it is a fatal error, so callers check first (HNSW.predict and ShardedHNSW.predict raise
+ * ValueError).  Sparse indices have no width limit.  Both return 1 if the search fits, else 0, and out[5] = {ring depth,
+ * result heap in shared memory (1) or global memory (0), per-warp bytes, nbmax, row stride in floats (sparse: 0)}.
+ *   search_fits: for a handle at its pb200_hnsw_set_stages setting; handles of the reference library report 1, out zeros.
+ *   dense_plan:  for a dense index of width feat_dim whose longest neighbour list has max_degree entries. */
+int pb200_hnsw_search_fits(void* model_ptr, uint32_t efS, uint32_t topk, uint32_t* out);
+int pb200_hnsw_dense_plan(uint32_t feat_dim, uint32_t max_degree, int stages, uint32_t efS, uint32_t topk, uint32_t* out);
 /* the last search launch of the handle's primary engine: out[5] = {ring depth it ran, warps per CTA, CTAs, dynamic shared
- * memory per CTA in bytes, result-heap entries allocated in global scratch (heaps of ef > 512 live there; grows only)} */
+ * memory per CTA in bytes, result-heap entries allocated in global scratch (heaps of ef > 512, and of the widest dense rows,
+ * live there; grows only)} */
 void pb200_hnsw_launch_info(void* model_ptr, uint64_t* out);
 void pb200_hnsw_get_info(void* model_ptr, uint64_t* out);
 /* Host-only ingest check of an HNSW index folder (<model>/c_model), no GPU needed: the loader's validation of config.json

@@ -439,6 +439,33 @@ class B200CoreLib(object):
                 f"row ({plan['vstride']} floats after padding) and 128 distances in at most 204,800 bytes of shared memory, "
                 f"which holds every feat_dim up to 51,024 and every multiple of 16 up to 51,072")
 
+    HNSW_PLAN_KEYS = ("stages", "heap_in_smem", "per_warp_bytes", "nbmax", "vstride")
+
+    def hnsw_search_fits(self, model_ptr, efS, topk):
+        """(fits, {stages, heap_in_smem, per_warp_bytes, nbmax, vstride}) of a search (efS, topk) on an HNSW handle.  Host-only."""
+        out = (c_uint32 * 5)()
+        fits = self.clib_float32.pb200_hnsw_search_fits(model_ptr, int(efS), int(topk), out)
+        return bool(fits), dict(zip(self.HNSW_PLAN_KEYS, [int(v) for v in out]))
+
+    def hnsw_dense_plan(self, feat_dim, max_degree, stages, efS, topk):
+        """(fits, plan) as hnsw_search_fits, for a dense index of width feat_dim whose longest neighbour list has max_degree
+        entries, at ring depth setting `stages`.  Host-only, no handle."""
+        out = (c_uint32 * 5)()
+        fits = self.clib_float32.pb200_hnsw_dense_plan(int(feat_dim), int(max_degree), int(stages), int(efS), int(topk), out)
+        return bool(fits), dict(zip(self.HNSW_PLAN_KEYS, [int(v) for v in out]))
+
+    def hnsw_check_search(self, model_ptr, feat_dim, efS, topk):
+        """Raises ValueError unless a search (efS, topk) on the HNSW handle can run.  Host-only, so it runs before any native
+        call that would search."""
+        fits, plan = self.hnsw_search_fits(model_ptr, efS, topk)
+        if not fits:
+            widest = (204800 - 8 * plan["nbmax"]) // 4 // 64 * 64
+            raise ValueError(
+                f"pecos_b200: this dense HNSW index (feat_dim={feat_dim}) cannot be searched: one warp stages the query row "
+                f"({plan['vstride']} floats after padding) and {plan['nbmax']} neighbour ids and distances in at most 204,800 "
+                f"bytes of shared memory; with this index's neighbour lists that holds every feat_dim up to {widest - 49:,} and "
+                f"every multiple of 16 up to {widest:,}")
+
     def pairwise_ann_host_info(self, c_model_dir, data_type):
         """Host-only ingest check of a <model>/c_model folder; returns its sizes, raises ValueError if it does not load."""
         out = (c_uint64 * 6)()
@@ -558,6 +585,8 @@ class B200CoreLib(object):
         fp(c.pb200_hnsw_get_counters, None, [c_void_p, POINTER(c_uint64)])
         fp(c.pb200_hnsw_set_stages, c_int, [c_void_p, c_int])
         fp(c.pb200_hnsw_launch_info, None, [c_void_p, POINTER(c_uint64)])
+        fp(c.pb200_hnsw_search_fits, c_int, [c_void_p, c_uint32, c_uint32, POINTER(c_uint32)])
+        fp(c.pb200_hnsw_dense_plan, c_int, [c_uint32, c_uint32, c_int, c_uint32, c_uint32, POINTER(c_uint32)])
         fp(c.pb200_hnsw_get_info, None, [c_void_p, POINTER(c_uint64)])
         fp(c.pb200_hnsw_host_info, c_int, [c_char_p, c_int, c_int, POINTER(c_uint64)])
         fp(c.pb200_pairwise_ann_get_counters, None, [c_void_p, POINTER(c_uint64)])

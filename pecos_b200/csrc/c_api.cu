@@ -1078,6 +1078,32 @@ void pb200_hnsw_launch_info(void* model_ptr, uint64_t* out) {
     PB200_API_END("pb200_hnsw_launch_info")
 }
 
+// Host-only: whether a search (efS, topk) on this handle fits one warp's shared memory, and the plan it would run with:
+// out = {ring depth, result heap in shared memory (1) or global memory (0), per-warp bytes, neighbour slots, row stride}.
+// Handles of the reference library report that they fit (out all zeros): they search on the CPU.
+int pb200_hnsw_search_fits(void* model_ptr, uint32_t efS, uint32_t topk, uint32_t* out) {
+    PB200_API_BEGIN
+    for (int i = 0; i < 5; ++i) out[i] = 0u;
+    if (!hnsw_is_ours(model_ptr)) return 1;
+    PB200_LOCK(hnsw_of(model_ptr))
+    const pb200::HnswEngine& e = hnsw_of(model_ptr).primary();
+    const pb200::HnswPlan p = e.search_plan(efS, topk);
+    out[0] = static_cast<uint32_t>(p.stages); out[1] = p.heap_in_smem ? 1u : 0u; out[2] = p.per_warp; out[3] = p.nbmax;
+    out[4] = e.sparse() ? 0u : pb200::dense_vstride(e.host().feat_dim);
+    return p.fits ? 1 : 0;
+    PB200_API_END("pb200_hnsw_search_fits")
+}
+
+// Host-only, no handle: the same plan for a dense index of width feat_dim whose longest neighbour list (level 0 or above) has
+// max_degree entries, at ring depth setting `stages`; out as above.
+int pb200_hnsw_dense_plan(uint32_t feat_dim, uint32_t max_degree, int stages, uint32_t efS, uint32_t topk, uint32_t* out) {
+    const uint32_t vstride = pb200::dense_vstride(feat_dim);
+    const pb200::HnswPlan p = pb200::hnsw_plan(false, vstride, max_degree, stages, std::max(efS, topk), 0u);
+    out[0] = static_cast<uint32_t>(p.stages); out[1] = p.heap_in_smem ? 1u : 0u; out[2] = p.per_warp; out[3] = p.nbmax;
+    out[4] = vstride;
+    return p.fits ? 1 : 0;
+}
+
 void pb200_hnsw_get_counters(void* model_ptr, uint64_t* out) {
     PB200_API_BEGIN
     PB200_LOCK(hnsw_of(model_ptr))

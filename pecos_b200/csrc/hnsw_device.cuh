@@ -155,6 +155,7 @@ struct SparseQuery {  // one query row: generic pointers (shared-memory copy, or
     const float* val;
     uint32_t n;
     const uint32_t* filter;
+    bool nonfinite;  // sparse "l2": the row stores a NaN or +-inf, so its squared norm in the reference is NaN
 };
 
 __device__ __forceinline__ uint2 ld_stream_u2(const uint2* p) {
@@ -191,7 +192,10 @@ __device__ __forceinline__ float sparse_step(const SparseQuery& q, bool has, uin
     return ret;
 }
 
-// distances of ids[0..n) -> dist[0..n) for a sparse index, two rows at a time (one per half-warp)
+// distances of ids[0..n) -> dist[0..n) for a sparse index, two rows at a time (one per half-warp).  The reference's sparse "l2"
+// adds the squared norms do_l2_distance_simd(x, x) + do_l2_distance_simd(y, y) before subtracting 2<x,y> (feat_vectors.hpp:
+// 186-192): 0 for finite rows, NaN when either row stores a NaN or +-inf anywhere, matched or not.  So l2 reads every stored
+// value, also for an empty query, and returns NaN for such a pair.
 template <int METRIC>
 __device__ __forceinline__ void batch_distances_sparse(const HnswDev& ix, const SparseQuery& q, const uint32_t* ids, float* dist,
                                                        uint32_t n, int lane, unsigned long long& n_entries) {
@@ -210,21 +214,28 @@ __device__ __forceinline__ void batch_distances_sparse(const HnswDev& ix, const 
         if (hl == 0) n_entries += len;
         const uint2* row = ix.sp_ent + r0;
         float ret = 0.0f;
+        bool nonfinite = false;  // l2: a stored NaN or +-inf among this lane's entries of the row
         for (uint32_t j0 = 0; j0 < len_max; j0 += 64) {  // four independent 128-byte loads per half-warp in flight
             uint2 e[4];
             bool has[4];
 #pragma unroll
             for (int u = 0; u < 4; ++u) {
                 const uint32_t j = j0 + 16u * u + hl;
-                has[u] = (j < len) && q.n != 0u;
+                has[u] = (j < len) && (METRIC == HNSW_L2 || q.n != 0u);
                 e[u] = has[u] ? ld_stream_u2(row + j) : make_uint2(0u, 0u);
+                if (METRIC == HNSW_L2) nonfinite |= has[u] && !isfinite(__uint_as_float(e[u].y));
             }
 #pragma unroll
             for (int u = 0; u < 4; ++u) {
                 if (j0 + 16u * u < len_max) ret = sparse_step(q, has[u], e[u], ret, lane);
             }
         }
-        if (hl == 0 && valid) dist[slot] = sparse_finalize<METRIC>(ret);
+        float d = sparse_finalize<METRIC>(ret);
+        if (METRIC == HNSW_L2) {
+            const unsigned bad = (__ballot_sync(kFull, nonfinite) >> (16 * half)) & 0xFFFFu;
+            if (bad || q.nonfinite) d = __uint_as_float(0x7FFFFFFFu);
+        }
+        if (hl == 0 && valid) dist[slot] = d;
     }
     __syncwarp();
 }

@@ -16,7 +16,8 @@
 // streams the neighbour's {index, value} entries (16 per step, 128 contiguous bytes), every lane looks its entry up in the query
 // row staged in shared memory (a 8,192-bit filter first, binary search on a filter hit) and the matched products are added in
 // ascending index order -- the order of the reference's block intersection (distance_impl/common.hpp:15-86) for rows with strictly
-// ascending indices.  The reference's sparse "l2" is -2<x,y> (its squared norms are do_l2_distance_simd(x, x) = 0): restated as is.
+// ascending indices.  The reference's sparse "l2" is -2<x,y> (its squared norms are do_l2_distance_simd(x, x) = 0, NaN for a row
+// that stores a NaN or +-inf): restated as is.
 //
 // HBM traffic per query (SURVEY 8d): n_dist * 4d + n_expand * 4(1+maxM0) + hops * 4(1+maxM) + 4d + 8k.
 #include "hnsw_engine.h"
@@ -30,8 +31,6 @@
 namespace pb200 {
 
 namespace {
-
-constexpr uint32_t kEfSmemMax = 512;  // result heaps up to this many entries live in shared memory
 
 template <int METRIC, int STAGES, bool SPARSE>
 __global__ void __launch_bounds__(256)
@@ -77,7 +76,7 @@ hnsw_search_kernel(const HnswDev ix, const float* __restrict__ Q, const HnswSpar
         const uint32_t q = static_cast<uint32_t>(qq);
         unsigned long long n_dist = 0, n_expand = 0, n_hops = 0, n_entries = 0;
 
-        SparseQuery sq{nullptr, nullptr, 0u, nullptr};
+        SparseQuery sq{nullptr, nullptr, 0u, nullptr, false};
         if (SPARSE) {
             // stage the query row (indices, values) and the membership filter of its indices
             const unsigned long long q0 = SQ.ptr[q];
@@ -85,12 +84,15 @@ hnsw_search_kernel(const HnswDev ix, const float* __restrict__ Q, const HnswSpar
             for (uint32_t w = lane; w < kSpFilterWords; w += 32) sq_filter[w] = 0u;
             __syncwarp();
             const bool staged = sq.n <= SQ.qcap;
+            bool nonfinite = false;
             for (uint32_t i = lane; i < sq.n; i += 32) {
                 const uint32_t c = SQ.idx[q0 + i];
                 if (staged) { sq_idx[i] = c; sq_val[i] = SQ.val[q0 + i]; }
+                if (METRIC == HNSW_L2) nonfinite |= !isfinite(SQ.val[q0 + i]);
                 const uint32_t h = sp_hash(c);
                 atomicOr(&sq_filter[h >> 5], 1u << (h & 31u));
             }
+            if (METRIC == HNSW_L2) sq.nonfinite = __any_sync(kFull, nonfinite);
             sq.idx = staged ? sq_idx : SQ.idx + q0;
             sq.val = staged ? sq_val : SQ.val + q0;
             sq.filter = sq_filter;
@@ -252,9 +254,10 @@ hnsw_search_kernel(const HnswDev ix, const float* __restrict__ Q, const HnswSpar
 }
 
 // Index sharding: this shard's [nq][topk] search results -> exchange records.  An empty slot (out_idx == 0xFFFFFFFF, the fill
-// of the sharded path) gets key 0.  key = (~orderable(dist) << 32) | ~(rank * topk + slot): the merge orders by distance
-// ascending, then shard rank, then slot, so one shard's own order (ties included) is kept; the low word is never 0 while
-// (rank + 1) * topk <= kSelKeys.
+// of the sharded path) gets key 0.  key = (~o << 32) | ~(rank * topk + slot) with o = orderable(dist), and o = 0xFFFFFFFF for
+// every NaN whatever its sign and payload: the merge orders by distance ascending with NaN last, then shard rank, then slot,
+// so one shard's own order (ties included) is kept wherever it is sorted -- a NaN in the search heaps can leave it out of order,
+// and the merge sorts it; the low word is never 0 while (rank + 1) * topk <= kSelKeys.
 __global__ void hnsw_shard_pack_kernel(const uint32_t* __restrict__ idx, const float* __restrict__ val, const uint64_t n,
                                        const uint32_t topk, const uint32_t rank, const uint32_t id_offset,
                                        ShardRecord* __restrict__ rec) {
@@ -265,7 +268,8 @@ __global__ void hnsw_shard_pack_kernel(const uint32_t* __restrict__ idx, const f
     ShardRecord out{0ull, 0u, 0.0f};
     if (id != 0xFFFFFFFFu) {
         const float d = val[i];
-        out.key = (static_cast<unsigned long long>(~orderable(d)) << 32) | static_cast<unsigned long long>(~(rank * topk + slot));
+        const uint32_t o = isnan(d) ? 0xFFFFFFFFu : orderable(d);
+        out.key = (static_cast<unsigned long long>(~o) << 32) | static_cast<unsigned long long>(~(rank * topk + slot));
         out.id = id_offset + id;
         out.val = d;
     }
@@ -307,6 +311,21 @@ uint32_t warp_smem_bytes(bool sparse, uint32_t vstride, int stages, uint32_t qca
     const uint32_t query = sparse ? qcap * 8u + kSpFilterWords * 4u
                                   : vstride * 4u * (1u + static_cast<uint32_t>(stages)) + static_cast<uint32_t>(stages) * 8u;
     return (query + tail + 15u) & ~15u;
+}
+
+HnswPlan hnsw_plan(bool sparse, uint32_t vstride, uint32_t max_degree, int stages, uint32_t ef, uint32_t qcap) {
+    const uint32_t nbmax = ((max_degree + 31u) / 32u) * 32u;
+    HnswPlan p{false, 0, false, 0u, nbmax};
+    for (const bool heap_in_smem : {true, false}) {
+        if (heap_in_smem && ef > kEfSmemMax) continue;
+        const uint32_t tail = nbmax * 8u + (heap_in_smem ? (ef + 1u) * 8u : 0u);
+        for (int s = sparse ? 0 : (stages <= 0 ? 0 : (stages <= 4 ? 4 : 8));; s = s > 4 ? 4 : 0) {
+            p = HnswPlan{false, s, heap_in_smem, warp_smem_bytes(sparse, vstride, s, qcap, tail), nbmax};
+            if (p.per_warp <= kWarpSmemMax) { p.fits = true; return p; }
+            if (s == 0) break;
+        }
+    }
+    return p;
 }
 
 CtaShape cta_shape(int device, uint32_t per_warp, uint32_t max_warps_per_sm) {
@@ -455,12 +474,13 @@ HnswEngine::~HnswEngine() {
     if (stream_) cudaStreamDestroy(stream_);
 }
 
-uint32_t HnswEngine::per_warp_smem_(uint32_t ef, int stages, uint32_t qcap, uint32_t* nbmax_out) const {
+HnswPlan HnswEngine::plan_(uint32_t ef, uint32_t qcap) const {
     const HnswHostIndex& H = *host_;
-    const uint32_t nbmax = ((std::max(H.l0_max_degree, H.l1_max_degree) + 31u) / 32u) * 32u;
-    if (nbmax_out) *nbmax_out = nbmax;
-    // [staged query | ids | distances | result heap]
-    return warp_smem_bytes(H.sparse, view_.vstride, stages, qcap, nbmax * 8 + (ef <= kEfSmemMax ? (ef + 1) * 8 : 0));
+    return hnsw_plan(H.sparse, view_.vstride, std::max(H.l0_max_degree, H.l1_max_degree), stages_, ef, qcap);
+}
+
+HnswPlan HnswEngine::search_plan(uint32_t efS, uint32_t topk) const {
+    return plan_(std::max(efS, topk), host_->sparse ? kSpQcapMax : 0u);
 }
 
 void HnswEngine::set_stages(int stages) {
@@ -469,21 +489,17 @@ void HnswEngine::set_stages(int stages) {
 }
 
 // One warp's shared-memory slice must fit kWarpSmemMax.  The ring takes stages + 1 rows of 4 * vstride bytes, so wide vectors
-// run the deepest ring that fits: the configured depth, else 8 -> 4 -> 0 (direct loads: one row, dense d up to about 50,000).
-// Results do not depend on the depth.
+// run the deepest ring that fits, and the widest ones move the result heap to global memory too (hnsw_plan).  Results do not
+// depend on the plan.  Callers check search_plan first (HNSW.predict raises ValueError), so the throw is a last guard.
 void HnswEngine::ensure_scratch_(uint32_t ef, uint32_t qcap) {
     const HnswHostIndex& H = *host_;
-    const bool top_in_smem = ef <= kEfSmemMax;
-    int stages = stages_;
-    uint32_t per_warp = per_warp_smem_(ef, stages, qcap, nullptr);
-    while (stages > 0 && per_warp > kWarpSmemMax) {
-        stages = stages > 4 ? 4 : 0;
-        per_warp = per_warp_smem_(ef, stages, qcap, nullptr);
-    }
-    if (per_warp > kWarpSmemMax)
+    const HnswPlan plan = plan_(ef, qcap);
+    if (!plan.fits)
         throw std::runtime_error("pecos_b200: HNSW query dimension too large for the shared-memory staging area, even with "
-                                 "direct loads (dense indices serve d up to about 50,000)");
-    run_stages_ = H.sparse ? 0 : stages;
+                                 "direct loads and the result heap in global memory");
+    run_plan_ = plan;
+    const bool top_in_smem = plan.heap_in_smem;
+    const uint32_t per_warp = plan.per_warp;
     const CtaShape shape = cta_shape(device_, per_warp, H.sparse ? 32u : 16u);
     const uint32_t warps = shape.warps, sms = shape.sms;
     uint32_t n_ctas = sms * shape.ctas_per_sm;
@@ -508,7 +524,7 @@ void HnswEngine::ensure_scratch_(uint32_t ef, uint32_t qcap) {
 }
 
 void HnswEngine::launch_info(uint64_t* out) const {
-    out[0] = static_cast<uint64_t>(run_stages_);
+    out[0] = static_cast<uint64_t>(run_plan_.stages);
     out[1] = warps_per_cta_;
     out[2] = last_ctas_;
     out[3] = last_smem_;
@@ -520,9 +536,9 @@ double HnswEngine::launch_once_(const SearchIo& io, uint32_t efS, uint32_t topk,
     const uint32_t ef = std::max(efS, topk), nq = io.nq;
     if (ef == 0) throw std::runtime_error("pecos_b200: efS and topk are both zero");
     ensure_scratch_(ef, io.queries->qcap());
-    uint32_t nbmax = 0;
-    const bool top_in_smem = ef <= kEfSmemMax;
-    const uint32_t per_warp = per_warp_smem_(ef, run_stages_, io.queries->qcap(), &nbmax);
+    const uint32_t nbmax = run_plan_.nbmax, per_warp = run_plan_.per_warp;
+    const bool top_in_smem = run_plan_.heap_in_smem;
+    const int stages = run_plan_.stages;
     const uint32_t words = static_cast<uint32_t>((static_cast<uint64_t>(H.num_node) + 31) / 32);
     PB200_CUDA(cudaMemsetAsync(ctrl_.get(), 0, 8 * sizeof(unsigned long long), stream_));
     PB200_CUDA(cudaMemsetAsync(io.idx, idx_fill, static_cast<uint64_t>(nq) * topk * 4, stream_));
@@ -539,8 +555,8 @@ double HnswEngine::launch_once_(const SearchIo& io, uint32_t efS, uint32_t topk,
     };
     const bool ip = H.metric == HNSW_IP;
     if (H.sparse) { if (ip) launch(hnsw_search_kernel<HNSW_IP, 0, true>); else launch(hnsw_search_kernel<HNSW_L2, 0, true>); }
-    else if (run_stages_ == 0) { if (ip) launch(hnsw_search_kernel<HNSW_IP, 0, false>); else launch(hnsw_search_kernel<HNSW_L2, 0, false>); }
-    else if (run_stages_ == 4) { if (ip) launch(hnsw_search_kernel<HNSW_IP, 4, false>); else launch(hnsw_search_kernel<HNSW_L2, 4, false>); }
+    else if (stages == 0) { if (ip) launch(hnsw_search_kernel<HNSW_IP, 0, false>); else launch(hnsw_search_kernel<HNSW_L2, 0, false>); }
+    else if (stages == 4) { if (ip) launch(hnsw_search_kernel<HNSW_IP, 4, false>); else launch(hnsw_search_kernel<HNSW_L2, 4, false>); }
     else { if (ip) launch(hnsw_search_kernel<HNSW_IP, 8, false>); else launch(hnsw_search_kernel<HNSW_L2, 8, false>); }
     PB200_CUDA(cudaGetLastError());
     last_ctas_ = ctas;

@@ -60,6 +60,22 @@ struct CtaShape {
 };
 CtaShape cta_shape(int device, uint32_t per_warp, uint32_t max_warps_per_sm);
 
+// Launch plan of one search with a result heap of ef = max(efS, topk) entries: the ring depth, where the result heap lives and
+// the bytes of one warp's shared-memory slice [staged query | ring rows | mbarriers | nbmax neighbour ids | distances | result
+// heap if held in shared memory].  Tried in order, the first that fits kWarpSmemMax wins: the heap in shared memory (only while
+// ef <= kEfSmemMax) at ring depths `stages`, 4, 0; then the heap in global memory at the same depths.  So a dense index serves
+// every ef up to the width that fits with the heap in global memory at depth 0 (vstride * 4 + nbmax * 8 bytes); fits = false
+// beyond it.  Sparse indices always run depth 0 and fit for every width.  Results do not depend on the plan.
+constexpr uint32_t kEfSmemMax = 512;
+struct HnswPlan {
+    bool fits;
+    int stages;
+    bool heap_in_smem;
+    uint32_t per_warp;
+    uint32_t nbmax;  // neighbour slots of the slice: the longest neighbour list, rounded up to 32
+};
+HnswPlan hnsw_plan(bool sparse, uint32_t vstride, uint32_t max_degree, int stages, uint32_t ef, uint32_t qcap);
+
 // A query batch in HBM, as the search kernels take it: dense rows, or csr rows with offsets rebased to the batch.
 class DeviceQueries {
 public:
@@ -131,6 +147,9 @@ public:
     // the last search launch: {ring depth it ran, warps per CTA, CTAs, dynamic shared memory per CTA (bytes),
     // result-heap entries held in global scratch (0 while every heap fitted in shared memory)}
     void launch_info(uint64_t* out) const;
+    // the plan a search (efS, topk) on this index will run with (sparse: for the longest query rows a batch can stage);
+    // host-only, so callers can refuse a search that does not fit before making it
+    HnswPlan search_plan(uint32_t efS, uint32_t topk) const;
 
 private:
     // selects the device, checks x against the index and uploads it into `into`, unless there is nothing to search (no rows
@@ -138,7 +157,7 @@ private:
     bool upload_(const HostMatrix& x, uint32_t topk, DeviceQueries& into);
     // the launch geometry follows the staging capacity qcap of the queries searched
     void ensure_scratch_(uint32_t ef, uint32_t qcap);
-    uint32_t per_warp_smem_(uint32_t ef, int stages, uint32_t qcap, uint32_t* nbmax_out) const;
+    HnswPlan plan_(uint32_t ef, uint32_t qcap) const;
     struct SearchIo {  // the first nq rows of *queries, searched into idx / val ([nq][topk])
         const DeviceQueries* queries;
         uint32_t nq;
@@ -162,7 +181,7 @@ private:
 
     // per-warp scratch
     uint32_t n_warps_ = 0, warps_per_cta_ = 0, n_ctas_ = 0;
-    int run_stages_ = 0;  // ring depth of the current launch geometry: stages_, or shallower where stages_ does not fit
+    HnswPlan run_plan_{};  // plan of the current launch geometry (ensure_scratch_): its ring depth is stages_ or shallower
     uint32_t last_ctas_ = 0, last_smem_ = 0;
     uint32_t vcap_ = 0;
     uint32_t vcap_floor_ = 0;    // minimum candidate-queue capacity (doubled after an overflow)

@@ -10,8 +10,9 @@ Two layouts for XR-Linear (SURVEY.md section 8e):
   those lists and a merge kernel give the global top-k, bit-identical to the single-GPU result.
 
 HNSW index sharding (:class:`ShardedHNSW`): one independent graph per contiguous row range, each rank searches its own shard
-and keeps its top-k as ``(key, global id, distance)`` with ``key = (~orderable(distance) << 32) | ~(rank * topk + slot)``; the
-same ONE all-gather and merge kernel give the top-k of the union, bit-identical to merging the per-shard searches.
+and keeps its top-k as ``(key, global id, distance)`` with ``key = (~orderable(distance) << 32) | ~(rank * topk + slot)`` (one
+fixed orderable for every NaN, after +inf); the same ONE all-gather and merge kernel give the top-k of the union, bit-identical
+to merging the per-shard searches.
 
 The reference has no inference-time model sharding (its parallelism is OpenMP threads inside one call,
 pecos/core/xmc/inference.hpp:969-1005); this module is the multi-GPU counterpart of that loop.
@@ -146,8 +147,10 @@ class ShardedHNSW(object):
     same result on every rank.
 
     The result is NOT the search of one graph over all rows (each shard is its own graph: recall level against it); it is,
-    bit for bit, the merge of the per-shard searches ordered by (distance, shard rank, slot within the shard), with global
-    ids ``row_begin[r] + local id``.  At world 1 it is the unsharded search."""
+    bit for bit, the merge of the per-shard searches ordered by (distance with NaN last, shard rank, slot within the shard),
+    with global ids ``row_begin[r] + local id``.  At world 1 this is the unsharded search when no NaN is returned; otherwise
+    it is the unsharded search's entries ordered by (distance with NaN last, position): a NaN in the search heaps can leave
+    the unsharded result out of order, and the merge sorts it."""
 
     MERGE_CAPACITY = MERGE_CAPACITY
 
@@ -203,6 +206,8 @@ class ShardedHNSW(object):
         n, k = int(view.rows), int(params.topk)
         if self.world * k > self.MERGE_CAPACITY:
             raise ValueError(f"world * topk = {self.world * k} exceeds the merge capacity of {self.MERGE_CAPACITY} records per query")
+        if n and k:  # every shard has the manifest's width and the same M, so every rank decides alike, before the exchange
+            self.index.check_search(params.efS, k)
         idx = np.zeros((n, k), dtype=np.uint32)
         dist = np.zeros((n, k), dtype=np.float32)
         if n and k:

@@ -115,6 +115,11 @@ class HNSW(object):
         return HNSW.Searchers(self, num_searcher)
 
     # ------------------------------------------------------------------ search
+    def check_search(self, efS, topk):
+        """Raises ValueError unless a search (efS, topk) fits one warp's shared memory: dense rows wider than about 51,000
+        components do not (pecos_b200.h, pb200_hnsw_search_fits).  Host-only."""
+        get_clib().hnsw_check_search(self.model_ptr, self.feat_dim, int(efS), int(topk))
+
     @staticmethod
     def create_pymat(X):
         """Query matrix -> (ctypes view, kind): dense float32 row-major, or csr float32 with ascending column indices."""
@@ -140,6 +145,8 @@ class HNSW(object):
         if view.cols != self.feat_dim:
             raise ValueError(f"query dimension {view.cols} != index dimension {self.feat_dim}")
         n, k = int(view.rows), int(params.topk)
+        if n and k:
+            self.check_search(params.efS, k)
         # the native call only fills the slots it found neighbours for; the rest must read as zeros (reference contract)
         idx = np.zeros((n, k), dtype=np.uint32)
         dist = np.zeros((n, k), dtype=np.float32)

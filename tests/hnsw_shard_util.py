@@ -31,9 +31,11 @@ def hnsw_result_counts(idx, dist):
 
 def hnsw_shard_records(idx, dist, cnt, rank, id_offset, topk):
     """One shard's exchange records (test-only restatement of hnsw_shard_pack_kernel): (keys u64, global ids, distances)
-    rows x topk, key = (~orderable(dist) << 32) | ~(rank * topk + slot), 0 for the slots at or beyond cnt."""
+    rows x topk, key = (~orderable(dist) << 32) | ~(rank * topk + slot), 0 for the slots at or beyond cnt; every NaN, whatever
+    its sign and payload, has orderable 0xFFFFFFFF (after +inf)."""
     u = np.asarray(dist, dtype=np.float32).view(np.uint32).astype(np.uint64)
     order = np.where(u & np.uint64(0x80000000), ~u & np.uint64(0xFFFFFFFF), u | np.uint64(0x80000000))
+    order = np.where(np.isnan(np.asarray(dist, dtype=np.float32)), np.uint64(0xFFFFFFFF), order)
     low = ~(np.uint64(rank * topk) + np.arange(topk, dtype=np.uint64)) & np.uint64(0xFFFFFFFF)
     keys = ((~order & np.uint64(0xFFFFFFFF)) << np.uint64(32)) | low[None, :]
     valid = np.arange(topk)[None, :] < np.asarray(cnt)[:, None]
@@ -44,7 +46,7 @@ def hnsw_shard_records(idx, dist, cnt, rank, id_offset, topk):
 
 def merge_hnsw_shards_numpy(idx, dist, row_begin, topk):
     """Reference semantics of the HNSW shard merge (test-only): per-shard search results idx / dist [world][rows][topk]
-    (local ids, zero-filled tails) -> the topk best of their union by (distance, shard rank, slot), global ids
+    (local ids, zero-filled tails) -> the topk best of their union by (distance with NaN last, shard rank, slot), global ids
     row_begin[r] + local id, zero-filled tails.  Returns (ids, distances), rows x topk."""
     world = idx.shape[0]
     recs = [hnsw_shard_records(idx[r], dist[r], hnsw_result_counts(idx[r], dist[r]), r, row_begin[r], topk) for r in range(world)]

@@ -225,3 +225,62 @@ def test_sparse_query_staging_limits(tmp_path, gpu_clib, have_ref):
     assert sorted(np.diff(Q.indptr))[-3:] == [4096, 4097, 20000]
     for efS, topk in [(64, 10), (600, 100)]:
         ix.check(Q, efS, topk, "csr staging")
+
+
+# (M, widest d that fits, first d that does not): for a width that is not a multiple of 16 and for one that is.  The limit is
+# 4 * dense_vstride(d) + 8 * nbmax <= 204,800 bytes (depth 0, the result heap in global memory), whatever ef.
+WIDEST = [(16, 51087, 51089), (16, 51136, 51152), (48, 50959, 50961), (48, 51008, 51024)]
+
+
+@pytest.mark.parametrize("M,d_fit,d_over", WIDEST)
+def test_widest_dense_rows_search_and_one_more_raises(tmp_path, gpu_clib, have_ref, M, d_fit, d_over):
+    """The widest rows run depth 0 with the result heap in global memory where the slice needs it (every ef), equal to the
+    restatement; one more 16-block makes predict raise ValueError before any native call, and the process lives on."""
+    from pecos_b200.hnsw import HNSW
+
+    from .test_hnsw_nonfinite_cpu import dense_plan_rule
+
+    rng = np.random.default_rng(d_fit)
+    X = _unit(rng, 40, d_fit)
+    ix = _Index(str(tmp_path / "fit"), X, M, "ip", have_ref, efC=20)
+    Q = _with_special_rows(_unit(rng, 5, d_fit), X)
+    for efS, topk in [(10, 10), (100, 10), (512, 10), (513, 10)]:
+        ix.check(Q, efS, topk, f"d={d_fit} M={M}")
+        fits, plan = gpu_clib.hnsw_search_fits(ix.m.model_ptr, efS, topk)
+        want = dense_plan_rule(d_fit, 2 * M, 4, max(efS, topk))
+        assert fits and want[0] and (plan["stages"], bool(plan["heap_in_smem"]), plan["per_warp_bytes"]) == want[1:]
+        info = _launch_info(ix.m)
+        assert info["stages"] == 0 and info["smem"] == info["warps"] * plan["per_warp_bytes"], (efS, info, plan)
+        assert plan["heap_in_smem"] or info["heap"] >= max(efS, topk) + 1
+    assert not gpu_clib.hnsw_search_fits(ix.m.model_ptr, 512, 10)[1]["heap_in_smem"]
+    Xo = _unit(rng, 40, d_over)
+    save_hnsw_index(str(tmp_path / "over"), Xo, M, 20, "ip", have_ref)
+    wide = HNSW.load(str(tmp_path / "over"))  # loading and creating searchers stay allowed, as in the reference
+    wide.searchers_create(2)
+    launches = (c_uint64 * 8)()
+    gpu_clib.clib_float32.pb200_hnsw_get_info(wide.model_ptr, launches)
+    before = int(launches[7])
+    for efS in (10, 512, 513):
+        assert not gpu_clib.hnsw_search_fits(wide.model_ptr, efS, 10)[0]
+        with pytest.raises(ValueError, match="cannot be searched"):
+            wide.predict(_unit(rng, 3, d_over), pred_params=HNSW.PredParams(efS=efS, topk=10), ret_csr=False)
+    gpu_clib.clib_float32.pb200_hnsw_get_info(wide.model_ptr, launches)
+    assert int(launches[7]) == before
+    ix.check(Q, 64, 10, "after the refusal")
+
+
+def test_heap_leaves_shared_memory_below_ef_513(tmp_path, gpu_clib, have_ref):
+    """d = 50,500 with M = 16 fits depth 0 with the heap in shared memory at ef = 100 but not at ef = 512: the heap moves to
+    global memory there, on one handle, between calls."""
+    rng = np.random.default_rng(50500)
+    X = _unit(rng, 40, 50500)
+    ix = _Index(str(tmp_path / "i"), X, 16, "l2", have_ref, efC=20)
+    Q = _with_special_rows(_unit(rng, 5, 50500), X)
+    placed = {}
+    for efS in (100, 512, 100, 600):
+        ix.check(Q, efS, 10, f"ef={efS}")
+        fits, plan = gpu_clib.hnsw_search_fits(ix.m.model_ptr, efS, 10)
+        info = _launch_info(ix.m)
+        assert fits and info["stages"] == 0 and info["smem"] == info["warps"] * plan["per_warp_bytes"]
+        placed[efS] = plan["heap_in_smem"]
+    assert placed == {100: 1, 512: 0, 600: 0}

@@ -20,6 +20,7 @@ import pytest
 import scipy.sparse as smat
 
 from tests.test_pairwise_ann_gpu import _pp, _random_case
+from tests.util import assert_same_nan
 
 pytestmark = pytest.mark.gpu
 
@@ -34,17 +35,6 @@ LENS = [0, 1, 127, 128, 129, 255, 256, 257, 1023, 1024, 1025]
 
 
 # ------------------------------------------------------------------------------------------------------------- helpers
-def assert_same_nan(got, want, what=""):
-    """I, M, V bit-equal; D bit-equal except that two NaNs (of any payload) are equal."""
-    for tag, g, w in zip("IMDV", got, want):
-        g, w = np.asarray(g), np.asarray(w)
-        if tag == "D":
-            both = np.isnan(g) & np.isnan(w)
-            assert np.array_equal(np.where(both, 0, g.view(np.uint32)), np.where(both, 0, w.view(np.uint32))), f"D {what}"
-        else:
-            assert np.array_equal(g.view(np.uint32), w.view(np.uint32)), f"{tag} {what}"
-
-
 def dense_rule(d):
     """(fits, ring depth, per-warp bytes, row stride) of a dense model of width d, from the row layout of hnsw_host.h."""
     vstride = 64 * ((d // 16 + 3) // 4) + (16 if d % 16 else 0)

@@ -28,6 +28,18 @@ def assert_csr_parity(got, want, rtol=1e-5, what=""):
     return exact
 
 
+def assert_same_nan(got, want, what="", tags="IMDV"):
+    """Arrays tagged by `tags` (PairwiseANN: I, M, D, V; HNSW: I, D) bit-equal, except that in D two NaNs of any payload
+    are equal: the GPU returns 0x7FFFFFFF for every NaN, x86 the first NaN operand or 0xFFC00000."""
+    for tag, g, w in zip(tags, got, want):
+        g, w = np.asarray(g), np.asarray(w)
+        if tag == "D":
+            both = np.isnan(g) & np.isnan(w)
+            assert np.array_equal(np.where(both, 0, g.view(np.uint32)), np.where(both, 0, w.view(np.uint32))), f"D {what}"
+        else:
+            assert np.array_equal(g.view(np.uint32), w.view(np.uint32)), f"{tag} {what}"
+
+
 def random_tree(seed, layer_sizes, D, nnz_per_col, bias=1.0, permute=False, prune=0.0, saturate=False):
     """Random label tree; `permute` shuffles child->parent assignment (non-contiguous C), `prune` drops that fraction of
     rows from every non-root C (pruned tree, pecos set_output_constraint style), `saturate` scales weights up so that the
