@@ -95,9 +95,9 @@ __host__ __device__ inline size_t cm_warp_bytes(uint32_t acc_cols, uint32_t stag
 // col_cap: a chunk wider than col_cap columns is cut into ceil(n_cols / col_cap) column ranges of (nearly) equal width, each
 // with its OWN image (only its entries) -- a "virtual chunk"; a (query, chunk) pair is then scored once per range.  The lookups
 // are repeated for the cut chunks, the accumulate work is not, and both the image and the per-warp accumulators shrink to the
-// cap, so more warps fit.  The load path takes the largest cap that fits (see the policy note in xlinear_engine.cu): a layer
-// is only cut when its widest chunk does not fit next to kCmMinWarps warps.  e_max = most entries of one virtual chunk,
-// n_vc = number of virtual chunks.
+// cap, so more warps fit.  The load path takes the largest cap that fits (cm_layer_layout): a layer is only cut when its
+// widest chunk does not fit next to kCmMinWarps warps.  e_max = most entries of one virtual chunk, n_vc = number of virtual
+// chunks.
 inline CmShape cm_shape(uint32_t fm_words, uint32_t w_rows, uint32_t r_max, uint32_t e_max, uint32_t col_cap, uint32_t n_chunks,
                         uint32_t n_vc) {
     CmShape s;
@@ -123,6 +123,66 @@ inline CmShape cm_shape(uint32_t fm_words, uint32_t w_rows, uint32_t r_max, uint
     s.warps_fit = static_cast<uint32_t>(std::min<size_t>(kCmMaxWarps, (kCmSmemBudget - s.img_bytes - 64) / cm_warp_bytes(s.acc_cols, s.stages)));
     s.ok = true;
     return s;
+}
+
+// The chunk images a layer with a feature map gets at load time: their shape (vc_ptr unset; ok == false: none fits) and the
+// host table of the first virtual chunk of every chunk, [n_chunks + 1] (empty when !shape.ok).
+struct CmLayout { CmShape shape; std::vector<uint32_t> vc_ptr; };
+
+// Policy: the LARGEST column cap that fits at all (no cut whenever the layer fits uncut), down in steps of 7/8 until the
+// cut would more than quadruple the layer's chunks (kCmMaxDup) or the cap drops below 8.  Cutting gives more warps per CTA,
+// but every cut repeats the pair's lookups.  Measured on an H100 80GB HBM3 at 400 W (eurlex-4k leaf, chunks of 46 - 84
+// columns, work-weighted CTA shares): uncut, 6 warps, 0.82 ms; cap 42, 15 warps, 1.08 ms; cap 28, 16 warps, 1.07 ms -- the
+// kernel is bound by the shared-memory accesses of lookups and entries, not by its warps.
+inline CmLayout cm_layer_layout(const ChunkedLayerHost& L) {
+    // virtual chunks under column cap `cap`; on request the vc_ptr table and the most entries of one column range
+    auto layout_for_cap = [&L](uint32_t cap, std::vector<uint32_t>* vc_ptr_out, uint32_t* e_max_out) {
+        uint32_t n_vc = 0, best = 0;
+        std::vector<uint32_t> cnt;
+        if (vc_ptr_out) vc_ptr_out->assign(static_cast<size_t>(L.n_chunks) + 1, 0u);
+        for (uint32_t p = 0; p < L.n_chunks; ++p) {
+            const ChunkHeader& ch = L.chunks[p];
+            if (vc_ptr_out) (*vc_ptr_out)[p] = n_vc;
+            if ((ch.has_bias & kChunkAbsent) || ch.n_cols == 0) continue;
+            const uint32_t nr = (ch.n_cols + cap - 1) / cap;
+            n_vc += nr;
+            if (!e_max_out || ch.nnz_rows == 0) continue;
+            const uint32_t* rp = L.meta.data() + ch.meta_off + round_up4(ch.nnz_rows);
+            if (nr == 1) { best = std::max(best, rp[ch.nnz_rows]); continue; }  // an uncut chunk: all its entries
+            const uint32_t width = (ch.n_cols + nr - 1) / nr;
+            cnt.assign(nr, 0u);
+            const ChunkEntry* en = L.entries.data() + ch.ent_off;
+            for (uint32_t i = 0; i < rp[ch.nnz_rows]; ++i) ++cnt[std::min(en[i].col_offset / width, nr - 1)];
+            for (uint32_t v : cnt) best = std::max(best, v);
+        }
+        if (vc_ptr_out) (*vc_ptr_out)[L.n_chunks] = n_vc;
+        if (e_max_out) *e_max_out = best;
+        return n_vc;
+    };
+    const uint32_t fm_words = static_cast<uint32_t>((static_cast<uint64_t>(L.w_rows) + 31) / 32);
+    CmLayout out;
+    const uint32_t n_real = layout_for_cap(std::max<uint32_t>(L.c_max, 1u), nullptr, nullptr);
+    for (uint32_t cap = std::max<uint32_t>(L.c_max, 1u); n_real > 0; cap = cap * 7 / 8) {
+        uint32_t e_cap = 0;
+        const uint32_t n_vc = layout_for_cap(cap, nullptr, &e_cap);
+        if (static_cast<uint64_t>(n_vc) * 100u > static_cast<uint64_t>(n_real) * kCmMaxDup) break;
+        const CmShape cand = cm_shape(fm_words, L.w_rows, L.r_max, e_cap, cap, L.n_chunks, n_vc);
+        if (cand.ok) { out.shape = cand; break; }
+        if (cap < 8u) break;
+    }
+    if (out.shape.ok) layout_for_cap(out.shape.col_cap, &out.vc_ptr, nullptr);
+    return out;
+}
+
+// Whether layers 0 and 1 have the structure the prefix launch needs (their merged layer is build_prefix_layer's): layer 0 is
+// one chunk of 1 .. kCmPrefixTop0 columns, each the parent of one layer-1 chunk; neither layer is rearranged or index-sharded;
+// both share a feature space small enough for a direct table and the bias; the merged chunk has at most 256 columns.
+inline bool prefix_mergeable(const ChunkedLayerHost& H0, const ChunkedLayerHost& H1) {
+    const auto absent = [](const ChunkHeader& ch) { return (ch.has_bias & kChunkAbsent) != 0; };
+    return H0.n_chunks == 1 && H0.n_cols >= 1 && H0.n_cols <= kCmPrefixTop0 && H1.n_chunks == H0.n_cols && !H0.reordered &&
+           !H1.reordered && H0.w_rows == H1.w_rows && H0.w_rows <= kCmDirectRows &&
+           std::memcmp(&H0.bias, &H1.bias, sizeof(float)) == 0 && H0.n_cols + H1.n_cols <= 256u &&
+           std::none_of(H0.chunks.begin(), H0.chunks.end(), absent) && std::none_of(H1.chunks.begin(), H1.chunks.end(), absent);
 }
 
 // force: take the kernel wherever the layer has images, ignoring the reuse / occupancy heuristics (kernel mode 5, tests)

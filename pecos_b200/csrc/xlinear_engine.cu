@@ -950,13 +950,8 @@ XLinearEngine::XLinearEngine(std::unique_ptr<XLinearHostModel> host, int device)
     for (size_t d = 0; d < layers_.size(); ++d) {
         auto& src = host_->layers[d];
         auto& dst = layers_[d];
-        dst.chunks.upload(src.chunks.data(), src.chunks.size(), stream_);
-        dst.meta.upload(src.meta.data(), src.meta.size(), stream_);
-        dst.entries.upload(reinterpret_cast<const uint2*>(src.entries.data()), src.entries.size(), stream_);
-        if (src.reordered) dst.label_of_col.upload(src.label_of_col.data(), src.label_of_col.size(), stream_);
+        upload_store_(src, dst);
         // query-driven lookup structure, unless it would blow the memory budget (then the kernel streams the row lists)
-        dst.view.featmap = nullptr;
-        dst.view.fm_words = 0;
         if (featmap_budget >= feature_map_bytes(src)) {
             featmap_budget -= feature_map_bytes(src);
             build_feature_map(src);
@@ -967,124 +962,34 @@ XLinearEngine::XLinearEngine(std::unique_ptr<XLinearHostModel> host, int device)
             model_bytes_ += src.featmap.size() * 8;
             std::vector<uint2_host>().swap(src.featmap);
         }
-        dst.e_max = 0;
-        for (const ChunkHeader& ch : src.chunks) {
-            if ((ch.has_bias & kChunkAbsent) || ch.nnz_rows == 0) continue;
-            const uint32_t* rp = src.meta.data() + ch.meta_off + round_up4(ch.nnz_rows);
-            dst.e_max = std::max(dst.e_max, rp[ch.nnz_rows]);
-        }
         dst.rowext.reserve(std::max<uint64_t>(src.meta.size(), 4));
         xl_build_rowext_kernel<<<n_sm_ * 8, 256, 0, stream_>>>(dst.chunks.get(), dst.meta.get(), dst.rowext.get(), src.n_chunks);
         PB200_CUDA(cudaGetLastError());
-        model_bytes_ += src.meta.size() * 4;
-        dst.view.chunks = dst.chunks.get();
-        dst.view.meta = dst.meta.get();
         dst.view.rowext = dst.rowext.get();
-        dst.view.entries = dst.entries.get();
-        dst.view.label_of_col = src.reordered ? dst.label_of_col.get() : nullptr;
-        dst.view.n_cols = src.n_cols;
-        dst.view.n_chunks = src.n_chunks;
-        dst.view.c_max = src.c_max;
-        dst.view.w_rows = src.w_rows;
-        dst.view.bias = src.bias;
-        // chunk images for the chunk-major score kernel (xlinear_cm_kernel.cuh), where the layer's shape allows it.  A column
-        // cap cuts the widest chunks of the layer into column ranges ("virtual chunks") when the layer does not fit uncut.
-        dst.cm_shape = CmShape{};
+        model_bytes_ += src.meta.size() * 4;
+        // chunk images for the chunk-major score kernel (xlinear_cm_kernel.cuh), where the layer's shape allows it
         if (dst.view.featmap) {
-            auto layout_for_cap = [&](uint32_t cap, std::vector<uint32_t>* vc_ptr_out, uint32_t* e_max_out) {
-                uint32_t n_vc = 0, best = 0;
-                std::vector<uint32_t> cnt;
-                if (vc_ptr_out) vc_ptr_out->assign(static_cast<size_t>(src.n_chunks) + 1, 0u);
-                for (uint32_t p = 0; p < src.n_chunks; ++p) {
-                    const ChunkHeader& ch = src.chunks[p];
-                    if (vc_ptr_out) (*vc_ptr_out)[p] = n_vc;
-                    if ((ch.has_bias & kChunkAbsent) || ch.n_cols == 0) continue;
-                    const uint32_t nr = (ch.n_cols + cap - 1) / cap;
-                    n_vc += nr;
-                    if (!e_max_out || ch.nnz_rows == 0) continue;
-                    const uint32_t* rp = src.meta.data() + ch.meta_off + round_up4(ch.nnz_rows);
-                    const uint32_t width = (ch.n_cols + nr - 1) / nr;
-                    cnt.assign(nr, 0u);
-                    const ChunkEntry* en = src.entries.data() + ch.ent_off;
-                    for (uint32_t i = 0; i < rp[ch.nnz_rows]; ++i) ++cnt[std::min(en[i].col_offset / width, nr - 1)];
-                    for (uint32_t v : cnt) best = std::max(best, v);
-                }
-                if (vc_ptr_out) (*vc_ptr_out)[src.n_chunks] = n_vc;
-                if (e_max_out) *e_max_out = best;
-                return n_vc;
-            };
-            // Policy: the LARGEST cap that fits at all (no cut whenever the layer fits uncut).  Cutting gives more warps per
-            // CTA, but every cut repeats the pair's lookups.  Measured on an H100 80GB HBM3 at 400 W (eurlex-4k leaf, chunks
-            // of 46 - 84 columns, work-weighted CTA shares): uncut, 6 warps, 0.82 ms; cap 42, 15 warps, 1.08 ms; cap 28,
-            // 16 warps, 1.07 ms -- the kernel is bound by the shared-memory accesses of lookups and entries, not by its warps.
-            CmShape shape;
-            const uint32_t n_real = layout_for_cap(std::max<uint32_t>(src.c_max, 1u), nullptr, nullptr);
-            for (uint32_t cap = std::max<uint32_t>(src.c_max, 1u); n_real > 0; cap = cap * 7 / 8) {
-                const uint32_t n_vc = layout_for_cap(cap, nullptr, nullptr);
-                if (static_cast<uint64_t>(n_vc) * 100u > static_cast<uint64_t>(n_real) * kCmMaxDup) break;
-                uint32_t e_cap = dst.e_max;
-                if (cap < src.c_max) layout_for_cap(cap, nullptr, &e_cap);
-                const CmShape cand = cm_shape(src.fm_words, src.w_rows, src.r_max, e_cap, cap, src.n_chunks, n_vc);
-                if (cand.ok) { shape = cand; break; }
-                if (cap < 8u) break;
-            }
-            const uint64_t bytes = static_cast<uint64_t>(shape.img_bytes) * shape.n_vc;
-            if (shape.ok && bytes <= cmimg_budget) {
+            const CmLayout cm = cm_layer_layout(src);
+            const uint64_t bytes = static_cast<uint64_t>(cm.shape.img_bytes) * cm.shape.n_vc;
+            if (cm.shape.ok && bytes <= cmimg_budget) {
                 cmimg_budget -= bytes;
-                std::vector<uint32_t> vc_ptr;
-                layout_for_cap(shape.col_cap, &vc_ptr, nullptr);
-                dst.cm_vc_ptr.upload(vc_ptr.data(), vc_ptr.size(), stream_);
-                PB200_CUDA(cudaStreamSynchronize(stream_));
-                shape.vc_ptr = dst.cm_vc_ptr.get();
-                dst.cm_shape = shape;
-                dst.cm_images.reserve(std::max<uint64_t>(bytes, 1));
-                xl_cm_build_images_kernel<<<shape.n_vc, 256, 0, stream_>>>(dst.view, shape, dst.cm_images.get());
-                PB200_CUDA(cudaGetLastError());
-                model_bytes_ += bytes;
+                place_images_(dst, cm.shape, cm.vc_ptr);
             }
         }
-        model_bytes_ += src.chunks.size() * sizeof(ChunkHeader) + src.meta.size() * 4 + src.entries.size() * 8 +
-                        src.label_of_col.size() * 4;
     }
-    // The prefix image: layers 0 and 1 merged into one chunk (build_prefix_layer) when layer 0 is one narrow chunk, neither
-    // layer is rearranged or index-sharded, both share features and bias, and the merged chunk fits a direct-table image.
-    if (layers_.size() >= 2 && layers_[0].view.featmap && layers_[1].view.featmap) {
-        const ChunkedLayerHost& H0 = host_->layers[0];
-        const ChunkedLayerHost& H1 = host_->layers[1];
-        bool ok = H0.n_chunks == 1 && H0.n_cols >= 1 && H0.n_cols <= kCmPrefixTop0 && H1.n_chunks == H0.n_cols &&
-                  !H0.reordered && !H1.reordered && H0.w_rows == H1.w_rows && H0.w_rows <= kCmDirectRows &&
-                  std::memcmp(&H0.bias, &H1.bias, sizeof(float)) == 0 && H0.n_cols + H1.n_cols <= 256u;
-        for (const ChunkHeader& ch : H0.chunks) ok = ok && !(ch.has_bias & kChunkAbsent);
-        for (const ChunkHeader& ch : H1.chunks) ok = ok && !(ch.has_bias & kChunkAbsent);
-        if (ok) {
-            ChunkedLayerHost M;
-            build_prefix_layer(H0, H1, M);
-            const uint32_t fm_words = static_cast<uint32_t>((static_cast<uint64_t>(M.w_rows) + 31) / 32);
-            const uint64_t n_ent = M.entries.size();
-            CmShape shape = n_ent < 65535u ? cm_shape(fm_words, M.w_rows, M.r_max, static_cast<uint32_t>(n_ent), M.c_max, 1, 1) : CmShape{};
-            if (shape.ok && shape.direct && shape.img_bytes <= cmimg_budget) {
-                LayerStore& P = prefix_;
-                P.chunks.upload(M.chunks.data(), M.chunks.size(), stream_);
-                P.meta.upload(M.meta.data(), M.meta.size(), stream_);
-                P.entries.upload(reinterpret_cast<const uint2*>(M.entries.data()), M.entries.size(), stream_);
-                const uint32_t vc_ptr[2] = {0u, 1u};
-                P.cm_vc_ptr.upload(vc_ptr, 2, stream_);
-                P.view.chunks = P.chunks.get();
-                P.view.meta = P.meta.get();
-                P.view.entries = P.entries.get();
-                P.view.n_cols = M.n_cols;
-                P.view.n_chunks = 1;
-                P.view.c_max = M.c_max;
-                P.view.w_rows = M.w_rows;
-                P.view.bias = M.bias;
-                shape.vc_ptr = P.cm_vc_ptr.get();
-                P.cm_shape = shape;
-                P.cm_images.reserve(shape.img_bytes);
-                xl_cm_build_images_kernel<<<1, 256, 0, stream_>>>(P.view, shape, P.cm_images.get());
-                PB200_CUDA(cudaGetLastError());
-                PB200_CUDA(cudaStreamSynchronize(stream_));  // M's host arrays go out of scope
-                model_bytes_ += shape.img_bytes + M.chunks.size() * sizeof(ChunkHeader) + M.meta.size() * 4 + M.entries.size() * 8 + 8;
-            }
+    // The prefix image: layers 0 and 1 merged into one chunk (build_prefix_layer) whose image has a direct table.
+    if (layers_.size() >= 2 && layers_[0].view.featmap && layers_[1].view.featmap &&
+        prefix_mergeable(host_->layers[0], host_->layers[1])) {
+        ChunkedLayerHost M;
+        build_prefix_layer(host_->layers[0], host_->layers[1], M);
+        const uint32_t fm_words = static_cast<uint32_t>((static_cast<uint64_t>(M.w_rows) + 31) / 32);
+        const uint64_t n_ent = M.entries.size();
+        const CmShape shape = n_ent < 65535u ? cm_shape(fm_words, M.w_rows, M.r_max, static_cast<uint32_t>(n_ent), M.c_max, 1, 1) : CmShape{};
+        if (shape.ok && shape.direct && shape.img_bytes <= cmimg_budget) {
+            upload_store_(M, prefix_);
+            place_images_(prefix_, shape, {0u, 1u});
+            model_bytes_ += 2 * sizeof(uint32_t);  // model_bytes() counts the prefix's virtual-chunk table, not the layers'
+            PB200_CUDA(cudaStreamSynchronize(stream_));  // M's host arrays go out of scope
         }
     }
     PB200_CUDA(cudaStreamSynchronize(stream_));
@@ -1117,6 +1022,35 @@ XLinearEngine::XLinearEngine(std::unique_ptr<XLinearHostModel> host, int device)
     layer_stats_.assign(layers_.size(), XLinearStats{});
 }
 
+void XLinearEngine::upload_store_(const ChunkedLayerHost& H, LayerStore& S) {
+    S.chunks.upload(H.chunks.data(), H.chunks.size(), stream_);
+    S.meta.upload(H.meta.data(), H.meta.size(), stream_);
+    S.entries.upload(reinterpret_cast<const uint2*>(H.entries.data()), H.entries.size(), stream_);
+    if (H.reordered) S.label_of_col.upload(H.label_of_col.data(), H.label_of_col.size(), stream_);
+    S.view.chunks = S.chunks.get();
+    S.view.meta = S.meta.get();
+    S.view.entries = S.entries.get();
+    S.view.label_of_col = H.reordered ? S.label_of_col.get() : nullptr;
+    S.view.n_cols = H.n_cols;
+    S.view.n_chunks = H.n_chunks;
+    S.view.c_max = H.c_max;
+    S.view.w_rows = H.w_rows;
+    S.view.bias = H.bias;
+    model_bytes_ += H.chunks.size() * sizeof(ChunkHeader) + H.meta.size() * 4 + H.entries.size() * 8 + H.label_of_col.size() * 4;
+}
+
+void XLinearEngine::place_images_(LayerStore& S, CmShape shape, const std::vector<uint32_t>& vc_ptr) {
+    S.cm_vc_ptr.upload(vc_ptr.data(), vc_ptr.size(), stream_);
+    PB200_CUDA(cudaStreamSynchronize(stream_));  // the host table may go out of scope
+    shape.vc_ptr = S.cm_vc_ptr.get();
+    const uint64_t bytes = static_cast<uint64_t>(shape.img_bytes) * shape.n_vc;
+    S.cm_images.reserve(bytes);
+    xl_cm_build_images_kernel<<<shape.n_vc, 256, 0, stream_>>>(S.view, shape, S.cm_images.get());
+    PB200_CUDA(cudaGetLastError());
+    S.cm_shape = shape;
+    model_bytes_ += bytes;
+}
+
 XLinearEngine::~XLinearEngine() {
     cudaSetDevice(device_);
     if (stream_) cudaStreamSynchronize(stream_);
@@ -1128,7 +1062,7 @@ XLinearEngine::~XLinearEngine() {
 }
 
 bool XLinearEngine::has_feature_maps() const {
-    for (auto& l : layers_) if (!l.featmap.capacity()) return false;
+    for (auto& l : layers_) if (!l.view.featmap) return false;
     return true;
 }
 
@@ -1251,9 +1185,9 @@ XLinearEngine::LayerKernels XLinearEngine::pick_kernels_(size_t d, const QueryDe
     const bool fills_gpu = force_cm || q.rows >= kCmMinPairsPerSm * n_sm_;
     k.prefix = d < 2 && root_tile && prefix_mode && prefix_.cm_shape.ok && sparse && keeps_layer0 && cm_offsets_fit && fills_gpu;
 
-    const bool lookup = sparse && !first_gen && S.featmap.capacity() != 0;  // mode 0: as if no layer had a feature map
+    const bool lookup = sparse && !first_gen && S.view.featmap;  // mode 0: as if no layer had a feature map
     // the statistics pass runs the query-major kernels: their counters are the canonical ones
-    if (!k.prefix && lookup && !t.collect_stats && cm_offsets_fit && chunk_major_workspace_() && S.cm_images.capacity())
+    if (!k.prefix && lookup && !t.collect_stats && cm_offsets_fit && chunk_major_workspace_())
         k.cm = cm_plan(S.cm_shape, S.view.n_chunks, static_cast<uint64_t>(q.rows) * lp.b_prev, n_sm_, force_cm);
     // One warp per query over the whole beam (feature-major) wins when the beam consists of MANY NARROW chunks (per-chunk
     // bookkeeping dominates: S layers 1-4, 20 x 8 columns), and loses on wide chunks where one warp per chunk keeps more

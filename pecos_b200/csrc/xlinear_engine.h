@@ -182,12 +182,15 @@ private:
         DeviceBuffer<uint2> entries;
         DeviceBuffer<uint32_t> label_of_col;
         DeviceBuffer<uint2> featmap;
-        uint32_t e_max = 0;  // most entries of one chunk (sizes the chunk-major kernel's shared-memory staging)
-        DeviceBuffer<unsigned char> cm_images;  // packed chunk images of the chunk-major kernel (empty: layer not eligible)
+        DeviceBuffer<unsigned char> cm_images;  // packed chunk images of the chunk-major kernel
         DeviceBuffer<uint32_t> cm_vc_ptr;
-        CmShape cm_shape;
-        LayerDev view{};
+        CmShape cm_shape;  // ok: the store has chunk images
+        LayerDev view{};   // view.featmap != nullptr: the store has a feature map
     };
+    // Uploads H's chunks, meta, entries and (when reordered) label_of_col into S, sets S.view from H and counts the bytes.
+    void upload_store_(const ChunkedLayerHost& H, LayerStore& S);
+    // Builds S's chunk images of the given shape from its view (vc_ptr: the host table of cm_layer_layout) and counts them.
+    void place_images_(LayerStore& S, CmShape shape, const std::vector<uint32_t>& vc_ptr);
 
     // Where the last layer of a tile writes its top-k: rows [0, tile) of these arrays (keys only in an index-sharded run).
     struct OutTarget {
@@ -304,7 +307,7 @@ private:
     bool profile_ = false;
     KernelMode mode_ = KernelMode::kDefault;
     // Merged one-chunk layer of layers 0 and 1 (build_prefix_layer) and its chunk-major image: scores both layers of a tile
-    // in one launch (prefix_.cm_images empty: the model is not eligible)
+    // in one launch (prefix_.cm_shape.ok == false: the model is not eligible)
     LayerStore prefix_;
     // Layer 0's beam into beam_*_[1] and layer 1's raw scores into its candidate rows, for rows [ws_row, ws_row + q.rows).
     void launch_prefix_(const QueryDev& q, const std::vector<LayerPlan>& plan, uint32_t ws_row);
